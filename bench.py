@@ -3,6 +3,7 @@
 frame's FPN features -> 200x200x16 semantic + flow volume).
 
     python bench.py --gpus N --steps K --warmup W            # this repo (CUDA path through the C ABI)
+    python bench.py --steps K --dump-outputs DIR             # + the last timed step's outputs as DIR/<name>.npy
     python bench.py --impl reference --steps K --warmup W    # the reference's CPU path (oracle restatement) on host cores
 
 Workload (config.workload): BASELINE configs[3] on top of configs[1]/[2] -- 6 x (928x1600-padded) cameras, FPN levels
@@ -11,8 +12,13 @@ Workload (config.workload): BASELINE configs[3] on top of configs[1]/[2] -- 6 x 
 random-init weights (fixtures.py).  One step = --frames-per-step (32) frames.  Frames are independent: N GPUs run N frame
 streams (weak scaling) and the only collective is the final all-reduce of the 187 metric counters.
 
-Timing: W >= 3 warm-up steps; K steps bracketed by barrier + cuda synchronize; device time from CUDA events on the
-launch stream, max over ranks.  Each step reads a different 189 MB input frame (3 rotating frames > 126 MB L2).
+Timing: W warm-up steps and >= 1 s of untimed steps; then --repeats regions (default 1) of exactly K steps, each bracketed
+by barrier + cuda synchronize; device time from CUDA events on the launch stream, max over ranks.  The frames rotate over 3
+different 95 MB (bf16) input frames, together larger than the 50 MB L2.
+
+--dump-outputs DIR: after the timed steps, the results the timed path returned for the frames of its last step (occ_cls,
+flow) at a fixed, seeded sample of voxels, as float32 .npy files (voxel_index.npy: the flat voxel indices of the sample,
+float64).  The inputs are a function of the seeds only, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -40,11 +46,12 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d['hbm_gbs'], tf_burst=d['bf16_tflops'], tf_sust=d.get('bf16_tflops_sustained', d['bf16_tflops']),
                     source='measured')
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, source='fallback')
+    # NVIDIA H100 SXM data sheet (700 W part): 3.35 TB/s HBM3, 989 dense bf16 TFLOP/s -- upper bounds, not reached
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, source='H100 SXM data sheet')
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
          'clocks_event_reasons.sw_power_cap')
@@ -219,7 +226,7 @@ def run_ours(args):
     _, vis_mask = eng.project_pillars()
     n_hit = int(vis_mask.any(dim=2).sum().item())                   # visible (camera, pillar) pairs = SCA work items
     NF, F, K = 3, args.frames_per_step, args.steps
-    W = max(args.warmup, 3)
+    W = args.warmup
     feat_dtype = torch.bfloat16 if args.precision == 'bf16' else torch.float32     # features in the storage precision
     frames_f32 = [[f[0].contiguous() for f in fixtures.make_feats(cfg, bs=1, seed=100 + rank * NF + i)] for i in range(NF)]
     frames_host = [[f.to(feat_dtype).contiguous().pin_memory() for f in fr] for fr in frames_f32]
@@ -232,12 +239,18 @@ def run_ours(args):
             dist.barrier()
         torch.cuda.synchronize()
 
+    last_step = []                                                  # what the last step of a call returned, frame by frame
+
     def run_steps(n):                                               # one step = F frames through the engine
+        last_step.clear()
         for i in range(n * F):
-            eng.forward(frames_dev[i % NF], want=want)
+            out = eng.forward(frames_dev[i % NF], want=want)
+            if i >= (n - 1) * F:
+                last_step.append(out)
 
     # ---- device-resident throughput (`value`): >= 1 s of warm-up, then `repeats` regions of EXACTLY K steps, median
-    run_steps(W)
+    if W > 0:
+        run_steps(W)
     barrier()
     t0 = time.perf_counter()
     while time.perf_counter() - t0 < 1.0:
@@ -248,6 +261,9 @@ def run_ours(args):
         sampler.start()
     reps = [occdist.max_over_ranks(timed_region(run_steps, K, barrier), dev) for _ in range(args.repeats)]
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_step)
+    last_step.clear()
     ms_med = float(np.median(reps))
     launches = eng.launches_per_frame
 
@@ -333,13 +349,6 @@ def run_ours(args):
     work = algorithmic_work(cfg, s, tc=use_tc, feat_bytes=frames_host[0][0].element_size())
     total_prof = sum(v[0] for v in prof.values()) or 1.0
     share = {k: round(v[0] / total_prof, 4) for k, v in prof.items()}
-    traffic = {}
-    for tname in ('r2_traffic.json', 'r1_traffic.json'):            # dram bytes from the committed ncu --set full captures
-        tpath = os.path.join(ROOT, 'profiles', tname)
-        if os.path.exists(tpath):
-            traffic = json.load(open(tpath))
-            traffic['_source'] = 'profiles/' + tname + ' (ncu --set full capture of this build; not measured in this run)'
-            break
     L = cfg['num_layers']
     per_frame_bytes = {'sca_gather': work['sca_bytes_per_launch'] * L, 'tsa_gather': work['tsa_bytes_per_launch'] * L,
                        'gemm': work['gemm_bytes'], 'pack': work['pack_bytes'], 'conv3d': work['conv_bytes'],
@@ -354,14 +363,14 @@ def run_ours(args):
         ach = nbytes / (per_frame_ms * 1e-3) / 1e9
         rooflines[k] = dict(bound='hbm', achieved=round(ach, 1), peak=pk['hbm'], unit='GB/s', frac=round(ach / pk['hbm'], 4),
                             algorithmic_bytes_per_frame=int(nbytes), launches_per_frame=n_k // prof_frames,
-                            ms_per_frame=round(per_frame_ms, 4), traffic=traffic.get(k))
+                            ms_per_frame=round(per_frame_ms, 4))
         if k in per_frame_flops:                                    # SURVEY 8(d): dense contractions are tensor-class
             tf = per_frame_flops[k] / (per_frame_ms * 1e-3) / 1e12
             rooflines[k].update(tensor_tflops=round(tf, 1), tensor_frac=round(tf / pk['tf_sust'], 4),
                                 tensor_peak=pk['tf_sust'], algorithmic_flops_per_frame=int(per_frame_flops[k]))
     # The two gather kernels are bound by the L1 data path, not by HBM: report the bytes the bilinear gathers pull
     # through L1 next to the HBM roofline.
-    sm_clk = (clocks or {}).get('sm_mhz') or 1965.0
+    sm_clk = (clocks or {}).get('sm_mhz') or torch.cuda.get_device_properties(dev).clock_rate / 1e3
     nsm = torch.cuda.get_device_properties(dev).multi_processor_count
     for k, nbytes_l1 in (('sca_gather', n_hit * 32 * 8 * 4 * 32 * s * L),
                          ('tsa_gather', work['Nq'] * 8 * 8 * 4 * 32 * s * L)):
@@ -374,23 +383,21 @@ def run_ours(args):
     dom = max(rooflines, key=lambda k: rooflines[k]['ms_per_frame'])
     r = rooflines[dom]
     n_l = max(r['launches_per_frame'], 1)
-    tr = traffic.get(dom) if isinstance(traffic.get(dom), dict) else None
     if dom in per_frame_flops:                                      # dense layers: tensor roofline per SURVEY 8(d)
         roof = dict(kernel={'gemm': 'gemm_tc_kernel (all dense layers of a frame)'}.get(dom, dom), bound='tensor',
                     achieved=r['tensor_tflops'], peak=pk['tf_sust'], unit='TFLOP/s', frac=r['tensor_frac'],
-                    peak_source=pk['source'] + ' (cuBLAS bf16 sustained)',
+                    peak_source=pk['source'],
                     algorithmic_flops_per_launch=int(per_frame_flops[dom] / n_l), hbm_frac_on_compulsory_bytes=r['frac'])
     else:
         roof = dict(kernel={'sca_gather': 'sca gather kernel'}.get(dom, dom), bound='hbm', achieved=r['achieved'],
-                    peak=pk['hbm'], unit='GB/s', frac=r['frac'], peak_source=pk['source'] + ' (copy bandwidth)',
+                    peak=pk['hbm'], unit='GB/s', frac=r['frac'], peak_source=pk['source'],
                     algorithmic_bytes_per_launch=int(r['algorithmic_bytes_per_frame'] / n_l),
                     l1_bytes_per_clk_per_sm=r.get('l1_bytes_per_clk_per_sm'))
     if dom == 'sca_gather':
         roof['algorithmic_bytes_note'] = ('operator boundary as launched: value maps 6*Nv*256*s + fp16 offsets/logits Nq*768*2 + output '
                                           'Nq*256*s (SURVEY 8(d) quotes 166 MB/layer for a kernel that never materialises offsets/logits); '
                                           'the kernel is bound by the L1/LSU data path (l1_bytes_per_clk_per_sm), not by HBM: DESIGN.md section 4')
-    roof.update(traffic=tr.get('dram_bytes_per_launch') if tr else None, traffic_source=traffic.get('_source'),
-                avg_launch_ms=round(r['ms_per_frame'] / n_l, 4), launches_per_frame=n_l)
+    roof.update(avg_launch_ms=round(r['ms_per_frame'] / n_l, 4), launches_per_frame=n_l)
     cpu = cpu_baseline(cfg) if (world == 1 and not args.no_cpu) else None
     backbone = run_backbone_leg(args, cfg, eng, dev, want) if (not args.no_backbone and world == 1) else None
     frames_total = world * K * F
@@ -433,6 +440,27 @@ def run_ours(args):
                        'collective': 'all_reduce(sum) of 187 fp64 counters' if world > 1 else 'none (1 rank)'},
     }
     print(json.dumps(line))
+
+
+DUMP_VOXELS = 65536                                                   # sampled voxels per frame in --dump-outputs
+DUMP_MAX_BYTES = 64 * 2 ** 20                                         # all --dump-outputs files together
+
+
+def dump_outputs(out_dir, outs):
+    """The last timed step's results (one entry per frame, as eng.forward returned them) at a fixed, seeded voxel sample:
+    occ_cls [frames, n] and flow [frames, n, 2] as float32 plus the sample's flat voxel indices (float64).  n = 65536 voxels,
+    fewer when that many frames would take more than 64 MB in all (8.4 + 16.8 MB for the default 32 frames)."""
+    os.makedirs(out_dir, exist_ok=True)
+    nvox = outs[0]['occ_cls'].numel()
+    per_voxel = 12 * len(outs) + 8                                    # occ_cls 4 B + flow 8 B per frame, index 8 B
+    n = min(DUMP_VOXELS, nvox, (DUMP_MAX_BYTES - 4096) // per_voxel)  # (npy headers)
+    idx = np.sort(np.random.RandomState(0).choice(nvox, n, replace=False))
+    ti = torch.from_numpy(idx).to(outs[0]['occ_cls'].device)
+    cls = torch.stack([o['occ_cls'].reshape(-1)[ti] for o in outs]).float().cpu().numpy()
+    flow = torch.stack([o['flow'].reshape(-1, 2)[ti] for o in outs]).float().cpu().numpy()
+    np.save(os.path.join(out_dir, 'occ_cls.npy'), cls.astype(np.float32))
+    np.save(os.path.join(out_dir, 'flow.npy'), flow.astype(np.float32))
+    np.save(os.path.join(out_dir, 'voxel_index.npy'), idx.astype(np.float64))
 
 
 def run_dropin_leg(args, cfg, params, metas, frames_host, dev):
@@ -496,7 +524,7 @@ def run_temporal_leg(args, cfg, eng, frames_dev):
 
 def run_fp32_leg(args, cfg, params, metas, frames_f32, dev):
     """BASELINE configs[1] ('fp32'): the reference-precision configuration of the same engine (fp32 storage), timed and
-    checked against the fp32 oracle's golden frame.  Headline = the tcgen05 3xbf16-split GEMMs (fp32-grade, <= 1e-3 at six
+    checked against the fp32 oracle's golden frame.  Headline = the tensor-core 3xbf16-split GEMMs (fp32-grade, <= 1e-3 at six
     layers); the CUDA-core variant is reported beside it."""
     from occnet_b200.engine import OccEngine
 
@@ -522,7 +550,7 @@ def run_fp32_leg(args, cfg, params, metas, frames_f32, dev):
         torch.cuda.empty_cache()
         return {'value': round(1e3 / ms, 2), 'unit': 'samples/s', 'ms_per_frame': round(ms, 4), 'frames': n,
                 'launches_per_frame': lpf, 'tensor_cores': tc,
-                'gemm': 'tcgen05 3xbf16-split (fp32-grade), fp32 storage; conv3d / heads / LayerNorm on CUDA cores' if tc
+                'gemm': 'tensor-core 3xbf16-split (fp32-grade), fp32 storage; conv3d / heads / LayerNorm on CUDA cores' if tc
                         else 'fp32 CUDA cores',
                 'parity_vs_fp32_oracle': par}
     try:
@@ -539,8 +567,8 @@ def run_fp32_leg(args, cfg, params, metas, frames_f32, dev):
 def run_gpu_eager_baseline(cfg, params, metas, frames_f32, dev):
     """BASELINE.md section 5 comparator ('stock CUDA build'): the restated reference modules (oracle/bevformer_occ.py) on
     `cuda` with stock library kernels -- torch grid_sample MSDA, cuBLAS Linear, cuDNN Conv3d + BatchNorm3d, fp32, eager,
-    including the reference's Python rebatch loops and nonzero() syncs.  mmcv's own CUDA op cannot be built here (its
-    source is not under /root/reference), so this is the stated stand-in for the 1.3x / 6.5x targets' denominator."""
+    including the reference's Python rebatch loops and nonzero() syncs.  mmcv's own CUDA op is not part of the reference
+    project's sources, so this is the stated stand-in for a stock CUDA build."""
     try:
         from oracle import bevformer_occ as O
         p = {k: v.to(dev) for k, v in params.items()}
@@ -728,14 +756,18 @@ def main():
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--layers', type=int, default=6)
     ap.add_argument('--precision', default='bf16', choices=['bf16', 'fp32'])
-    ap.add_argument('--tc', type=int, default=1, help='tcgen05 tensor-core kernels (bf16 only)')
+    ap.add_argument('--tc', type=int, default=1, help='tensor-core (wgmma) kernels')
     ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg')
     ap.add_argument('--no-eager', action='store_true', help='skip the gpu_eager_baseline leg (stock torch kernels)')
     ap.add_argument('--no-dropin', action='store_true', help='skip the drop-in module-call e2e leg')
     ap.add_argument('--frames-per-step', type=int, default=32, help='one step = this many frames through the engine')
-    ap.add_argument('--repeats', type=int, default=3, help='timed regions (each exactly --steps steps); median reported')
+    ap.add_argument('--repeats', type=int, default=1, help='timed regions (each exactly --steps steps); median reported')
     ap.add_argument('--no-backbone', action='store_true', help='skip the images -> ResNet-50+FPN -> hot path leg')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help="write the last timed step's outputs (seeded voxel sample, float32 .npy) to DIR")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error('--steps must be >= 1 and --warmup >= 0')
     if args.impl == 'reference':
         run_reference(args)
     else:

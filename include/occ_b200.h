@@ -1,4 +1,4 @@
-/* libocc_b200 -- C ABI of the B200-native camera->occupancy hot path.
+/* libocc_b200 -- C ABI of the H100 (sm_90a) camera->occupancy hot path.
  *
  * Every entry point takes plain pointers and sizes (no torch / C++ types) and returns 0 on success;
  * on failure it returns non-zero and occb200_last_error() describes the problem (thread-local).
@@ -25,7 +25,7 @@ extern "C" {
 #endif
 
 const char* occb200_last_error(void);
-/* "occ_b200 <ver> sm_100a" */
+/* "occ_b200 <ver> sm_90a" */
 const char* occb200_version(void);
 
 /* ---------------------------------------------------------------------------------------------
@@ -73,7 +73,7 @@ typedef struct occb200_config {
     float pc_range[6];
     int precision;                 /* 0 = fp32 storage + fp32 CUDA-core GEMMs (parity config),
                                       1 = bf16 storage, fp32 accumulate (throughput config)                  */
-    int use_tensor_cores;          /* 1 = tcgen05 GEMM / conv kernels where available                       */
+    int use_tensor_cores;          /* 1 = wgmma GEMM / conv kernels where available                         */
     int use_cams_embeds;           /* TransformerOcc(use_cams_embeds=...), transformer_occ.py:214-215; 0 = the
                                       camera embedding is NOT added to the packed features                    */
     int rotate_center[2];          /* TransformerOcc(rotate_center=[100,100]), transformer_occ.py:200: centre
@@ -180,7 +180,7 @@ int occb200_linear_f32(const float* A, const float* W, const float* bias, const 
                        int N, int K, int act, void* stream);
 int occb200_layernorm_f32(const float* x, const float* gamma, const float* beta, float* y, int rows, int C,
                           void* stream);
-/* tcgen05 bf16 GEMM self-test entry: C f32 [M,N] = A bf16 [M,K] . W bf16 [N,K]^T (+bias); used by tests */
+/* tensor-core bf16 GEMM self-test entry: C f32 [M,N] = A bf16 [M,K] . W bf16 [N,K]^T (+bias); used by tests */
 int occb200_gemm_bf16_tc(const void* A_bf16, const void* W_bf16, const float* bias, float* C, int M, int N, int K,
                          void* stream);
 
@@ -191,7 +191,7 @@ int occb200_gemm_bf16_tc(const void* A_bf16, const void* W_bf16, const float* bi
  * (detectors/bevformer_occ.py:66-99) for the shipped configuration (bevformer_base_occ.py:48-66): mmdet
  * ResNet(depth=50, out_indices=(1,2,3), style='pytorch', norm_eval=True) + FPN(in_channels=[512,1024,2048],
  * out_channels=256, start_level=0, add_extra_convs='on_output', num_outs=4), eval mode.
- *   precision 0: fp32 storage, CUDA-core GEMMs (parity configuration); 1: bf16 storage (+ tcgen05 GEMMs).
+ *   precision 0: fp32 storage, CUDA-core GEMMs (parity configuration); 1: bf16 storage (+ tensor-core GEMMs).
  *   Parameters by their key in the detector's state_dict: "img_backbone.conv1.weight", "img_backbone.layer1.0.bn1.
  *   running_mean", "img_neck.lateral_convs.0.conv.bias", ... (HOST fp32; `num_batches_tracked` is not a parameter).
  *   forward: img dev f32 [num_images, 3, H, W] (mean/std-normalised, padded) -> out_l dev f32 [num_images, 256, h_l, w_l]

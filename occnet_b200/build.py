@@ -1,10 +1,9 @@
-"""Build libocc_b200.so in-tree with nvcc for sm_100a (no torch headers, no JIT cache).
+"""Build libocc_b200.so in-tree with nvcc for sm_90a (H100; no torch headers, no JIT cache).
 
     python -m occnet_b200.build            # incremental
     python -m occnet_b200.build --force
 
-The library is a plain C-ABI shared object (include/occ_b200.h).  It travels to the GPU box
-with the repo snapshot (git-ignored, not gpurun-ignored).
+The library is a plain C-ABI shared object (include/occ_b200.h), git-ignored.
 """
 import os
 import subprocess
@@ -16,7 +15,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(HERE, 'lib', 'obj')
 LIB = os.path.join(HERE, 'lib', 'libocc_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
          '--expt-relaxed-constexpr', '--expt-extended-lambda', '-Xptxas', '-v']
 
 
@@ -53,7 +52,7 @@ def build(force=False, log=True):
         res = list(ex.map(lambda s: _compile(s, force, log), srcs))
     objs = [r[0] for r in res]
     if force or any(r[1] for r in res) or not os.path.exists(LIB):
-        cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart']
+        cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a', '-lcudart']
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError('link failed:\n' + r.stderr[-4000:])

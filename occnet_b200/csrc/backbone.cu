@@ -3,9 +3,9 @@
 // bevformer_base_occ.py:48-66 puts in front of the hot path (caller: detectors/bevformer_occ.py:66-99; eval mode:
 // GridMask is the identity, BatchNorm uses running statistics).  SURVEY 8f rank 1 ("next").
 //
-// STATUS: validated on B200 in round 2 (tests/test_backbone_gpu.py); default feature extractor of the drop-in detector when it
+// Checked by tests/test_backbone_gpu.py; default feature extractor of the drop-in detector when it
 // is given images.  See backbone_kernels.cu / conv2d_tc.cu for the design (NHWC activations, BatchNorm folded, stride-1
-// convolutions on the TMA-im2col implicit-GEMM kernel, the others explicit im2col + the tcgen05 GEMM; fp32 parity
+// convolutions on the TMA-im2col implicit-GEMM kernel, the others explicit im2col + the wgmma GEMM; fp32 parity
 // configuration: the CUDA-core GEMM).
 #include <cuda_runtime.h>
 
@@ -143,9 +143,8 @@ int conv_gemm(occb200_backbone* e, const T* A, int64_t M, const ConvW& c, T* out
                            c.cout, c.kpad, act, st);
 }
 
-// Stride-1 3x3 convolutions (and 1x1 + residual) go through the TMA-im2col implicit-GEMM kernel conv2d_tc.cu (default since its
-// GPU validation in round 2: 7/7 backbone parity tests, backbone 10.3 -> 7.3 ms per frame); OCC_BACKBONE_IMPLICIT=0 selects the
-// explicit im2col + gemm_tc path for everything.
+// Stride-1 3x3 convolutions (and 1x1 + residual) go through the TMA-im2col implicit-GEMM kernel conv2d_tc.cu (the default: it
+// skips the im2col round trip through memory); OCC_BACKBONE_IMPLICIT=0 selects the explicit im2col + gemm_tc path for everything.
 bool implicit_enabled()
 {
     static const bool on = getenv("OCC_BACKBONE_IMPLICIT") == nullptr || atoi(getenv("OCC_BACKBONE_IMPLICIT")) != 0;

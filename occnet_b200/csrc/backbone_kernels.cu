@@ -1,12 +1,12 @@
 // Layout / data-movement kernels of the image backbone + neck (ResNet-50 + FPN feeding the hot path, SURVEY 8f rank 1;
 // reference: detectors/bevformer_occ.py:66-99 with the mmdet modules configured in bevformer_base_occ.py:48-66).
 //
-// STATUS: validated on B200 in round 2 (tests/test_backbone_gpu.py, 8 tests against the pinned backbone oracle); the bench's
-// `images_to_voxels` leg times it (profiles/README.md).  The stride-1 3x3 convolutions and the bottleneck's last 1x1 moved to the
+// Checked by tests/test_backbone_gpu.py (8 tests against the pinned backbone oracle); the bench's
+// `images_to_voxels` leg times it.  The stride-1 3x3 convolutions and the bottleneck's last 1x1 moved to the
 // TMA-im2col kernel conv2d_tc.cu; what is described here is the explicit-im2col path that the remaining convolutions still use.
 //
 // Design of the explicit path: activations are channels-last (NHWC); every convolution is a GEMM on the validated
-// tcgen05 kernel (gemm_tc.cu; CUDA-core gemm_simt.cu in the fp32 parity configuration):
+// wgmma kernel (gemm_tc.cu; CUDA-core gemm_simt.cu in the fp32 parity configuration):
 //   1x1 stride 1          : the NHWC tensor IS the [pixels, Cin] operand
 //   3x3 / 7x7 / strided   : explicit im2col into a [pixels_out, K] operand (K = KH*KW*Cin zero-padded to 64)
 // BatchNorm is folded into the weights at finalize, ReLU rides the GEMM epilogue, the bottleneck's residual add and
@@ -58,7 +58,7 @@ __global__ void im2col_nhwc_kernel(const T* __restrict__ in, T* __restrict__ out
 }
 
 // Any C (the 7x7 stem: C = 3): 8 consecutive k per thread, ONE 16-byte store, (tap, c) advanced incrementally.  The element-per-
-// thread form (VEC = 1) spent its time in five 64-bit divisions per 2-byte element: 3.3 ms of the 7.3 ms backbone on the stem alone.
+// thread form (VEC = 1) spends its time in five 64-bit divisions per 2-byte element.
 template <typename T>
 __global__ void im2col_nhwc_any_kernel(const T* __restrict__ in, T* __restrict__ out, int N, int H, int W, int C, int KH,
                                        int KW, int stride, int pad, int Ho, int Wo, int Kpad)
@@ -89,8 +89,8 @@ __global__ void im2col_nhwc_any_kernel(const T* __restrict__ in, T* __restrict__
 
 // Small-C im2col through shared memory (the 7x7 / stride-2 stem, C = 3): one CTA = 128 output pixels of one output row.  The KH
 // input rows it needs ((127*stride + KW) * C elements each) are staged once with coalesced loads; every thread then assembles
-// 16-byte chunks (8 consecutive k) of the output rows from shared memory and writes them coalesced.  855 MB of im2col rows for
-// 6 x 928 x 1600 images: element-per-thread 3.3 ms, 8-per-thread from global 0.81 ms, this kernel see profiles/README.md.
+// 16-byte chunks (8 consecutive k) of the output rows from shared memory and writes them coalesced (855 MB of im2col rows for
+// 6 x 928 x 1600 images: an element-per-thread gather from global memory was the slowest step of the backbone).
 constexpr int STEM_TW = 128, STEM_MAX_KH = 7, STEM_MAX_SPAN = 1024;
 template <typename T>
 __global__ void __launch_bounds__(256)

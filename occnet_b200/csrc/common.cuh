@@ -1,4 +1,4 @@
-// Shared device/host helpers for libocc_b200 (sm_100a only).
+// Shared device/host helpers for libocc_b200 (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

@@ -1,20 +1,16 @@
-// Implicit-GEMM 2-D convolution (stride 1) on the 5th-gen tensor cores for the image backbone / neck (sm_100a):
+// Implicit-GEMM 2-D convolution (stride 1) on the tensor cores for the image backbone / neck (sm_90a):
 //     out[n, y, x, co] = act( sum_{ky,kx,ci} in[n, y+ky-pad, x+kx-pad, ci] * w[co][(ky*KW+kx)*Cin + ci] + bias[co]
-//                             (+ residual[n, y, x, co]) ),      NHWC bf16 tensors, fp32 accumulation in TMEM.
+//                             (+ residual[n, y, x, co]) ),      NHWC bf16 tensors, fp32 accumulation in registers.
 // Used for the 3x3 convolutions of ResNet-50 / FPN and (KH = KW = 1) for the bottleneck's last 1x1 convolution with the
 // residual add + ReLU fused (reference: mmdet ResNet / FPN as configured in bevformer_base_occ.py:48-66).
-//
-// STATUS: validated on B200 in round 2 (tests/test_backbone_gpu.py with and without it; images -> voxels 75.9 -> 98.9 samples/s);
-// default for the stride-1 convolutions of the backbone (OCC_BACKBONE_IMPLICIT=0: explicit im2col + gemm_tc for everything).
+// Default for the stride-1 convolutions of the backbone (OCC_BACKBONE_IMPLICIT=0: explicit im2col + gemm_tc for everything).
 //
 // Same skeleton as gemm_tc.cu (persistent, one CTA per SM, warp-specialised), with im2col done by TMA as in conv3d_tc.cu:
 //   M tile  = 128 output pixels = 8 rows x 16 columns of one image; K loop = taps x (Cin / 64)
-//   warp 0   TMA producer : per k-block one 4-D box {64 ch, 16 x, 8 y, 1 n} of the input at the tap's (ky,kx) offset
-//                           (out-of-bounds pixels zero-filled by the TMA unit = the conv's zero padding) + the weight
-//                           k-block [BN x 64]; 128B swizzle; 4-6 stage mbarrier ring
-//   warp 1   MMA issuer   : tcgen05.mma.cta_group::1.kind::f16, M=128, N=BN, K=16 x4 per stage; 2 x 256 TMEM columns
-//   warps 2-9 epilogue    : tcgen05.ld -> +bias (+residual, fetched by TMA into a per-warp staging block) -> ReLU ->
-//                           bf16 -> swizzled staging -> TMA store of a {32 ch, 16 x, 2 y} box
+//   warps 8-11 producer warpgroup (warp 8 issues): per k-block one 4-D box {64 ch, 16 x, 8 y, 1 n} of the input at the tap's (ky,kx) offset
+//                             (out-of-bounds pixels zero-filled by the TMA unit = the conv's zero padding) + the weight
+//                             k-block [BN x 64]; 128B swizzle; 2-6 stage mbarrier ring
+//   warps 0-7  two consumer warpgroups: wgmma.m64n64k16 over 64 pixels each, then +bias (+residual) -> ReLU -> bf16 stores
 #include <cstdlib>
 
 #include "common.cuh"
@@ -26,32 +22,25 @@ namespace occ {
 namespace {
 
 constexpr int BLOCK_M = 128, BLOCK_K = 64, A_TILE_BYTES = BLOCK_M * BLOCK_K * 2, TILE_W = 16, TILE_H = 8;
-constexpr int NUM_THREADS = 320, MAX_STAGES = 6, STG_BYTES = 2048;
+constexpr int NUM_THREADS = 384, MAX_STAGES = 6;      // 2 consumer warpgroups + 1 producer warpgroup
 constexpr int SMEM_MAX = 232448 - 1024;
-// tail: 8 output staging blocks + 8 residual staging blocks + barriers + per-column bias
-constexpr int SMEM_TAIL = 8 * STG_BYTES + 8 * STG_BYTES + 256 + 1024;
+constexpr int SMEM_TAIL = 256 + 1024;                     // barriers + per-column bias
 
 struct Geom { int N, H, W, Cin, Cout, KH, KW, pad; };
 
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv2d_tc_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant__ CUtensorMap tmW,
-                 const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes,
-                 const float* __restrict__ bias, Geom g, int BN, int stages, int act, int has_res)
+                 const float* __restrict__ bias, const bf16* __restrict__ residual, bf16* __restrict__ out, Geom g, int BN,
+                 int stages, int act)
 {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t w_tile_bytes = BN * BLOCK_K * 2;
     const uint32_t stage_bytes = A_TILE_BYTES + w_tile_bytes;
     const uint32_t ring_base = smem_base;
-    const uint32_t stg_base = ring_base + stages * stage_bytes;              // 8 x 2 KB output staging (1024-aligned)
-    const uint32_t res_base = stg_base + 8 * STG_BYTES;                      // 8 x 2 KB residual staging
-    const uint32_t bar_base = res_base + 8 * STG_BYTES;
+    const uint32_t bar_base = ring_base + stages * stage_bytes;
     auto full_bar = [&](int s) { return bar_base + s * 8; };
     auto empty_bar = [&](int s) { return bar_base + (MAX_STAGES + s) * 8; };
-    auto tfull_bar = [&](int s) { return bar_base + (2 * MAX_STAGES + s) * 8; };
-    auto tempty_bar = [&](int s) { return bar_base + (2 * MAX_STAGES + 2 + s) * 8; };
-    const uint32_t tmem_slot = bar_base + (2 * MAX_STAGES + 4) * 8;
-    auto res_bar = [&](int w) { return bar_base + (2 * MAX_STAGES + 6 + w) * 8; };   // one per epilogue warp
     float* const cvec = reinterpret_cast<float*>(smem_raw + (bar_base + 256 - tc::smem_u32(smem_raw)));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -63,28 +52,22 @@ conv2d_tc_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant
     const int t_begin = (int)(((long long)m_tiles * grp) / ngrp), t_end = (int)(((long long)m_tiles * (grp + 1)) / ngrp);
     const int taps = g.KH * g.KW, ncb = g.Cin / BLOCK_K, nk = taps * ncb;
 
-    if (warp == 0 && lane == 0) {
-        tc::tma_prefetch_desc(&tmIn); tc::tma_prefetch_desc(&tmW); tc::tma_prefetch_desc(&tmOut);
-        if (has_res) tc::tma_prefetch_desc(&tmRes);
-        for (int s = 0; s < stages; ++s) { tc::mbar_init(full_bar(s), 1); tc::mbar_init(empty_bar(s), 1); }
-        for (int s = 0; s < 2; ++s) { tc::mbar_init(tfull_bar(s), 1); tc::mbar_init(tempty_bar(s), 256); }
-        for (int w = 0; w < 8; ++w) tc::mbar_init(res_bar(w), 1);
+    if (warp == 8 && lane == 0) {
+        tc::tma_prefetch_desc(&tmIn); tc::tma_prefetch_desc(&tmW);
+        for (int s = 0; s < stages; ++s) { tc::mbar_init(full_bar(s), 1); tc::mbar_init(empty_bar(s), 2); }
         tc::mbar_fence_init();
     }
-    if (warp == 1) tc::tmem_alloc(tmem_slot, 512);
-    tc::tc_fence_before();
+    if (threadIdx.x < BN) cvec[threadIdx.x] = bias ? __ldg(bias + n_blk * BN + threadIdx.x) : 0.f;
     __syncthreads();
-    tc::tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
     auto decode = [&](int t, int& n, int& y0, int& x0) {
         const int tx = t % tiles_x, ty = (t / tiles_x) % tiles_y;
         n = t / (tiles_x * tiles_y); y0 = ty * TILE_H; x0 = tx * TILE_W;
     };
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= 8) {
+        tc::setmaxnreg_dec<40>();                                 // producer warpgroup: registers go to the consumers
+        if (warp == 8 && lane == 0) {
             int s = 0; uint32_t ph = 0;
             for (int t = t_begin; t < t_end; ++t) {
                 int n, y0, x0;
@@ -102,121 +85,52 @@ conv2d_tc_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant
                 }
             }
         }
-    } else if (warp == 1) {
-        // all 32 lanes run the issue loop in warp-uniform control flow (operands in the uniform datapath); elect.sync picks the
-        // issuing lane -- see tc::umma_bf16_elect (the N = 64 / 128 layers of the backbone are MMA-issue bound)
-        tmem_base = __shfl_sync(0xffffffffu, tmem_base, 0);
-        {
-            const uint32_t idesc = tc::make_idesc_bf16(BLOCK_M, BN);
-            int s = 0; uint32_t ph = 0; int as = 0; uint32_t aph = 0;
-            for (int t = t_begin; t < t_end; ++t) {
-                tc::mbar_wait(tempty_bar(as), aph ^ 1);
-                tc::tc_fence_after();
-                for (int kb = 0; kb < nk; ++kb) {
-                    tc::mbar_wait(full_bar(s), ph);
-                    tc::tc_fence_after();
-                    const uint32_t a_addr = ring_base + s * stage_bytes;
-                    const uint64_t da = tc::make_smem_desc(a_addr, 128);
-                    const uint64_t db = tc::make_smem_desc(a_addr + A_TILE_BYTES, 128);
-#pragma unroll
-                    for (int k = 0; k < BLOCK_K / 16; ++k)
-                        tc::umma_bf16_elect(tmem_base + as * 256, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-                    tc::umma_commit_elect(empty_bar(s));
-                    tc::umma_commit_elect(tfull_bar(as), kb == nk - 1 ? 1u : 0u);
-                    __syncwarp();
-                    if (++s == stages) { s = 0; ph ^= 1; }
-                }
-                if (++as == 2) { as = 0; aph ^= 1; }
+        return;
+    }
+
+    tc::setmaxnreg_inc<232>();
+    const int wg = warp >> 2, wl = warp & 3;
+    const int nsubs = BN >> 6;
+    const int quad_col = 2 * (lane & 3);
+    int s = 0; uint32_t ph = 0;
+    for (int t = t_begin; t < t_end; ++t) {
+        int n, y0, x0;
+        decode(t, n, y0, x0);
+        float acc[4][32];
+        for (int kb = 0; kb < nk; ++kb) {
+            tc::mbar_wait(full_bar(s), ph);
+            const uint32_t a_addr = ring_base + s * stage_bytes + wg * (64 * 128);
+            const uint32_t b_addr = ring_base + s * stage_bytes + A_TILE_BYTES;
+            switch (nsubs) {
+            case 4: tc::wgmma_kblock<4>(acc, a_addr, b_addr, kb == 0); break;
+            case 2: tc::wgmma_kblock<2>(acc, a_addr, b_addr, kb == 0); break;
+            default: tc::wgmma_kblock<1>(acc, a_addr, b_addr, kb == 0); break;
             }
+            if ((threadIdx.x & 127) == 0) tc::mbar_arrive(empty_bar(s));
+            if (++s == stages) { s = 0; ph ^= 1; }
         }
-    } else {
-        // per-column bias of this CTA's n-block -> shared memory, once (see gemm_tc.cu for why not __ldg in the loop)
-        {
-            const int c = threadIdx.x - 64;
-            if (c < BN) cvec[c] = bias ? __ldg(bias + n_blk * BN + c) : 0.f;
-            asm volatile("bar.sync 5, 256;" ::: "memory");
-        }
-        const int quarter = warp & 3, half = (warp - 2) >> 2, ew = warp - 2;
-        const int ncol = BN >> 1, cbeg = half * ncol;
-        const uint32_t stg = stg_base + ew * STG_BYTES, rstg = res_base + ew * STG_BYTES;
-        const uint32_t rbar = res_bar(ew);
-        uint32_t rph = 0;
-        int as = 0; uint32_t aph = 0;
-        for (int t = t_begin; t < t_end; ++t) {
-            int n, y0, x0;
-            decode(t, n, y0, x0);
-            const int yq = y0 + quarter * 2;                      // this warp's 32 TMEM lanes = 2 image rows x 16 pixels
-            const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + as * 256;
-            if (has_res && lane == 0) {                           // residual of the first box: in flight during the main loop
-                tc::mbar_arrive_expect_tx(rbar, STG_BYTES);
-                tc::tma_load_4d(rstg, &tmRes, rbar, n_blk * BN + cbeg, x0, yq, n);
-            }
-            tc::mbar_wait(tfull_bar(as), aph);
-            tc::tc_fence_after();
-            for (int c0 = cbeg; c0 < cbeg + ncol; c0 += 32) {
-                uint32_t r[32];
-                tc::tmem_ld32(taddr + c0, r);
-                tc::tmem_ld_wait();
-                float res[32];
 #pragma unroll
-                for (int j = 0; j < 32; ++j) res[j] = 0.f;
-                if (has_res) {
-                    tc::mbar_wait(rbar, rph);
-                    rph ^= 1;
+        for (int h = 0; h < 2; ++h) {
+            const int r = wg * 64 + 16 * wl + (lane >> 2) + 8 * h;     // tile row = 16 * (y - y0) + (x - x0)
+            const int y = y0 + (r >> 4), x = x0 + (r & 15);
+            if (y >= g.H || x >= g.W) continue;
+            const size_t pix = (((size_t)n * g.H + y) * g.W + x) * g.Cout + n_blk * BN;
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {                 // my row's 64 bytes: piece j sits at j ^ ((row >> 1) & 3)
-                        uint32_t a, b, c, d;
-                        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d)
-                                     : "r"(rstg + lane * 64 + ((j ^ ((lane >> 1) & 3)) << 4)) : "memory");
-                        const uint32_t wds[4] = {a, b, c, d};
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) {
-                            res[8 * j + 2 * q] = __uint_as_float(wds[q] << 16);
-                            res[8 * j + 2 * q + 1] = __uint_as_float(wds[q] & 0xffff0000u);
-                        }
-                    }
-                    tc::fence_proxy_async_smem();                 // generic reads done before the next TMA write
-                    __syncwarp();
-                    if (lane == 0 && c0 + 32 < cbeg + ncol) {     // prefetch the residual of the next box
-                        tc::mbar_arrive_expect_tx(rbar, STG_BYTES);
-                        tc::tma_load_4d(rstg, &tmRes, rbar, n_blk * BN + c0 + 32, x0, yq, n);
-                    }
-                }
-                uint32_t pk[16];
+            for (int ns = 0; ns < 4; ++ns) {
+                if (ns >= nsubs) break;
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
-                    const float4 b4 = reinterpret_cast<const float4*>(cvec + c0)[j];
-                    float x0f = __uint_as_float(r[4 * j]) + b4.x + res[4 * j];
-                    float x1f = __uint_as_float(r[4 * j + 1]) + b4.y + res[4 * j + 1];
-                    float x2f = __uint_as_float(r[4 * j + 2]) + b4.z + res[4 * j + 2];
-                    float x3f = __uint_as_float(r[4 * j + 3]) + b4.w + res[4 * j + 3];
-                    if (act == ACT_RELU) { x0f = fmaxf(x0f, 0.f); x1f = fmaxf(x1f, 0.f); x2f = fmaxf(x2f, 0.f); x3f = fmaxf(x3f, 0.f); }
-                    pk[2 * j] = pack_bf16x2(x0f, x1f); pk[2 * j + 1] = pack_bf16x2(x2f, x3f);
-                }
-                if (lane == 0) tc::tma_store_wait_read();         // the previous store has drained the staging block
-                __syncwarp();
-#pragma unroll
-                for (int j = 0; j < 4; ++j)                       // 64-byte rows, SWIZZLE_64B: piece j -> j ^ ((row >> 1) & 3)
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(stg + lane * 64 + ((j ^ ((lane >> 1) & 3)) << 4)),
-                                 "r"(pk[4 * j]), "r"(pk[4 * j + 1]), "r"(pk[4 * j + 2]), "r"(pk[4 * j + 3]) : "memory");
-                tc::fence_proxy_async_smem();
-                __syncwarp();
-                if (lane == 0) {
-                    tc::tma_store_4d(&tmOut, stg, n_blk * BN + c0, x0, yq, n);
-                    tc::tma_store_commit();
+                    const int cl = ns * 64 + 8 * j + quad_col;
+                    float v0 = acc[ns][4 * j + 2 * h] + cvec[cl], v1 = acc[ns][4 * j + 2 * h + 1] + cvec[cl + 1];
+                    if (residual) {
+                        const uint32_t q = __ldg(reinterpret_cast<const unsigned int*>(residual + pix + cl));
+                        v0 += __uint_as_float(q << 16); v1 += __uint_as_float(q & 0xffff0000u);
+                    }
+                    if (act == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                    *reinterpret_cast<uint32_t*>(out + pix + cl) = pack_bf16x2(v0, v1);
                 }
             }
-            tc::tc_fence_before();
-            tc::mbar_arrive(tempty_bar(as));
-            if (++as == 2) { as = 0; aph ^= 1; }
         }
-        if (lane == 0) tc::tma_store_wait_all();
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc::tc_fence_after();
-        tc::tmem_dealloc(tmem_base, 512);
     }
 }
 
@@ -238,7 +152,7 @@ int conv2d_tc(const bf16* in, const bf16* w_tap_major, const float* bias, const 
     if (stages > MAX_STAGES) stages = MAX_STAGES;
     OCC_CHECK(stages >= 2, "conv2d_tc: not enough shared memory for two stages");
     const int smem = 1024 + stages * stage + SMEM_TAIL;
-    CUtensorMap tmIn, tmW, tmOut, tmRes;
+    CUtensorMap tmIn, tmW;
     {
         const uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
         const uint64_t strides[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
@@ -250,14 +164,6 @@ int conv2d_tc(const bf16* in, const bf16* w_tap_major, const float* bias, const 
         const uint32_t box[2] = {BLOCK_K, (uint32_t)BN};
         if (make_tensor_map_bf16(&tmW, w_tap_major, 2, dims, strides, box, 128)) return 1;
     }
-    {
-        const uint64_t dims[4] = {(uint64_t)Cout, (uint64_t)W, (uint64_t)H, (uint64_t)N};
-        const uint64_t strides[3] = {(uint64_t)Cout * 2, (uint64_t)W * Cout * 2, (uint64_t)H * W * Cout * 2};
-        const uint32_t box[4] = {32, TILE_W, 2, 1};
-        if (make_tensor_map_bf16(&tmOut, out, 4, dims, strides, box, 64)) return 1;
-        tmRes = tmOut;
-        if (residual && make_tensor_map_bf16(&tmRes, residual, 4, dims, strides, box, 64)) return 1;
-    }
     const int num_sms = sm_count_current_device();
     OCC_CUDA(cudaFuncSetAttribute(conv2d_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));   // per device
     const int m_tiles = N * ((H + TILE_H - 1) / TILE_H) * ((W + TILE_W - 1) / TILE_W), n_tiles = Cout / BN;
@@ -265,8 +171,7 @@ int conv2d_tc(const bf16* in, const bf16* w_tap_major, const float* bias, const 
     if (per_n < 1) per_n = 1;
     if (per_n > m_tiles) per_n = m_tiles;
     const Geom g{N, H, W, Cin, Cout, KH, KW, pad};
-    conv2d_tc_kernel<<<per_n * n_tiles, NUM_THREADS, smem, stream>>>(tmIn, tmW, tmOut, tmRes, bias, g, BN, stages, act,
-                                                                     residual != nullptr ? 1 : 0);
+    conv2d_tc_kernel<<<per_n * n_tiles, NUM_THREADS, smem, stream>>>(tmIn, tmW, bias, residual, out, g, BN, stages, act);
     OCC_CUDA(cudaGetLastError());
     return 0;
 }

@@ -1,4 +1,4 @@
-// Implicit-GEMM stride-1 2-D convolution on tcgen05 (conv2d_tc.cu): NHWC bf16, weights tap-major [Cout][KH*KW*Cin].
+// Implicit-GEMM stride-1 2-D convolution on wgmma (conv2d_tc.cu): NHWC bf16, weights tap-major [Cout][KH*KW*Cin].
 #pragma once
 #include "common.cuh"
 

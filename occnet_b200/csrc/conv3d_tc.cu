@@ -1,4 +1,4 @@
-// Voxel decoder on the 5th-gen tensor cores (sm_100a): 3x3x3 Conv3d (pad 1, no bias) + folded
+// Voxel decoder on the tensor cores (sm_90a): 3x3x3 Conv3d (pad 1, no bias) + folded
 // BatchNorm3d + ReLU as an implicit GEMM.   Reference: TransformerOcc.decoder (use_3d),
 // projects/mmdet3d_plugin/bevformer/modules/transformer_occ.py:106-131, applied at :305-308.
 //
@@ -9,9 +9,20 @@
 // coordinates and a one-row y halo on both sides, so the three dy shifts are SUB-VIEWS of the same shared-memory tile
 // (row offset dy * 16, a multiple of the 8-row swizzle atom); out-of-bounds rows are zero-filled by the TMA unit, which
 // IS the conv's zero padding (including the z = -1 / z = 16 halo).  All 27 weight tiles stay resident in shared memory.
-//   warp 0: TMA producer (8-stage ring)    warp 1: tcgen05.mma issuer (plane-major: each loaded tile feeds the
-//   dx = 0/1/2 taps of three neighbouring outputs through ONE N = 96 MMA into adjacent TMEM slots, ring of 8)
-//   warps 2-5: epilogue (tcgen05.ld -> +bias -> ReLU -> bf16 -> 64-byte rows, contiguous 8 KB per tile)
+//   warp 8: TMA producer (8-stage ring)
+//   warps 0-7: two consumer warpgroups, each owning 64 of the tile's 128 voxels (4 y rows x 16 z)
+//
+// Plane-major schedule: an input tile (plane x = p, shift (dz,dy)) is the A operand of three taps -- dx = 0, 1, 2 of
+// the outputs x = p+1, p, p-1 -- so it is loaded ONCE (~9 instead of 27 tile loads per output tile) and multiplied into the
+// three live accumulators with ONE wgmma of N = 96: the weight tiles of a (dz,dy) pair are resident in the order dx = 2, 1, 0,
+// so accumulator columns [0,32) belong to output p-1, [32,64) to p and [64,96) to p+1.  After plane p the output p-1 is
+// complete: it is written out and the accumulator window slides by 32 columns (register moves).
+// Each CTA owns a contiguous range of the (y_tile, x) tile sequence, cut into segments of constant y_tile; a segment
+// [xa, xb) streams the planes max(xa-1,0) .. min(xb, X-1).
+// EPI: 0 = bf16 out = relu(acc + bias) (the bf16 configuration); fp32-storage configuration, one of three split passes
+// (hi.W_hi, lo.W_hi, hi.W_lo of the bf16 split of an fp32 input, relative error ~2^-16 like gemm_tc_split3):
+// 1 = out_f32 = acc, 2 = out_f32 += acc, 3 = out_f32 = relu(out_f32 + acc + bias).  Every output element is owned by one thread
+// per pass, so the fp32 accumulation across passes needs no atomics.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -22,30 +33,12 @@ namespace occ {
 
 namespace {
 
-constexpr int STAGES = 8, TILE_Y = 8, TILE_Z = 16, BLOCK_M = 128, COUT = 32, TAPS = 27, SLOTS = 8;
+constexpr int STAGES = 8, TILE_Y = 8, TILE_Z = 16, COUT = 32, TAPS = 27;
 constexpr int HALO_ROWS = (TILE_Y + 2) * TILE_Z;          // rows of one staged tile: y0-1 .. y0+8, all 16 z
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 288;
 constexpr int BAR_BYTES = 512;
 
-// Plane-major schedule: an input tile (plane x = p, shift (dz,dy)) is the A operand of three taps -- dx = 0, 1, 2 of
-// the outputs x = p+1, p, p-1 -- so it is loaded ONCE (L2->SMEM traffic: ~9 instead of 27 tile loads per output tile)
-// and multiplied into the three live accumulators with ONE tcgen05.mma of N = 96: the accumulators of consecutive
-// outputs sit in consecutive 32-column TMEM slots (ring of 8), and the weight tiles of a (dz,dy) pair are resident in
-// the order dx = 2, 1, 0, i.e. ascending output x.  (The first version issued three N = 32 MMAs per tile: ncu showed
-// the single MMA-issuing thread, not TMA or the tensor pipe, was the limiter -- ~64 pipe cycles and ~180 issue-thread
-// cycles per tiny MMA.)  Accumulators are zeroed by the epilogue warps when they drain a slot, so every MMA
-// accumulates and the issue loop has no per-output special cases.
-// Each CTA owns a contiguous range of the (y_tile, x) tile sequence, cut into segments of constant y_tile; a segment
-// [xa, xb) streams the planes max(xa-1,0) .. min(xb, X-1).
-// UNI: the producer / issuer warps run their loops with ALL 32 lanes (lane 0 alone executes the TMA / MMA / commit
-// instructions): loop counters, stage indices and UMMA descriptors are then warp-uniform values the compiler keeps in the
-// uniform datapath, instead of per-lane registers that need an R2UR move in front of every tcgen05.mma operand (ncu of the
-// single-lane version: 1.8 M R2UR + 1.3 M IMAD around 0.19 M MMAs; the issuing thread, not the tensor pipe, was the limiter).
-// EPI: 0 = bf16 out = relu(acc + bias) (the bf16 configuration); fp32-storage configuration, one of three split passes
-// (hi.W_hi, lo.W_hi, hi.W_lo of the bf16 split of an fp32 input, relative error ~2^-16 like gemm_tc_split3):
-// 1 = out_f32 = acc, 2 = out_f32 += acc, 3 = out_f32 = relu(out_f32 + acc + bias).  Every output row is owned by one thread per
-// pass, so the fp32 accumulation across passes needs no atomics.
-template <int CIN, bool UNI, int EPI>
+template <int CIN, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv3d_tc_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant__ CUtensorMap tmW,
                  const float* __restrict__ bias, bf16* __restrict__ out, float* __restrict__ out_f32, int X, int Y)
@@ -61,38 +54,26 @@ conv3d_tc_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant
     const uint32_t bar_base = a_base + STAGES * A_BYTES;
     auto full_bar = [&](int s) { return bar_base + s * 8; };
     auto empty_bar = [&](int s) { return bar_base + (STAGES + s) * 8; };
-    auto tfull_bar = [&](int s) { return bar_base + (2 * STAGES + s) * 8; };
-    auto tempty_bar = [&](int s) { return bar_base + (2 * STAGES + SLOTS + s) * 8; };
-    const uint32_t w_bar = bar_base + (2 * STAGES + 2 * SLOTS) * 8;
-    const uint32_t tmem_slot = bar_base + (2 * STAGES + 2 * SLOTS + 1) * 8;
+    const uint32_t w_bar = bar_base + (2 * STAGES) * 8;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int y_tiles = (Y + TILE_Y - 1) / TILE_Y;
     const long long total = (long long)X * y_tiles;
     const int t_begin = (int)(total * blockIdx.x / gridDim.x), t_end = (int)(total * (blockIdx.x + 1) / gridDim.x);
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tc::tma_prefetch_desc(&tmIn); tc::tma_prefetch_desc(&tmW);
-        for (int s = 0; s < STAGES; ++s) { tc::mbar_init(full_bar(s), 1); tc::mbar_init(empty_bar(s), 1); }
-        for (int s = 0; s < SLOTS; ++s) { tc::mbar_init(tfull_bar(s), 1); tc::mbar_init(tempty_bar(s), 128); }
+        for (int s = 0; s < STAGES; ++s) { tc::mbar_init(full_bar(s), 1); tc::mbar_init(empty_bar(s), 2); }
         tc::mbar_init(w_bar, 1);
         tc::mbar_fence_init();
     }
-    if (warp == 1) tc::tmem_alloc(tmem_slot, 32 * SLOTS);
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-    const bool leader = lane == 0;
-    if (warp == 0) {
-        if (UNI || leader) {
-            if (leader) {
-                tc::mbar_arrive_expect_tx(w_bar, TAPS * W_TAP_BYTES);
-                for (int t = 0; t < TAPS; ++t)               // global tap order is (dz,dy,dx); resident order (dz,dy,2-dx)
-                    tc::tma_load_2d(w_base + ((t / 3) * 3 + (2 - t % 3)) * W_TAP_BYTES, &tmW, w_bar, 0, t * COUT);
-            }
+    if (warp == 8) {
+        if (lane == 0) {
+            tc::mbar_arrive_expect_tx(w_bar, TAPS * W_TAP_BYTES);
+            for (int t = 0; t < TAPS; ++t)                   // global tap order is (dz,dy,dx); resident order (dz,dy,2-dx)
+                tc::tma_load_2d(w_base + ((t / 3) * 3 + (2 - t % 3)) * W_TAP_BYTES, &tmW, w_bar, 0, t * COUT);
             int s = 0; uint32_t ph = 0;
             for (int t = t_begin; t < t_end;) {
                 const int yt = t / X, xa = t % X;
@@ -102,172 +83,83 @@ conv3d_tc_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant
                 for (int p = p_lo; p <= p_hi; ++p) {
                     for (int dz = 0; dz < 3; ++dz) {
                         tc::mbar_wait(empty_bar(s), ph ^ 1);
-                        if (leader) {
-                            tc::mbar_arrive_expect_tx(full_bar(s), A_BYTES);
-                            tc::tma_load_4d(a_base + s * A_BYTES, &tmIn, full_bar(s), 0, dz - 1, y0 - 1, p);
-                        }
+                        tc::mbar_arrive_expect_tx(full_bar(s), A_BYTES);
+                        tc::tma_load_4d(a_base + s * A_BYTES, &tmIn, full_bar(s), 0, dz - 1, y0 - 1, p);
                         if (++s == STAGES) { s = 0; ph ^= 1; }
                     }
                 }
                 t += xb - xa;
             }
         }
-    } else if (warp == 1) {
-        if (UNI || leader) {
-            const uint32_t idesc1 = tc::make_idesc_bf16(BLOCK_M, COUT), idesc2 = tc::make_idesc_bf16(BLOCK_M, 2 * COUT),
-                           idesc3 = tc::make_idesc_bf16(BLOCK_M, 3 * COUT);
-            auto idesc_of = [&](int outputs) { return outputs == 1 ? idesc1 : (outputs == 2 ? idesc2 : idesc3); };
-            const uint64_t da0 = tc::make_smem_desc(a_base, ROW_BYTES), db0 = tc::make_smem_desc(w_base, ROW_BYTES);
-            int s = 0; uint32_t ph = 0;
-            int n_base = 0;
-            if (UNI) tmem_base = __shfl_sync(0xffffffffu, tmem_base, 0);     // (a broadcast from lane 0 is a uniform value to ptxas)
-            tc::mbar_wait(w_bar, 0);
-            tc::tc_fence_after();
-            for (int t = t_begin; t < t_end;) {
-                const int xa = t % X;
-                const int xb = min(X, xa + (t_end - t));
-                const int p_lo = max(xa - 1, 0), p_hi = min(xb, X - 1);
-                for (int p = p_lo; p <= p_hi; ++p) {
-                    const int x_lo = max(p - 1, xa), x_hi = min(p + 1, xb - 1);      // outputs this plane feeds
-                    const int cnt = x_hi - x_lo + 1, off = x_lo - (p - 1);            // 1..3 outputs, first weight sub-tile
-                    const int n_lo = n_base + (x_lo - xa), slot_lo = n_lo & (SLOTS - 1);
-                    const int first = min(cnt, SLOTS - slot_lo);                       // outputs before the ring wraps
-                    // outputs whose first plane this is: x = p+1 (and x = 0 on plane 0) -- their slot must be drained + zeroed
-                    for (int x = x_lo; x <= x_hi; ++x) {
-                        if (max(x - 1, 0) != p) continue;
-                        const int n = n_base + (x - xa);
-                        tc::mbar_wait(tempty_bar(n & (SLOTS - 1)), (n / SLOTS) & 1);
-                    }
-                    tc::tc_fence_after();
-                    const uint32_t d0 = tmem_base + slot_lo * COUT;
-                    const uint32_t i_first = idesc_of(first), i_rest = idesc_of(cnt - first);
-                    for (int dz = 0; dz < 3; ++dz) {
-                        tc::mbar_wait(full_bar(s), ph);
-                        tc::tc_fence_after();
-                        if constexpr (UNI) {
-                            // warp-uniform control flow: operands stay in the uniform datapath, elect.sync issues from one lane
-                            const uint32_t desc_hi = (uint32_t)(da0 >> 32);                    // == high word of db0 (same ROW_BYTES)
-                            const uint32_t a_s = (uint32_t)da0 + (uint32_t)((s * A_BYTES) >> 4);
-                            const uint32_t b_z = (uint32_t)db0 + (uint32_t)(((dz * 9 + off) * W_TAP_BYTES) >> 4);
-                            const uint32_t wrap = first < cnt ? 1u : 0u, b_wrap = (uint32_t)((first * W_TAP_BYTES) >> 4);
-                            // one (warp-uniform) branch per STAGE: the 3-output window wraps around the TMEM slot ring for 2 of 8
-                            // positions only, and the second MMA's operand set-up costs as much as the first's
-                            if (!wrap) {
-#pragma unroll
-                                for (int dy = 0; dy < 3; ++dy) {
-#pragma unroll
-                                    for (int k = 0; k < CIN / 16; ++k)
-                                        tc::umma_bf16_acc_elect_lo(d0, a_s + (uint32_t)((dy * DY_BYTES) >> 4) + 2 * k,
-                                                                   b_z + (uint32_t)((dy * 3 * W_TAP_BYTES) >> 4) + 2 * k, desc_hi, i_first);
-                                }
-                            } else {
-#pragma unroll
-                                for (int dy = 0; dy < 3; ++dy) {
-#pragma unroll
-                                    for (int k = 0; k < CIN / 16; ++k) {
-                                        const uint32_t a_lo = a_s + (uint32_t)((dy * DY_BYTES) >> 4) + 2 * k;
-                                        const uint32_t b_lo = b_z + (uint32_t)((dy * 3 * W_TAP_BYTES) >> 4) + 2 * k;
-                                        tc::umma_bf16_acc_elect_lo(d0, a_lo, b_lo, desc_hi, i_first);
-                                        tc::umma_bf16_acc_elect_lo(tmem_base, a_lo, b_lo + b_wrap, desc_hi, i_rest);
-                                    }
-                                }
-                            }
-                            __syncwarp();
-                            tc::umma_commit_elect(empty_bar(s));
-                        } else if (leader) {
-#pragma unroll
-                            for (int dy = 0; dy < 3; ++dy) {
-                                const int t9 = dz * 3 + dy;
-                                const uint64_t da = da0 + (uint64_t)((s * A_BYTES + dy * DY_BYTES) >> 4);
-                                const uint64_t db = db0 + (uint64_t)(((t9 * 3 + off) * W_TAP_BYTES) >> 4);
-#pragma unroll
-                                for (int k = 0; k < CIN / 16; ++k) {
-                                    tc::umma_bf16(d0, da + 2 * k, db + 2 * k, i_first, 1);
-                                    if (first < cnt)
-                                        tc::umma_bf16(tmem_base, da + 2 * k, db + (uint64_t)((first * W_TAP_BYTES) >> 4) + 2 * k, i_rest, 1);
-                                }
-                            }
-                            tc::umma_commit(empty_bar(s));
-                        }
-                        if (UNI) __syncwarp();
-                        if (++s == STAGES) { s = 0; ph ^= 1; }
-                    }
-                    // outputs whose last plane this was: x = p-1 (and x = X-1 on the last plane)
-                    for (int x = x_lo; x <= x_hi; ++x) {
-                        if (min(x + 1, X - 1) != p) continue;
-                        if constexpr (UNI) tc::umma_commit_elect(tfull_bar((n_base + (x - xa)) & (SLOTS - 1)));
-                        else if (leader) tc::umma_commit(tfull_bar((n_base + (x - xa)) & (SLOTS - 1)));
-                    }
-                }
-                n_base += xb - xa;
-                t += xb - xa;
-            }
-        }
-    } else {
-        const int quarter = warp & 3;
-        const uint32_t tq = tmem_base + ((uint32_t)(quarter * 32) << 16);
-        uint32_t zero[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) zero[i] = 0u;
-#pragma unroll
-        for (int sl = 0; sl < SLOTS; ++sl) tc::tmem_st32(tq + sl * COUT, zero);      // all accumulators start at zero
-        tc::tmem_st_wait();
-        tc::tc_fence_before();
-#pragma unroll
-        for (int sl = 0; sl < SLOTS; ++sl) tc::mbar_arrive(tempty_bar(sl));
-        float b[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) b[i] = __ldg(bias + i);
-        int n = 0;
-        for (int t = t_begin; t < t_end; ++t, ++n) {
-            const int x = t % X, y0 = (t / X) * TILE_Y;
-            const int slot = n & (SLOTS - 1);
-            tc::mbar_wait(tfull_bar(slot), (n / SLOTS) & 1);
-            tc::tc_fence_after();
-            uint32_t r[32];
-            tc::tmem_ld32(tq + slot * COUT, r);
-            tc::tmem_ld_wait();
-            tc::tmem_st32(tq + slot * COUT, zero);           // accumulator is in registers: re-zero and release the slot
-            tc::tmem_st_wait();
-            tc::tc_fence_before();
-            tc::mbar_arrive(tempty_bar(slot));
-            const int row = quarter * 32 + lane;
-            const int y = y0 + row / TILE_Z, z = row % TILE_Z;
-            if (y < Y) {
-                if constexpr (EPI == 0) {
-                    uint4* op = reinterpret_cast<uint4*>(out + ((((size_t)x * Y + y) * TILE_Z + z) * COUT));
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        float v[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) v[j] = fmaxf(__uint_as_float(r[8 * i + j]) + b[8 * i + j], 0.f);
-                        uint4 u;
-                        u.x = pack_bf16x2(v[0], v[1]); u.y = pack_bf16x2(v[2], v[3]);
-                        u.z = pack_bf16x2(v[4], v[5]); u.w = pack_bf16x2(v[6], v[7]);
-                        op[i] = u;
-                    }
-                } else {
-                    float4* op = reinterpret_cast<float4*>(out_f32 + ((((size_t)x * Y + y) * TILE_Z + z) * COUT));
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        float4 a = make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]), __uint_as_float(r[4 * i + 2]),
-                                               __uint_as_float(r[4 * i + 3]));
-                        if constexpr (EPI >= 2) { const float4 q = op[i]; a.x += q.x; a.y += q.y; a.z += q.z; a.w += q.w; }
-                        if constexpr (EPI == 3) {
-                            a.x = fmaxf(a.x + b[4 * i], 0.f); a.y = fmaxf(a.y + b[4 * i + 1], 0.f);
-                            a.z = fmaxf(a.z + b[4 * i + 2], 0.f); a.w = fmaxf(a.w + b[4 * i + 3], 0.f);
-                        }
-                        op[i] = a;
-                    }
-                }
-            }
-        }
+        return;
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc::tc_fence_after();
-        tc::tmem_dealloc(tmem_base, 32 * SLOTS);
+
+    const int wg = warp >> 2, wl = warp & 3;
+    const int quad_col = 2 * (lane & 3);
+    float b[8];                                              // bias of this thread's 8 output channels 8 j + quad_col + e
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { b[2 * j] = __ldg(bias + 8 * j + quad_col); b[2 * j + 1] = __ldg(bias + 8 * j + quad_col + 1); }
+    const uint64_t da0 = tc::make_smem_desc(a_base + wg * 64 * ROW_BYTES, ROW_BYTES), db0 = tc::make_smem_desc(w_base, ROW_BYTES);
+    tc::mbar_wait(w_bar, 0);
+    int s = 0; uint32_t ph = 0;
+    for (int t = t_begin; t < t_end;) {
+        const int yt = t / X, xa = t % X;
+        const int xb = min(X, xa + (t_end - t));
+        const int y0 = yt * TILE_Y;
+        float acc[48];                                       // outputs p-1 | p | p+1 of the current plane p
+#pragma unroll
+        for (int i = 0; i < 48; ++i) acc[i] = 0.f;
+        for (int p = xa - 1; p <= xb; ++p) {
+            if (p >= 0 && p < X) {                           // planes outside the volume are the zero padding
+                for (int dz = 0; dz < 3; ++dz) {
+                    tc::mbar_wait(full_bar(s), ph);
+                    const uint64_t da = da0 + (uint64_t)((s * A_BYTES) >> 4);
+                    tc::wgmma_fence();
+#pragma unroll
+                    for (int dy = 0; dy < 3; ++dy) {
+#pragma unroll
+                        for (int k = 0; k < CIN / 16; ++k)
+                            tc::wgmma_m64n96(acc, da + (uint64_t)((dy * DY_BYTES) >> 4) + 2 * k,
+                                             db0 + (uint64_t)(((dz * 3 + dy) * 3 * W_TAP_BYTES) >> 4) + 2 * k, 1);
+                    }
+                    tc::wgmma_commit();
+                    tc::wgmma_wait_all();
+                    tc::reg_fence(acc);
+                    if ((threadIdx.x & 127) == 0) tc::mbar_arrive(empty_bar(s));
+                    if (++s == STAGES) { s = 0; ph ^= 1; }
+                }
+            }
+            const int x = p - 1;                              // complete: accumulator columns [0, 32)
+            if (x >= xa) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = wg * 64 + 16 * wl + (lane >> 2) + 8 * h;
+                    const int y = y0 + row / TILE_Z, z = row % TILE_Z;
+                    if (y >= Y) continue;
+                    const size_t vox = (((size_t)x * Y + y) * TILE_Z + z) * COUT;
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const int c = 8 * j + quad_col;
+                        const float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
+                        if constexpr (EPI == 0) {
+                            *reinterpret_cast<uint32_t*>(out + vox + c) =
+                                pack_bf16x2(fmaxf(a0 + b[2 * j], 0.f), fmaxf(a1 + b[2 * j + 1], 0.f));
+                        } else {
+                            float2* op = reinterpret_cast<float2*>(out_f32 + vox + c);
+                            float2 v = make_float2(a0, a1);
+                            if constexpr (EPI >= 2) { const float2 q = *op; v.x += q.x; v.y += q.y; }
+                            if constexpr (EPI == 3) { v.x = fmaxf(v.x + b[2 * j], 0.f); v.y = fmaxf(v.y + b[2 * j + 1], 0.f); }
+                            *op = v;
+                        }
+                    }
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < 32; ++i) acc[i] = acc[i + 16];   // slide the window: p | p+1 | 0
+#pragma unroll
+            for (int i = 32; i < 48; ++i) acc[i] = 0.f;
+        }
+        t += xb - xa;
     }
 }
 
@@ -299,18 +191,12 @@ int launch_conv3d_tc_impl(const bf16* in, int in_pitch, const bf16* w_tap_major,
     const int num_sms = sm_count_current_device();
     const int tiles = X * ((Y + TILE_Y - 1) / TILE_Y);
     const int grid = tiles < num_sms ? tiles : num_sms;
-    static const bool uni = getenv("OCC_CONV_SINGLE_LANE") == nullptr;      // OCC_CONV_SINGLE_LANE=1: the lane-0-only loops (EPI 0 only)
-#define OCC_CONV_LAUNCH(C, U)                                                                                          \
-    do {                                                                                                               \
-        OCC_CUDA(cudaFuncSetAttribute(conv3d_tc_kernel<C, U, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
-        conv3d_tc_kernel<C, U, EPI><<<grid, NUM_THREADS, smem, stream>>>(tmIn, tmW, bias, out, out_f32, X, Y);         \
+#define OCC_CONV_LAUNCH(C)                                                                                          \
+    do {                                                                                                            \
+        OCC_CUDA(cudaFuncSetAttribute(conv3d_tc_kernel<C, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
+        conv3d_tc_kernel<C, EPI><<<grid, NUM_THREADS, smem, stream>>>(tmIn, tmW, bias, out, out_f32, X, Y);         \
     } while (0)
-    if constexpr (EPI == 0) {
-        if (Cin == 16) { if (uni) OCC_CONV_LAUNCH(16, true); else OCC_CONV_LAUNCH(16, false); }
-        else           { if (uni) OCC_CONV_LAUNCH(32, true); else OCC_CONV_LAUNCH(32, false); }
-    } else {
-        if (Cin == 16) OCC_CONV_LAUNCH(16, true); else OCC_CONV_LAUNCH(32, true);
-    }
+    if (Cin == 16) OCC_CONV_LAUNCH(16); else OCC_CONV_LAUNCH(32);
 #undef OCC_CONV_LAUNCH
     OCC_CUDA(cudaGetLastError());
     return 0;

@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM kernels of the voxel decoder and the occupancy / flow heads (conv3d_tc.cu, head_tc.cu)
+// wgmma implicit-GEMM kernels of the voxel decoder and the occupancy / flow heads (conv3d_tc.cu, head_tc.cu)
 #pragma once
 #include "common.cuh"
 #include "kernels.cuh"

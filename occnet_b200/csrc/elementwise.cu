@@ -151,7 +151,7 @@ layernorm256_kernel(const float* __restrict__ x, const float* __restrict__ gamma
 
 // "T32" layout of a [rows, 256] fp32 matrix used for the residual stream on the tensor-core path: 32x32 blocks,
 // inside a block [piece j = (col%32)/4][row%32][4 floats].  A thread that owns one ROW of a tile (the shape
-// tcgen05.ld produces) then reads / writes 16 bytes per instruction with the 32 lanes of a warp contiguous.
+// of the LayerNorm rows) then reads / writes 16 bytes per instruction with the 32 lanes of a warp contiguous.
 __device__ __forceinline__ int64_t t32_index(int64_t row, int col)
 {
     return ((((row >> 5) * 8 + (col >> 5)) * 8 + ((col & 31) >> 2)) * 32 + (row & 31)) * 4 + (col & 3);

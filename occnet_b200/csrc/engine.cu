@@ -51,7 +51,7 @@ struct LayerW {
     DevBuf tsa_v_wh, tsa_q_wh, tsa_o_wh, sca_q_wh, sca_v_wh, sca_o_wh, ffn1_wh, ffn2_wh;
     // self mode (prev_bev = None): W1 q + W2 (q + pos) + b == (W1 + W2) q + [W2 pos + b]; the bracket depends on parameters
     // only -> an fp32 [Nq,192] constant per layer, added by the GEMM epilogue (K = 256, weight block resident, A read once)
-    DevBuf tsa_q_wh_fold, tsa_q_const, tsa_q_const_t32;   // (_t32: the constant in the T32 block layout, TMA-store epilogue)
+    DevBuf tsa_q_wh_fold, tsa_q_const, tsa_q_const_t32;   // (_t32: the constant in the T32 block layout, read by the GEMM epilogue)
 };
 
 }  // namespace
@@ -192,7 +192,7 @@ int gemm(occb200_engine* e, const TA* A, const TA* A2, int K1, const float* W, c
     }
     if constexpr (sizeof(TA) == 4 && std::is_same<TC, float>::value) {
         // fp32 storage + tensor cores: operand split into bf16 hi/lo, weights [W_hi | W_hi | W_lo], three passes in one
-        // tcgen05 GEMM (relative error ~2^-16: fp32-grade).  The camera tokens are split once per frame.
+        // wgmma GEMM (relative error ~2^-16: fp32-grade).  The camera tokens are split once per frame.
         if (e->cfg.use_tensor_cores && e->cfg.precision == 0 && Wh != nullptr && e->split_ws.p != nullptr &&
             gemm_tc_supported(M, N, 3 * K, 2 * K)) {
             const bf16* S = e->split_ws.as<bf16>();
@@ -215,7 +215,7 @@ int gemm(occb200_engine* e, const TA* A, const TA* A2, int K1, const float* W, c
     }
 }
 
-// y = LayerNorm(A.W^T + b + residual): one tcgen05 kernel (GEMM with LayerNorm epilogue) on the tensor-core path
+// y = LayerNorm(A.W^T + b + residual): one wgmma kernel (GEMM with LayerNorm epilogue) on the tensor-core path
 int gemm_ln_fused(occb200_engine* e, const bf16* A, const void* Wh, const float* bias, const float* residual,
                   const float* gamma, const float* beta, const float* pos, float* y_f32, bf16* y_t, bf16* y_pos_t, int M,
                   int K, cudaStream_t st)
@@ -321,9 +321,8 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
     }
     // Chained dense layers (gemm_chain.cu, OCC_GEMM_CHAIN=1): [TSA output_proj+LN -> SCA sampling projection] and [SCA
     // output_proj+LN -> FFN1 -> FFN2+LN -> next layer's TSA value / sampling projections] as ONE persistent launch each: 30 launches
-    // per frame instead of 52 (13 dense-layer launches), bit-identical outputs -- and MEASURED 3 % SLOWER per frame (2.94 vs 2.86 ms,
-    // r2 call 11): every (op, n-block) switch inside the kernel re-pays the 128 KB weight load that a fresh launch pays, and the
-    // per-tile epilogues were already the bound.  Off by default.
+    // per frame instead of 52 (13 dense-layer launches), bit-identical outputs; every (op, n-block) switch inside the kernel re-pays
+    // the 128 KB weight load that a fresh launch pays.  Off by default.
     const bool use_chain = sizeof(T) == 2 && fuse_ln && q_half && e->gemm_chain && mode == MODE_FRAME && !e->value_head_major;
     static const bool tsa_merge_env0 = getenv("OCC_TSA_MERGE") == nullptr || atoi(getenv("OCC_TSA_MERGE")) != 0;
     const bool tsa_merge_ok = tsa_merge_env0;
@@ -623,7 +622,7 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
 extern "C" {
 
 const char* occb200_last_error(void) { return g_last_error.c_str(); }
-const char* occb200_version(void) { return "occ_b200 0.1 sm_100a"; }
+const char* occb200_version(void) { return "occ_b200 0.1 sm_90a"; }
 
 int occb200_ms_deform_attn_forward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
                                    const float* sampling_loc, const float* attn_weight, int B, int Nv, int M, int C,
@@ -819,7 +818,7 @@ int occb200_engine_finalize(occb200_engine* e)
                 if (gemm_simt<float, float>(e->pos.as<float>(), (int)half, nullptr, 0, (int)half, w2.as<float>(), bbuf.as<float>(),
                                             nullptr, (int)rows, fold_const->as<float>(), (int)rows, Nq, (int)rows, (int)half,
                                             ACT_NONE, 0)) return 2;
-                // the same constant in the T32 block layout (rows padded to 32) for the TMA-store epilogue of the merged launch
+                // the same constant in the T32 block layout (rows padded to 32) for the epilogue of the merged launch
                 if (rows % 32 == 0) {
                     const size_t rows_pad = ((size_t)Nq + 31) / 32 * 32;
                     if (w.tsa_q_const_t32.alloc(rows_pad * rows * 4)) return 2;
@@ -866,8 +865,8 @@ int occb200_engine_finalize(occb200_engine* e)
         const size_t hack2 = (getenv("OCC_PAIR_HACK") && atoi(getenv("OCC_PAIR_HACK")) == 2) ? 2 : 1;   // timing experiment: 128-byte token pitch
         if (e->sca_value_all.alloc((size_t)c.num_layers * c.num_cams * e->Nv * C * 2 * hack2 + 256)) return 2;   // (+ one pair over-read)
         OCC_CUDA(cudaMemset(e->sca_value_all.p, 0, e->sca_value_all.bytes));
-        // OCC_VALUE_HEADMAJOR=1: head-major value maps + pair-fetch gathers (sca_pair / tsa_pair).  MEASURED SLOWER than the
-        // row-major layout + sca_pipe / tsa_fused (SCA 1.63 vs 1.32 ms, TSA 0.31 vs 0.23 ms per frame): kept as an experiment
+        // OCC_VALUE_HEADMAJOR=1: head-major value maps + pair-fetch gathers (sca_pair / tsa_pair), an experiment next to the
+        // default row-major layout + sca_pipe / tsa_fused
         e->value_head_major = getenv("OCC_VALUE_HEADMAJOR") != nullptr;
     }
     // decoder: fold BatchNorm3d (eval) into the conv weights; torch layout [Cout][Cin][kz][ky][kx] -> [tap][Cin][Cout]
@@ -1232,7 +1231,7 @@ int occb200_layernorm_f32(const float* x, const float* gamma, const float* beta,
 int occb200_gemm_bf16_tc(const void* A, const void* W, const float* bias, float* C, int M, int N, int K, void* stream)
 {
     OCC_CHECK(A && W && C, "null pointer");
-    OCC_CHECK(gemm_tc_supported(M, N, K, K), "shape not supported by the tcgen05 GEMM");
+    OCC_CHECK(gemm_tc_supported(M, N, K, K), "shape not supported by the tensor-core GEMM");
     return gemm_tc<float>(reinterpret_cast<const bf16*>(A), nullptr, 0, reinterpret_cast<const bf16*>(W), bias, nullptr,
                           C, M, N, K, ACT_NONE, (cudaStream_t)stream);
 }

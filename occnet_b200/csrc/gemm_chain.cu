@@ -1,30 +1,28 @@
-// Chained tcgen05 GEMMs: several dense layers of the encoder in ONE persistent launch.
+// Chained wgmma GEMMs: several dense layers of the encoder in ONE persistent launch.
 //
 // Every nn.Linear of the encoder is row-wise independent (output row r depends on input row r only), and the launch-per-layer
-// schedule of gemm_tc.cu gives each of the 148 CTAs only ~2.1 tiles per launch: its kernels are start-up + a latency chain
-// (in-kernel timeline, profiles/README.md: ~4.2 us from CTA start to the first accumulator, then one epilogue per tile, then a
-// drain) and roughly a third of the dense-layer time is spent ramping up and draining.  Here a CTA keeps its row range
-// [row_begin, row_end) and walks a LIST of ops over it:
+// schedule of gemm_tc.cu gives each CTA only ~2 tiles per launch: its kernels are start-up + a latency chain, and a large share
+// of the dense-layer time is spent ramping up and draining.  Here a CTA keeps its row range [row_begin, row_end) and walks a
+// LIST of ops over it:
 //
 //     chain A (per encoder layer):  SCA output_proj + LayerNorm  ->  FFN linear 1 (ReLU)  ->  FFN linear 2 + LayerNorm
 //                                   ->  next layer's TSA value_proj  ->  next layer's TSA sampling projection
 //     chain B (per encoder layer):  TSA output_proj + LayerNorm  ->  SCA sampling projection
 //
 // (reference: custom_base_transformer_layer.py:150-165, temporal_self_attention.py:198-211,267, spatial_cross_attention.py:173,
-// 338-348).  An op whose A operand is produced by the previous op waits, per tile, on a shared-memory counter that the epilogue
+// 338-348).  An op whose A operand is produced by the previous op waits, per tile, on a shared-memory counter that the consumer
 // warps bump after their global writes of that tile are visible to the async proxy; nothing crosses CTAs, so there is no grid-wide
-// synchronisation.  The epilogue warps run back to back across op boundaries: while they drain the last tiles of op k, the
-// producer already loads op k+1's weights and first tiles and the MMA warp fills the free TMEM buffer.
+// synchronisation.  While the consumers run the epilogue of op k, the producer already loads op k+1's first tiles.
 //
-// Roles as in gemm_tc.cu: warp 0 TMA producer, warp 1 MMA issuer (tcgen05, M = 128, N = BN <= 256, accumulators double-buffered
-// in TMEM 2 x 256 columns), warps 2-9 epilogue.  Two epilogue kinds:
-//   kind 0  16-bit output (bf16 / fp16): bias (+ fp32 T32 constant) (+ ReLU) -> swizzled 2 KB staging -> TMA store [32 x 32]
-//   kind 1  fused LayerNorm (N = 256): x = acc + bias + residual written back to TMEM, row statistics exchanged between the two
-//           column-half warps, second pass normalises; fp32 residual stream (T32 layout) + bf16 operand copy (+ bf16 copy of y + pos)
+// Roles as in gemm_tc.cu: warps 0-7 two consumer warpgroups (wgmma.m64n64k16, accumulators in registers, epilogue from the
+// accumulator fragment), warps 8-11 the producer warpgroup (warp 8 issues the TMA loads).  Two epilogue kinds:
+//   kind 0  16-bit output (bf16 / fp16): bias (+ fp32 T32 constant) (+ ReLU)
+//   kind 1  fused LayerNorm (N = 256): x = acc + bias + residual, row statistics over the 4 threads of a quad; fp32 residual
+//           stream (T32 layout) + bf16 operand copy (+ bf16 copy of y + pos)
 // Weights of an n-block stay resident in shared memory when they fit next to the ring (<= 128 KB), else a W k-block travels with
 // every A stage.  N > 256 is walked as n-blocks (outer loop) x tiles (inner loop).
 #include <cstdlib>
-#include <vector>
+#include <cstring>
 
 #include "gemm_tc.cuh"
 #include "tc_common.cuh"
@@ -32,35 +30,29 @@
 namespace occ {
 
 int cached_map_2d(const void* base, uint64_t inner, uint64_t rows, uint32_t box_inner, uint32_t box_rows, CUtensorMap* out, uint64_t ld);
-int cached_map_out(const void* base, uint64_t cols, uint64_t rows, uint64_t blocks, uint32_t box_cols, CUtensorMap* out);
 
 namespace {
 
 constexpr int BLOCK_M = 128, BLOCK_K = 64, A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;
-constexpr int NUM_THREADS = 320;
+constexpr int NUM_THREADS = 384;                           // 2 consumer warpgroups + 1 producer warpgroup
 constexpr int SMEM_TOTAL = 232448;                           // 227 KB opt-in maximum
-// fixed tail at the END of the dynamic shared memory: barriers 512 B | done counters 64 B | LN partials 2 KB | constants 3 KB
-constexpr int TAIL_BYTES = 512 + 64 + 2048 + 3072;
+// fixed tail at the END of the dynamic shared memory: barriers 512 B | done counters 64 B | constants 3 KB
+constexpr int TAIL_BYTES = 512 + 64 + 3072;
 constexpr int MAX_STAGES = 6;
 
 struct ChainOp {
-    CUtensorMap tmA, tmA2, tmW, tmC, tmC2;                   // tmC: 16-bit output (LN: y_bf16), tmC2: LN's y + pos copy
+    CUtensorMap tmA, tmA2, tmW;
+    void* C;                                                 // 16-bit output [M, N] (kind 0)
     const float* bias; const float* res_t32;
     const float* residual; const float* gamma; const float* beta; const float* pos;
     float* y_f32; bf16* y_bf16; bf16* y_pos_bf16;
-    int kind;                                                // 0: 16-bit TMA-store epilogue, 1: LayerNorm epilogue
+    int kind;                                                // 0: 16-bit epilogue, 1: LayerNorm epilogue
     int N, BN, nk, nk1, act, out_half, w_resident;
     int dep;                                                 // A rows are written by the previous op of this chain
     int signal;                                              // the next op depends on this one: publish tile completions
 };
-struct ChainArgs { ChainOp op[GEMM_CHAIN_MAX_OPS]; int n_ops, M, stages, stg_bytes; };
+struct ChainArgs { ChainOp op[GEMM_CHAIN_MAX_OPS]; int n_ops, M, stages; };
 
-__device__ __forceinline__ float4 ldg_coherent(const float4* p)
-{
-    float4 v;
-    asm volatile("ld.global.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p) : "memory");
-    return v;
-}
 __device__ __forceinline__ int ld_acquire_shared(uint32_t addr)
 {
     int v;
@@ -70,18 +62,6 @@ __device__ __forceinline__ int ld_acquire_shared(uint32_t addr)
 __device__ __forceinline__ void red_release_shared_add(uint32_t addr, int v)
 {
     asm volatile("red.release.cta.shared::cta.add.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
-// at most `pending` of this thread's most recent bulk store groups are still in flight (0, 1, 2, 3, 4 or 8)
-__device__ __forceinline__ void tma_store_wait_pending(int pending)
-{
-    switch (pending) {
-    case 1: asm volatile("cp.async.bulk.wait_group 1;" ::: "memory"); break;
-    case 2: asm volatile("cp.async.bulk.wait_group 2;" ::: "memory"); break;
-    case 3: asm volatile("cp.async.bulk.wait_group 3;" ::: "memory"); break;
-    case 4: asm volatile("cp.async.bulk.wait_group 4;" ::: "memory"); break;
-    case 8: asm volatile("cp.async.bulk.wait_group 8;" ::: "memory"); break;
-    default: asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); break;
-    }
 }
 __device__ __forceinline__ void st_release_shared(uint32_t addr, int v)
 {
@@ -98,17 +78,12 @@ gemm_chain_kernel(const __grid_constant__ ChainArgs args)
     const uint32_t tail_base = (smem_end - TAIL_BYTES) & ~15u;
     const uint32_t bar_base = tail_base;                          // 512 B of mbarriers
     const uint32_t done_base = tail_base + 512;                   // int done[GEMM_CHAIN_MAX_OPS]: tiles of op i fully written
-    const uint32_t part_base = done_base + 64;                    // float2 [2][128] LayerNorm partial sums
-    const uint32_t cvec_base = part_base + 2048;                  // float [3][256] bias / gamma / beta of the current op
-    const int stages = args.stages, stg_bytes = args.stg_bytes;
-    const uint32_t stg_base = (tail_base - 8 * stg_bytes) & ~1023u;   // 8 per-warp staging blocks (1024-byte aligned: TMA swizzle)
+    const uint32_t cvec_base = done_base + 64;                    // float [3][256] bias / gamma / beta of the current op
+    const int stages = args.stages;
     auto full_bar = [&](int s) { return bar_base + s * 8; };
     auto empty_bar = [&](int s) { return bar_base + (MAX_STAGES + s) * 8; };
-    auto tfull_bar = [&](int s) { return bar_base + (2 * MAX_STAGES + s) * 8; };
-    auto tempty_bar = [&](int s) { return bar_base + (2 * MAX_STAGES + 2 + s) * 8; };
-    auto w_bar = [&](int kb) { return bar_base + (2 * MAX_STAGES + 6 + (kb < 7 ? kb : 7)) * 8; };
-    const uint32_t wfree_bar = bar_base + (2 * MAX_STAGES + 14) * 8;   // every MMA issued so far has retired (weights / ring reusable)
-    const uint32_t tmem_slot = bar_base + (2 * MAX_STAGES + 5) * 8;
+    auto w_bar = [&](int kb) { return bar_base + (2 * MAX_STAGES + (kb < 7 ? kb : 7)) * 8; };
+    const uint32_t wfree_bar = bar_base + (2 * MAX_STAGES + 8) * 8;   // every MMA of the (op, n-block) has completed
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int M = args.M;
@@ -117,27 +92,22 @@ gemm_chain_kernel(const __grid_constant__ ChainArgs args)
     const int row_end = min(M, (int)(((long long)nb32 * (blockIdx.x + 1)) / gridDim.x) << 5);
     const int n_tiles_m = (row_end - row_begin + BLOCK_M - 1) / BLOCK_M;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         for (int o = 0; o < args.n_ops; ++o) {
             tc::tma_prefetch_desc(&args.op[o].tmA); tc::tma_prefetch_desc(&args.op[o].tmW);
         }
-        for (int s = 0; s < stages; ++s) { tc::mbar_init(full_bar(s), 1); tc::mbar_init(empty_bar(s), 1); }
-        for (int s = 0; s < 2; ++s) { tc::mbar_init(tfull_bar(s), 1); tc::mbar_init(tempty_bar(s), 256); }
+        for (int s = 0; s < stages; ++s) { tc::mbar_init(full_bar(s), 1); tc::mbar_init(empty_bar(s), 2); }
         for (int kb = 0; kb < 8; ++kb) tc::mbar_init(w_bar(kb), 1);
-        tc::mbar_init(wfree_bar, 1);
+        tc::mbar_init(wfree_bar, 2);
         for (int o = 0; o < GEMM_CHAIN_MAX_OPS; ++o) st_release_shared(done_base + 4 * o, 0);
         tc::mbar_fence_init();
     }
-    if (warp == 1) tc::tmem_alloc(tmem_slot, 512);
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-    if (warp == 0) {
-        // ================================================================= TMA producer
-        if (lane == 0) {
+    if (warp >= 8) {
+        // ================================================================= TMA producer warpgroup (warp 8 issues)
+        tc::setmaxnreg_dec<40>();                                 // registers go to the consumers
+        if (warp == 8 && lane == 0) {
             int s = 0; uint32_t ph = 0; uint32_t wfree_ph = 0;
             bool first_block = true;
             asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -148,7 +118,7 @@ gemm_chain_kernel(const __grid_constant__ ChainArgs args)
                 const uint32_t stage_bytes = A_TILE_BYTES + (op.w_resident ? 0 : w_tile_bytes);
                 const uint32_t ring_base = smem_base + (op.w_resident ? nk * w_tile_bytes : 0);
                 for (int nb = 0; nb < n_blks; ++nb) {
-                    // the weight region / the re-carved ring may only be overwritten once every MMA issued so far has retired
+                    // the weight region / the re-carved ring may only be overwritten once every MMA issued so far has completed
                     if (!first_block) { tc::mbar_wait(wfree_bar, wfree_ph); wfree_ph ^= 1; }
                     first_block = false;
                     if (op.w_resident) {
@@ -165,7 +135,7 @@ gemm_chain_kernel(const __grid_constant__ ChainArgs args)
                                 __nanosleep(32);
                                 if (++spins > 50000000u) { asm volatile("trap;"); }
                             }
-                            asm volatile("fence.proxy.async;" ::: "memory");
+                            asm volatile("fence.proxy.async.global;" ::: "memory");
                         }
                         for (int kb = 0; kb < nk; ++kb) {
                             tc::mbar_wait(empty_bar(s), ph ^ 1);
@@ -181,222 +151,89 @@ gemm_chain_kernel(const __grid_constant__ ChainArgs args)
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================================================================= MMA issuer
-        if (lane == 0) {
-            int s = 0; uint32_t ph = 0; int as = 0; uint32_t aph = 0;
-            uint32_t wmask = 0;                                  // phase parity of each weight barrier (bit kb)
-            for (int o = 0; o < args.n_ops; ++o) {
-                const ChainOp& op = args.op[o];
-                const int BN = op.BN, nk = op.nk, n_blks = op.N / BN;
-                const uint32_t w_tile_bytes = BN * BLOCK_K * 2;
-                const uint32_t stage_bytes = A_TILE_BYTES + (op.w_resident ? 0 : w_tile_bytes);
-                const uint32_t ring_base = smem_base + (op.w_resident ? nk * w_tile_bytes : 0);
-                const uint32_t idesc = tc::make_idesc_bf16(BLOCK_M, BN);
-                for (int nb = 0; nb < n_blks; ++nb) {
-                    for (int t = 0; t < n_tiles_m; ++t) {
-                        tc::mbar_wait(tempty_bar(as), aph ^ 1);
-                        tc::tc_fence_after();
-                        for (int kb = 0; kb < nk; ++kb) {
-                            if (op.w_resident && t == 0) tc::mbar_wait(w_bar(kb), (wmask >> (kb < 7 ? kb : 7)) & 1u);
-                            tc::mbar_wait(full_bar(s), ph);
-                            tc::tc_fence_after();
-                            const uint32_t a_addr = ring_base + s * stage_bytes;
-                            const uint64_t da = tc::make_smem_desc(a_addr, 128);
-                            const uint64_t db = tc::make_smem_desc(op.w_resident ? smem_base + kb * w_tile_bytes : a_addr + A_TILE_BYTES, 128);
-#pragma unroll
-                            for (int k = 0; k < BLOCK_K / 16; ++k)
-                                tc::umma_bf16(tmem_base + as * 256, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-                            tc::umma_commit(empty_bar(s));
-                            if (kb == nk - 1) tc::umma_commit(tfull_bar(as));
-                            if (++s == stages) { s = 0; ph ^= 1; }
-                        }
-                        if (++as == 2) { as = 0; aph ^= 1; }
-                    }
-                    if (op.w_resident) wmask ^= (1u << (nk < 8 ? nk : 8)) - 1u;
-                    tc::umma_commit(wfree_bar);                   // arrives when every MMA of this (op, n-block) has retired
-                }
-            }
-        }
-    } else {
-        // ================================================================= epilogue warps
-        const int quarter = warp & 3;
-        const int half = (warp - 2) >> 2;
-        const int ew = warp - 2;
-        const uint32_t stg = stg_base + ew * stg_bytes;
-        float* const cvec = reinterpret_cast<float*>(smem_raw + (cvec_base - tc::smem_u32(smem_raw)));
-        float2* const part = reinterpret_cast<float2*>(smem_raw + (part_base - tc::smem_u32(smem_raw)));
-        float4* const stg4 = reinterpret_cast<float4*>(smem_raw + (stg - tc::smem_u32(smem_raw)));
-        int as = 0; uint32_t aph = 0;
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-        for (int o = 0; o < args.n_ops; ++o) {
-            const ChainOp& op = args.op[o];
-            const int BN = op.BN, n_blks = op.N / BN, N = op.N;
-            const int ncol = BN >> 1, cbeg = half * ncol;
-            const bool ln = op.kind == 1;
-            for (int nb = 0; nb < n_blks; ++nb) {
-                // per-column constants of this (op, n-block) -> shared memory (all 8 warps are past the previous block's reads)
-                asm volatile("bar.sync 5, 256;" ::: "memory");
-                {
-                    const int t = threadIdx.x - 64;
-                    if (t < BN) {
-                        cvec[t] = op.bias ? __ldg(op.bias + nb * BN + t) : 0.f;
-                        if (ln) { cvec[256 + t] = __ldg(op.gamma + t); cvec[512 + t] = __ldg(op.beta + t); }
-                    }
-                }
-                asm volatile("bar.sync 5, 256;" ::: "memory");
-                for (int t = 0; t < n_tiles_m; ++t) {
-                    const int m_row = row_begin + t * BLOCK_M;
-                    const int row0 = m_row + quarter * 32;
-                    const bool active = row0 < row_end;          // (warp-uniform; the partner column-half warp agrees)
-                    int groups = 0;                              // bulk store groups committed by lane 0 for this tile pass
-                    tc::mbar_wait(tfull_bar(as), aph);
-                    tc::tc_fence_after();
-                    const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + as * 256;
-                    if (active && ln) {
-                        const size_t blk4 = (size_t)(row0 >> 5) * 8 * 8 * 32 + lane;
-                        auto t32_load = [&](const float* base, int c0, float4 (&dst)[8], bool coherent) {
-                            const float4* p4 = reinterpret_cast<const float4*>(base) + blk4 + (size_t)(c0 >> 5) * 256;
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) dst[j] = coherent ? ldg_coherent(p4 + j * 32) : __ldg(p4 + j * 32);
-                        };
-                        float sum = 0.f, sumsq = 0.f;
-                        float4 nxt[8];
-                        t32_load(op.residual, cbeg, nxt, true);   // (may have been written earlier in THIS launch: no ld.global.nc)
-#pragma unroll
-                        for (int ci = 0; ci < 4; ++ci) {
-                            const int c0 = cbeg + ci * 32;
-                            float4 q[8];
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) q[j] = nxt[j];
-                            if (ci + 1 < 4) t32_load(op.residual, c0 + 32, nxt, true);
-                            uint32_t r[32];
-                            tc::tmem_ld32(taddr + c0, r);
-                            tc::tmem_ld_wait();
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) {
-                                const float4 b = reinterpret_cast<const float4*>(cvec + c0)[i];
-                                const float x0 = __uint_as_float(r[4 * i]) + b.x + q[i].x, x1 = __uint_as_float(r[4 * i + 1]) + b.y + q[i].y;
-                                const float x2 = __uint_as_float(r[4 * i + 2]) + b.z + q[i].z, x3 = __uint_as_float(r[4 * i + 3]) + b.w + q[i].w;
-                                sum += (x0 + x1) + (x2 + x3);
-                                sumsq = fmaf(x0, x0, fmaf(x1, x1, fmaf(x2, x2, fmaf(x3, x3, sumsq))));
-                                r[4 * i] = __float_as_uint(x0); r[4 * i + 1] = __float_as_uint(x1);
-                                r[4 * i + 2] = __float_as_uint(x2); r[4 * i + 3] = __float_as_uint(x3);
-                            }
-                            tc::tmem_st32(taddr + c0, r);
-                        }
-                        if (op.y_pos_bf16) t32_load(op.pos, cbeg, nxt, false);
-                        part[half * 128 + quarter * 32 + lane] = make_float2(sum, sumsq);
-                        tc::tmem_st_wait();
-                        asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
-                        const float2 other = part[(half ^ 1) * 128 + quarter * 32 + lane];
-                        const float mean = (sum + other.x) * (1.f / 256.f);
-                        const float var = fmaxf((sumsq + other.y) * (1.f / 256.f) - mean * mean, 0.f);
-                        const float rstd = rsqrtf(var + 1e-5f);
-#pragma unroll
-                        for (int ci = 0; ci < 4; ++ci) {
-                            const int c0 = cbeg + ci * 32;
-                            uint32_t r[32];
-                            tc::tmem_ld32(taddr + c0, r);
-                            tc::tmem_ld_wait();
-                            float4* yo = reinterpret_cast<float4*>(op.y_f32) + blk4 + (size_t)(c0 >> 5) * 256;
-                            // bf16 copies: my row -> swizzled staging ([32 rows x 64 B], SWIZZLE_64B: 16-byte piece p of row r at
-                            // p ^ ((r >> 1) & 3)) -> one TMA store per [32 x 32] block
-                            if (lane == 0) tc::tma_store_wait_read();
-                            __syncwarp();
-                            const uint32_t srow = stg + lane * 64, swz = (lane >> 1) & 3;
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                const float4 g = reinterpret_cast<const float4*>(cvec + 256 + c0)[j];
-                                const float4 be = reinterpret_cast<const float4*>(cvec + 512 + c0)[j];
-                                float4 y;
-                                y.x = (__uint_as_float(r[4 * j]) - mean) * rstd * g.x + be.x;
-                                y.y = (__uint_as_float(r[4 * j + 1]) - mean) * rstd * g.y + be.y;
-                                y.z = (__uint_as_float(r[4 * j + 2]) - mean) * rstd * g.z + be.z;
-                                y.w = (__uint_as_float(r[4 * j + 3]) - mean) * rstd * g.w + be.w;
-                                if (op.y_f32) yo[j * 32] = y;
-                                const uint32_t dst = srow + ((((uint32_t)j >> 1) ^ swz) << 4) + (j & 1) * 8;
-                                asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(dst), "r"(pack_bf16x2(y.x, y.y)), "r"(pack_bf16x2(y.z, y.w)) : "memory");
-                                if (op.y_pos_bf16) {
-                                    const float4 p4 = nxt[j];
-                                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(dst + 2048), "r"(pack_bf16x2(y.x + p4.x, y.y + p4.y)),
-                                                 "r"(pack_bf16x2(y.z + p4.z, y.w + p4.w)) : "memory");
-                                }
-                            }
-                            if (op.y_pos_bf16 && ci + 1 < 4) t32_load(op.pos, c0 + 32, nxt, false);
-                            tc::fence_proxy_async_smem();
-                            __syncwarp();
-                            if (lane == 0) {
-                                if (op.y_bf16) { tc::tma_store_3d(&op.tmC, stg, c0, row0, 0); tc::tma_store_commit(); ++groups; }
-                                if (op.y_pos_bf16) { tc::tma_store_3d(&op.tmC2, stg + 2048, c0, row0, 0); tc::tma_store_commit(); ++groups; }
-                            }
-                        }
-                    } else if (active) {
-                        // 16-bit outputs through TMA stores of [32 rows x 32 columns]
-                        for (int c0 = cbeg; c0 < cbeg + ncol; c0 += 32) {
-                            const int col = nb * BN + c0;
-                            float4 kq[8];
-                            if (op.res_t32) {
-                                const float4* p4 = reinterpret_cast<const float4*>(op.res_t32) +
-                                                   ((size_t)(row0 >> 5) * (N >> 5) + (size_t)(col >> 5)) * 256 + lane;
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) kq[j] = __ldg(p4 + j * 32);
-                            }
-                            uint32_t r[32];
-                            tc::tmem_ld32(taddr + c0, r);
-                            tc::tmem_ld_wait();
-                            uint32_t pk[16];
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                const float4 b4 = reinterpret_cast<const float4*>(cvec + c0)[j];
-                                float x0 = __uint_as_float(r[4 * j]) + b4.x, x1 = __uint_as_float(r[4 * j + 1]) + b4.y;
-                                float x2 = __uint_as_float(r[4 * j + 2]) + b4.z, x3 = __uint_as_float(r[4 * j + 3]) + b4.w;
-                                if (op.res_t32) { x0 += kq[j].x; x1 += kq[j].y; x2 += kq[j].z; x3 += kq[j].w; }
-                                if (op.act == ACT_RELU) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); x2 = fmaxf(x2, 0.f); x3 = fmaxf(x3, 0.f); }
-                                if (op.out_half) {
-                                    const __half2 a = __floats2half2_rn(x0, x1), b = __floats2half2_rn(x2, x3);
-                                    pk[2 * j] = *reinterpret_cast<const uint32_t*>(&a); pk[2 * j + 1] = *reinterpret_cast<const uint32_t*>(&b);
-                                } else {
-                                    pk[2 * j] = pack_bf16x2(x0, x1); pk[2 * j + 1] = pack_bf16x2(x2, x3);
-                                }
-                            }
-                            if (lane == 0) tc::tma_store_wait_read();
-                            __syncwarp();
-#pragma unroll
-                            for (int j = 0; j < 4; ++j)
-                                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(stg + lane * 64 + ((j ^ ((lane >> 1) & 3)) << 4)),
-                                             "r"(pk[4 * j]), "r"(pk[4 * j + 1]), "r"(pk[4 * j + 2]), "r"(pk[4 * j + 3]) : "memory");
-                            tc::fence_proxy_async_smem();
-                            __syncwarp();
-                            if (lane == 0) {
-                                tc::tma_store_3d(&op.tmC, stg, col, row0, 0);
-                                tc::tma_store_commit();
-                                ++groups;
-                            }
-                        }
-                    }
-                    tc::tc_fence_before();
-                    tc::mbar_arrive(tempty_bar(as));
-                    if (++as == 2) { as = 0; aph ^= 1; }
-                    // Tile t of this op is complete once its LAST n-block is written.  Every cross-thread dependency of a chain goes
-                    // through TMA stores (bulk groups of the issuing lane) -> TMA loads, so completion is published WITHOUT stalling
-                    // the epilogue on its own fresh stores: after tile t, wait only until the groups of the tiles before it have
-                    // completed and publish tile t-1; the last tile of the op is published after a full wait.  (A first version
-                    // fenced every tile with __threadfence: +0.17 ms per frame.)
-                    if (op.signal && nb == n_blks - 1 && lane == 0) {
-                        if (t > 0) { tma_store_wait_pending(groups); red_release_shared_add(done_base + 4 * o, 1); }
-                        if (t == n_tiles_m - 1) { tma_store_wait_pending(0); red_release_shared_add(done_base + 4 * o, 1); }
-                    }
-                }
-            }
-        }
-        if (lane == 0) tc::tma_store_wait_all();
+        return;
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc::tc_fence_after();
-        tc::tmem_dealloc(tmem_base, 512);
+
+    // ================================================================= consumer warpgroups
+    tc::setmaxnreg_inc<232>();
+    const int wg = warp >> 2, wl = warp & 3;
+    const int quad_col = 2 * (lane & 3);
+    float* const cvec = reinterpret_cast<float*>(smem_raw + (cvec_base - tc::smem_u32(smem_raw)));
+    int s = 0; uint32_t ph = 0;
+    uint32_t wmask = 0;                                          // phase parity of each weight barrier (bit kb)
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    for (int o = 0; o < args.n_ops; ++o) {
+        const ChainOp& op = args.op[o];
+        const int BN = op.BN, nk = op.nk, n_blks = op.N / BN, N = op.N;
+        const int nsubs = BN >> 6;
+        const uint32_t w_tile_bytes = BN * BLOCK_K * 2;
+        const uint32_t stage_bytes = A_TILE_BYTES + (op.w_resident ? 0 : w_tile_bytes);
+        const uint32_t ring_base = smem_base + (op.w_resident ? nk * w_tile_bytes : 0);
+        const bool ln = op.kind == 1;
+        for (int nb = 0; nb < n_blks; ++nb) {
+            // per-column constants of this (op, n-block) -> shared memory (both warpgroups are past the previous block's reads)
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            if (threadIdx.x < BN) {
+                const int t = threadIdx.x;
+                cvec[t] = op.bias ? __ldg(op.bias + nb * BN + t) : 0.f;
+                if (ln) { cvec[256 + t] = __ldg(op.gamma + t); cvec[512 + t] = __ldg(op.beta + t); }
+            }
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            for (int t = 0; t < n_tiles_m; ++t) {
+                const int m_row = row_begin + t * BLOCK_M;
+                float acc[4][32];
+                for (int kb = 0; kb < nk; ++kb) {
+                    if (op.w_resident && t == 0) tc::mbar_wait(w_bar(kb), (wmask >> (kb < 7 ? kb : 7)) & 1u);
+                    tc::mbar_wait(full_bar(s), ph);
+                    const uint32_t a_addr = ring_base + s * stage_bytes + wg * (64 * 128);
+                    const uint32_t b_addr = op.w_resident ? smem_base + kb * w_tile_bytes : ring_base + s * stage_bytes + A_TILE_BYTES;
+                    switch (nsubs) {
+                    case 4: tc::wgmma_kblock<4>(acc, a_addr, b_addr, kb == 0); break;
+                    case 3: tc::wgmma_kblock<3>(acc, a_addr, b_addr, kb == 0); break;
+                    case 2: tc::wgmma_kblock<2>(acc, a_addr, b_addr, kb == 0); break;
+                    default: tc::wgmma_kblock<1>(acc, a_addr, b_addr, kb == 0); break;
+                    }
+                    if ((threadIdx.x & 127) == 0) tc::mbar_arrive(empty_bar(s));
+                    if (++s == stages) { s = 0; ph ^= 1; }
+                }
+                // last tile of this (op, n-block): the weights and the ring may be recarved
+                if (t == n_tiles_m - 1 && (threadIdx.x & 127) == 0) tc::mbar_arrive(wfree_bar);
+                const int r0 = m_row + wg * 64 + wl * 16 + (lane >> 2);
+                if (ln) {
+                    tc::ln_epilogue(acc, r0, row_end, quad_col, cvec, op.residual, op.pos, op.y_f32, op.y_bf16, op.y_pos_bf16);
+                } else {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = r0 + 8 * h;
+                        if (row >= row_end) continue;
+#pragma unroll
+                        for (int ns = 0; ns < 4; ++ns) {
+                            if (ns >= nsubs) break;
+#pragma unroll
+                            for (int j = 0; j < 8; ++j) {
+                                const int col = nb * BN + ns * 64 + 8 * j + quad_col, cl = col - nb * BN;
+                                float x0 = acc[ns][4 * j + 2 * h] + cvec[cl], x1 = acc[ns][4 * j + 2 * h + 1] + cvec[cl + 1];
+                                if (op.res_t32) {
+                                    const float2 q = __ldg(reinterpret_cast<const float2*>(op.res_t32 + tc::t32_index(row, col, N)));
+                                    x0 += q.x; x1 += q.y;
+                                }
+                                if (op.act == ACT_RELU) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                                *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(op.C) + (size_t)row * N + col) =
+                                    tc::pack_16(x0, x1, op.out_half != 0);
+                            }
+                        }
+                    }
+                }
+                // Tile t of this op is complete once its LAST n-block is written: make this thread's global writes visible to
+                // the async proxy (the producer's TMA loads of the next op), then one arrival per warp (8 per tile)
+                if (op.signal && nb == n_blks - 1) {
+                    asm volatile("fence.proxy.async.global;" ::: "memory");
+                    __syncwarp();
+                    if (lane == 0) red_release_shared_add(done_base + 4 * o, 1);
+                }
+            }
+            if (op.w_resident) wmask ^= (1u << (nk < 8 ? nk : 8)) - 1u;
+        }
     }
 }
 
@@ -409,10 +246,7 @@ int gemm_chain_launch(const GemmChainOp* ops, int n_ops, int M, cudaStream_t str
     ChainArgs a;
     memset(&a, 0, sizeof(a));
     a.n_ops = n_ops; a.M = M;
-    bool any_pos = false;
-    for (int i = 0; i < n_ops; ++i) any_pos = any_pos || (ops[i].ln && ops[i].y_pos_bf16 != nullptr);
-    a.stg_bytes = any_pos ? 4096 : 2048;                      // LN staging: [0,2K) y, [2K,4K) y + pos
-    const int avail = SMEM_TOTAL - 1024 - TAIL_BYTES - 16 - 8 * a.stg_bytes - 1024;
+    const int avail = SMEM_TOTAL - 1024 - TAIL_BYTES - 16;
     int stages = MAX_STAGES;
     for (int i = 0; i < n_ops; ++i) {
         const GemmChainOp& g = ops[i];
@@ -434,16 +268,13 @@ int gemm_chain_launch(const GemmChainOp* ops, int n_ops, int M, cudaStream_t str
         if (g.A2) { if (cached_map_2d(g.A2, (uint64_t)(g.K - g.K1), (uint64_t)M, BLOCK_K, BLOCK_M, &o.tmA2, 0)) return 1; }
         else o.tmA2 = o.tmA;
         if (cached_map_2d(g.W, (uint64_t)g.K, (uint64_t)g.N, BLOCK_K, (uint32_t)BN, &o.tmW, 0)) return 1;
-        o.tmC = o.tmW; o.tmC2 = o.tmW;
         if (!g.ln) {
             OCC_CHECK(g.C != nullptr, "gemm_chain: output pointer");
-            if (cached_map_out(g.C, (uint64_t)g.N, (uint64_t)M, 1, 32u, &o.tmC)) return 1;
         } else {
             OCC_CHECK(g.bias && g.residual && g.gamma && g.beta && g.y_f32, "gemm_chain: LayerNorm op needs bias, residual, gamma, beta, y_f32");
             OCC_CHECK(g.y_pos_bf16 == nullptr || g.pos != nullptr, "gemm_chain: pos required for y_pos");
-            if (g.y_bf16 && cached_map_out(g.y_bf16, 256, (uint64_t)M, 1, 32u, &o.tmC)) return 1;
-            if (g.y_pos_bf16 && cached_map_out(g.y_pos_bf16, 256, (uint64_t)M, 1, 32u, &o.tmC2)) return 1;
         }
+        o.C = g.C;
         o.signal = (i + 1 < n_ops && ops[i + 1].dep) ? 1 : 0;
         o.bias = g.bias; o.res_t32 = g.res_t32; o.residual = g.residual; o.gamma = g.gamma; o.beta = g.beta; o.pos = g.pos;
         o.y_f32 = g.y_f32; o.y_bf16 = g.y_bf16; o.y_pos_bf16 = g.y_pos_bf16;

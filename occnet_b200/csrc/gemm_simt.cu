@@ -2,7 +2,7 @@
 //   C[M,N] = act(A[M,K] . W[N,K]^T + bias[N]) (+ residual[M,N])
 // Every dense layer of the path is an nn.Linear (weight [N,K], K contiguous), reference:
 //   temporal_self_attention.py:99-104, spatial_cross_attention.py:245-249,:67, mmcv FFN.
-// fp32 accumulation; A may be fp32 or bf16, C fp32 or bf16.  The tensor-core (tcgen05) path
+// fp32 accumulation; A may be fp32 or bf16, C fp32 or bf16.  The tensor-core (wgmma) path
 // in gemm_tc.cu replaces this for the bf16 configurations.
 #include "common.cuh"
 

@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA bf16 GEMM (gemm_tc.cu):  C[M,N] = act(A[M,K] . W[N,K]^T + bias) (+ residual)
+// wgmma / TMA bf16 GEMM (gemm_tc.cu):  C[M,N] = act(A[M,K] . W[N,K]^T + bias) (+ residual)
 #pragma once
 #include "common.cuh"
 

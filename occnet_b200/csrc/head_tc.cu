@@ -1,18 +1,15 @@
-// Occupancy + flow heads on the tensor cores (sm_100a).  Reference: TransformerOcc.predicter /
+// Occupancy + flow heads on the tensor cores (sm_90a).  Reference: TransformerOcc.predicter /
 // flow_predicter (transformer_occ.py:132-141, applied :318-319) and BEVFormerOccHead.get_occ
 // (bevformer_occ_head.py:211-212; argmax of the logits == argmax of their softmax).
 //
-// Per 128-voxel tile, a chain of two tcgen05 GEMMs with the activations kept on chip:
-//   GEMM1  [128 x 32] . [32 x 128]   hidden = [ predicter.0 | flow_predicter.0 ]        -> TMEM cols [0,128)
-//   epilogue A: +bias, Softplus (cols 0-63) / ReLU (cols 64-127), bf16, written back to shared memory in the
-//               128B-swizzled K-major layout the tensor core reads (generic-proxy stores + fence.proxy.async)
-//   GEMM2  [128 x 128] . [128 x 32]  block-diagonal [ predicter.2 (17) ; flow_predicter.2 (2) ; 0-pad ]
-//                                                                                        -> TMEM cols [128,160)
-//   epilogue B: +bias, argmax over the 17 classes, coalesced stores of logits / class / flow via shared memory
-// Two tiles are in flight (TMEM and the hidden buffer are double-buffered): GEMM1 of tile i+1 is issued
-// before GEMM2 of tile i, and the 8 epilogue warps run epilogue A of tile i+1 BEFORE epilogue B of tile i, so the
-// MUFU-heavy activation pass never waits for GEMM2.  Warp (quarter q, half h) owns TMEM lanes 32q..32q+31 and the
-// hidden columns [32h, 32h+32) (Softplus) + [64+32h, 64+32h+32) (ReLU); the half-0 warps also run epilogue B.
+// Per 128-voxel tile, a chain of two wgmma GEMMs with the activations kept on chip.  Each of the two consumer warpgroups owns
+// 64 voxels of the tile:
+//   GEMM1  [64 x 32] . [32 x 128]   hidden = [ predicter.0 | flow_predicter.0 ]          (registers)
+//   epilogue A: +bias, Softplus (cols 0-63) / ReLU (cols 64-127), bf16, written to the warpgroup's shared-memory buffer in
+//               the 128B-swizzled K-major layout the tensor core reads (generic-proxy stores + fence.proxy.async)
+//   GEMM2  [64 x 128] . [128 x 32]  block-diagonal [ predicter.2 (17) ; flow_predicter.2 (2) ; 0-pad ]
+//   epilogue B: +bias, argmax over the 17 classes (reduced over the 4 threads of a quad), logits / class / flow
+// Warp 8 streams the voxel tiles through a 4-stage TMA ring; the weights stay resident.
 #include "common.cuh"
 #include "conv3d_tc.cuh"
 #include "tc_common.cuh"
@@ -25,42 +22,25 @@ constexpr int A_STAGES = 4, BLOCK_M = 128, HID = 128, NOUT = 32;
 constexpr int A_BYTES = BLOCK_M * 64;                 // 128 rows x 32 bf16
 constexpr int W1_BYTES = HID * 64;                    // 128 rows x 32 bf16
 constexpr int W2_CHUNK_BYTES = NOUT * 128;            // 32 rows x 64 bf16
-constexpr int H_CHUNK_BYTES = BLOCK_M * 128;          // 128 rows x 64 bf16
-constexpr int NUM_THREADS = 320;                     // TMA warp, MMA warp, 8 epilogue warps
+constexpr int H_CHUNK_BYTES = 64 * 128;               // 64 rows x 64 bf16 (one warpgroup)
+constexpr int NUM_THREADS = 288;                     // 2 consumer warpgroups + 1 TMA warp
 constexpr int MAX_CLS = 19;                           // 17 classes + 2 flow channels live in the 32 GEMM2 columns
 
-// Softplus of TWO hidden units with ONE MUFU op each: softplus(x) = max(x, 0) + log1p(t), t = exp(-|x|) in (0, 1], and
-// log1p(t) = t * P(t) with a degree-5 minimax polynomial (|P - log1p(t)/t| <= 7.2e-6 on [0,1], so the result is within 7.2e-6
-// RELATIVE of softplus everywhere -- the hidden activations are then rounded to bf16, 2^-9).  The polynomial runs on the packed
-// fp32x2 FMA of sm_100 (fma.rn.f32x2: two lanes per issue slot).  The previous form log(1 + exp(x)) needed ex2 AND lg2: the kernel
-// issued 820 M MUFU ops per frame and was bound by that pipe (profiles/README.md).
-__device__ __forceinline__ unsigned long long pack2(float a, float b)
-{
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-    return r;
-}
-__device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c)
-{
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
-}
-__device__ __forceinline__ void softplus2(float x0, float x1, float& y0, float& y1)
+// Softplus with ONE MUFU op: softplus(x) = max(x, 0) + log1p(t), t = exp(-|x|) in (0, 1], and log1p(t) = t * P(t) with a degree-5
+// minimax polynomial (|P - log1p(t)/t| <= 7.2e-6 on [0,1], so the result is within 7.2e-6 RELATIVE of softplus everywhere -- the
+// hidden activations are then rounded to bf16, 2^-9).  The form log(1 + exp(x)) needs ex2 AND lg2 and is bound by the MUFU pipe.
+__device__ __forceinline__ float softplus1(float x)
 {
     constexpr float C0 = 0.9999929070472717f, C1 = -0.4994262754917145f, C2 = 0.32572421431541443f, C3 = -0.211494579911232f,
                     C4 = 0.10287206619977951f, C5 = -0.024528255686163902f;
-    float t0, t1;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(t0) : "f"(-fabsf(x0) * 1.4426950408889634f));
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(t1) : "f"(-fabsf(x1) * 1.4426950408889634f));
-    const unsigned long long t = pack2(t0, t1);
-    unsigned long long p = fma2(pack2(C5, C5), t, pack2(C4, C4));
-    p = fma2(p, t, pack2(C3, C3));
-    p = fma2(p, t, pack2(C2, C2));
-    p = fma2(p, t, pack2(C1, C1));
-    p = fma2(p, t, pack2(C0, C0));
-    const unsigned long long y = fma2(t, p, pack2(fmaxf(x0, 0.f), fmaxf(x1, 0.f)));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(y0), "=f"(y1) : "l"(y));
+    float t;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(-fabsf(x) * 1.4426950408889634f));
+    float p = fmaf(C5, t, C4);
+    p = fmaf(p, t, C3);
+    p = fmaf(p, t, C2);
+    p = fmaf(p, t, C1);
+    p = fmaf(p, t, C0);
+    return fmaf(t, p, fmaxf(x, 0.f));
 }
 
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -75,45 +55,30 @@ head_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const uint32_t w1_base = smem_base;                                  // 8 KB
     const uint32_t w2_base = w1_base + W1_BYTES;                         // 2 x 4 KB
     const uint32_t a_base = w2_base + 2 * W2_CHUNK_BYTES;                // 4 x 8 KB
-    const uint32_t h_base = a_base + A_STAGES * A_BYTES;                 // 2 stages x 2 chunks x 16 KB
-    const uint32_t stage_out = h_base + 4 * H_CHUNK_BYTES;               // 4 warps x 32 x 19 floats
-    const uint32_t bias_base = stage_out + 4 * 32 * MAX_CLS * 4;         // 128 + 32 floats: b1cat | b2cat
+    const uint32_t h_base = a_base + A_STAGES * A_BYTES;                 // 2 warpgroups x 2 chunks x 8 KB
+    const uint32_t bias_base = h_base + 4 * H_CHUNK_BYTES;               // 128 + 32 floats: b1cat | b2cat
     const uint32_t bar_base = bias_base + (HID + NOUT) * 4 + 64;
     auto a_full = [&](int s) { return bar_base + s * 8; };
     auto a_empty = [&](int s) { return bar_base + (A_STAGES + s) * 8; };
-    auto h1_full = [&](int s) { return bar_base + (2 * A_STAGES + s) * 8; };      // GEMM1 done
-    auto h_ready = [&](int s) { return bar_base + (2 * A_STAGES + 2 + s) * 8; };  // hidden tile written
-    auto l_full = [&](int s) { return bar_base + (2 * A_STAGES + 4 + s) * 8; };   // GEMM2 done
-    auto t_empty = [&](int s) { return bar_base + (2 * A_STAGES + 6 + s) * 8; };  // TMEM stage drained
-    const uint32_t w_bar = bar_base + (2 * A_STAGES + 8) * 8;
-    const uint32_t tmem_slot = bar_base + (2 * A_STAGES + 9) * 8;
+    const uint32_t w_bar = bar_base + (2 * A_STAGES) * 8;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int num_tiles = (int)((nvox + BLOCK_M - 1) / BLOCK_M);
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tc::tma_prefetch_desc(&tmA); tc::tma_prefetch_desc(&tmW1); tc::tma_prefetch_desc(&tmW2);
-        for (int s = 0; s < A_STAGES; ++s) { tc::mbar_init(a_full(s), 1); tc::mbar_init(a_empty(s), 1); }
-        for (int s = 0; s < 2; ++s) {
-            tc::mbar_init(h1_full(s), 1); tc::mbar_init(h_ready(s), 256);
-            tc::mbar_init(l_full(s), 1); tc::mbar_init(t_empty(s), 128);
-        }
+        for (int s = 0; s < A_STAGES; ++s) { tc::mbar_init(a_full(s), 1); tc::mbar_init(a_empty(s), 2); }
         tc::mbar_init(w_bar, 1);
         tc::mbar_fence_init();
     }
-    if (warp == 1) tc::tmem_alloc(tmem_slot, 512);
     float* const sbias = reinterpret_cast<float*>(smem_gen + (bias_base - smem_base));
-    if (threadIdx.x >= 64 && threadIdx.x < 64 + HID + NOUT) {
-        const int t = threadIdx.x - 64;
+    if (threadIdx.x < HID + NOUT) {
+        const int t = threadIdx.x;
         sbias[t] = t < HID ? __ldg(b1cat + t) : (t - HID < ncls + 2 ? __ldg(b2cat + t - HID) : 0.f);
     }
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             tc::mbar_arrive_expect_tx(w_bar, W1_BYTES + 2 * W2_CHUNK_BYTES);
             tc::tma_load_2d(w1_base, &tmW1, w_bar, 0, 0);
@@ -127,134 +92,88 @@ head_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 if (++s == A_STAGES) { s = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc1 = tc::make_idesc_bf16(BLOCK_M, HID), idesc2 = tc::make_idesc_bf16(BLOCK_M, NOUT);
-            tc::mbar_wait(w_bar, 0);
-            tc::tc_fence_after();
-            int s = 0; uint32_t ph = 0;
-            int n_my = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) ++n_my;
-            for (int i = 0; i <= n_my; ++i) {
-                if (i < n_my) {                                           // GEMM1 of tile i
-                    const int as = i & 1; const uint32_t aph = (i >> 1) & 1;
-                    tc::mbar_wait(t_empty(as), aph ^ 1);
-                    tc::mbar_wait(a_full(s), ph);
-                    tc::tc_fence_after();
-                    const uint64_t da = tc::make_smem_desc(a_base + s * A_BYTES, 64);
-                    const uint64_t db = tc::make_smem_desc(w1_base, 64);
+        return;
+    }
+
+    const int wg = warp >> 2, wl = warp & 3;
+    const int quad_col = 2 * (lane & 3);
+    const uint32_t hbuf = h_base + wg * 2 * H_CHUNK_BYTES;
+    tc::mbar_wait(w_bar, 0);
+    int s = 0; uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        // ---- GEMM1: hidden = A . W1cat^T (K = 32: two K = 16 steps inside the 64-byte swizzle atom)
+        float hid[64];
+        tc::mbar_wait(a_full(s), ph);
+        {
+            const uint64_t da = tc::make_smem_desc(a_base + s * A_BYTES + wg * (64 * 64), 64);
+            const uint64_t db = tc::make_smem_desc(w1_base, 64);
+            tc::wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < 2; ++k)
-                        tc::umma_bf16(tmem_base + as * 256, da + 2 * k, db + 2 * k, idesc1, k != 0);
-                    tc::umma_commit(a_empty(s));
-                    tc::umma_commit(h1_full(as));
-                    if (++s == A_STAGES) { s = 0; ph ^= 1; }
-                }
-                if (i >= 1) {                                             // GEMM2 of tile i-1
-                    const int j = i - 1, as = j & 1; const uint32_t aph = (j >> 1) & 1;
-                    tc::mbar_wait(h_ready(as), aph);
-                    tc::tc_fence_after();
+            for (int k = 0; k < 2; ++k) tc::wgmma_m64n128(hid, da + 2 * k, db + 2 * k, k != 0);
+            tc::wgmma_commit();
+            tc::wgmma_wait_all();
+            tc::reg_fence(hid);
+        }
+        if ((threadIdx.x & 127) == 0) tc::mbar_arrive(a_empty(s));
+        if (++s == A_STAGES) { s = 0; ph ^= 1; }
+        // ---- epilogue A: activations -> bf16 -> swizzled K-major A operand of GEMM2 (chunk c = hidden columns [64c, 64c+64))
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // the previous tile's GEMM2 is done with the buffer
 #pragma unroll
-                    for (int c = 0; c < 2; ++c) {
-                        const uint64_t da = tc::make_smem_desc(h_base + (as * 2 + c) * H_CHUNK_BYTES, 128);
-                        const uint64_t db = tc::make_smem_desc(w2_base + c * W2_CHUNK_BYTES, 128);
+        for (int j = 0; j < 16; ++j) {
 #pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            tc::umma_bf16(tmem_base + as * 256 + 128, da + 2 * k, db + 2 * k, idesc2, (c | k) != 0);
-                    }
-                    tc::umma_commit(l_full(as));
-                }
+            for (int h = 0; h < 2; ++h) {
+                const int col = 8 * j + quad_col, row = 16 * wl + (lane >> 2) + 8 * h;
+                const float x0 = hid[4 * j + 2 * h] + sbias[col], x1 = hid[4 * j + 2 * h + 1] + sbias[col + 1];
+                const float v0 = j < 8 ? softplus1(x0) : fmaxf(x0, 0.f), v1 = j < 8 ? softplus1(x1) : fmaxf(x1, 0.f);
+                const uint32_t addr = hbuf + (j >> 3) * H_CHUNK_BYTES + row * 128 + (((j & 7) ^ (row & 7)) << 4) + quad_col * 2;
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_bf16x2(v0, v1)) : "memory");
             }
         }
-    } else {
-        const int quarter = warp & 3, half = (warp - 2) >> 2;
-        const int row = quarter * 32 + lane;
-        float* sout = reinterpret_cast<float*>(smem_gen + (stage_out - smem_base)) + quarter * 32 * MAX_CLS;
-        int n_my = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) ++n_my;
-        // ---- epilogue A of my tile #i: hidden activations -> swizzled bf16 A operand of GEMM2 in shared memory
-        auto epi_a = [&](int i) {
-            const int as = i & 1; const uint32_t aph = (i >> 1) & 1;
-            const uint32_t tbase = tmem_base + ((uint32_t)(quarter * 32) << 16) + as * 256;
-            tc::mbar_wait(h1_full(as), aph);
-            tc::tc_fence_after();
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic-proxy writes -> visible to wgmma
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+        // ---- GEMM2: logits = hidden . W2cat^T (K = 128: two 64-column chunks of four K = 16 steps)
+        float lg[16];
+        tc::wgmma_fence();
 #pragma unroll
-            for (int part = 0; part < 2; ++part) {
-                const int c0 = part * 64 + half * 32;                     // part 0: Softplus columns, part 1: ReLU columns
-                uint32_t r[32];
-                tc::tmem_ld32(tbase + c0, r);
-                tc::tmem_ld_wait();
-                const uint32_t chunk_base = h_base + (as * 2 + part) * H_CHUNK_BYTES + row * 128;
+        for (int c = 0; c < 2; ++c) {
+            const uint64_t da = tc::make_smem_desc(hbuf + c * H_CHUNK_BYTES, 128);
+            const uint64_t db = tc::make_smem_desc(w2_base + c * W2_CHUNK_BYTES, 128);
 #pragma unroll
-                for (int p = 0; p < 4; ++p) {                             // 4 x 16 bytes = 8 hidden units each
-                    float v[8];
-                    const float4 b0 = reinterpret_cast<const float4*>(sbias + c0)[2 * p];
-                    const float4 b1 = reinterpret_cast<const float4*>(sbias + c0)[2 * p + 1];
-                    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+            for (int k = 0; k < 4; ++k) tc::wgmma_m64n32(lg, da + 2 * k, db + 2 * k, (c | k) != 0);
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait_all();
+        tc::reg_fence(lg);
+        // ---- epilogue B: +bias, logits, argmax (first maximum, as torch.argmax), flow
 #pragma unroll
-                    for (int k = 0; k < 8; k += 2) {
-                        const float x0 = __uint_as_float(r[p * 8 + k]) + bb[k], x1 = __uint_as_float(r[p * 8 + k + 1]) + bb[k + 1];
-                        if (part == 0) softplus2(x0, x1, v[k], v[k + 1]);
-                        else { v[k] = fmaxf(x0, 0.f); v[k + 1] = fmaxf(x1, 0.f); }
+        for (int h = 0; h < 2; ++h) {
+            const int64_t v = (int64_t)tile * BLOCK_M + wg * 64 + 16 * wl + (lane >> 2) + 8 * h;
+            float best = -INFINITY; int arg = 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int c = 8 * j + quad_col + e;
+                    const float a = lg[4 * j + 2 * h + e] + sbias[HID + c];
+                    if (c < ncls) {
+                        if (a > best) { best = a; arg = c; }
+                        if (occ_logits && v < nvox) occ_logits[v * ncls + c] = a;
+                    } else if (c < ncls + 2 && flow && v < nvox) {
+                        flow[v * 2 + (c - ncls)] = a;
                     }
-                    const int piece = half * 4 + p;                       // 16-byte piece index inside the 128 B row
-                    const uint32_t addr = chunk_base + ((piece ^ (row & 7)) << 4);
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(pack_bf16x2(v[0], v[1])),
-                                 "r"(pack_bf16x2(v[2], v[3])), "r"(pack_bf16x2(v[4], v[5])), "r"(pack_bf16x2(v[6], v[7]))
-                                 : "memory");
                 }
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to UMMA
-            tc::tc_fence_before();
-            tc::mbar_arrive(h_ready(as));
-        };
-        // ---- epilogue B of my tile #i (half-0 warps): logits / class / flow
-        auto epi_b = [&](int i, int tile) {
-            const int as = i & 1; const uint32_t aph = (i >> 1) & 1;
-            const uint32_t tbase = tmem_base + ((uint32_t)(quarter * 32) << 16) + as * 256;
-            tc::mbar_wait(l_full(as), aph);
-            tc::tc_fence_after();
-            uint32_t r[32];
-            tc::tmem_ld32(tbase + 128, r);
-            tc::tmem_ld_wait();
-            tc::tc_fence_before();
-            tc::mbar_arrive(t_empty(as));
-            const int64_t v0 = (int64_t)tile * BLOCK_M + quarter * 32;    // first voxel of this warp
-            float best = -INFINITY, f0 = 0.f, f1 = 0.f; int arg = 0;
 #pragma unroll
-            for (int c = 0; c < MAX_CLS; ++c) {                           // static register indices (no local memory)
-                const float a = __uint_as_float(r[c]) + sbias[HID + c];
-                if (c < ncls) {
-                    sout[lane * MAX_CLS + c] = a;
-                    if (a > best) { best = a; arg = c; }
-                } else if (c == ncls) f0 = a;
-                else if (c == ncls + 1) f1 = a;
+            for (int d = 1; d <= 2; d <<= 1) {
+                const float ob = __shfl_xor_sync(0xffffffffu, best, d);
+                const int oa = __shfl_xor_sync(0xffffffffu, arg, d);
+                if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
             }
-            const int64_t v = v0 + lane;
-            if (v < nvox) {
+            if ((lane & 3) == 0 && v < nvox) {
                 if (cls_u8) cls_u8[v] = (uint8_t)arg;
                 if (cls_i64) cls_i64[v] = arg;
-                if (flow) *reinterpret_cast<float2*>(flow + v * 2) = make_float2(f0, f1);
             }
-            if (occ_logits) {
-                __syncwarp();
-                const int64_t nvalid = (nvox - v0 < 32 ? nvox - v0 : 32);
-                float* dst = occ_logits + v0 * ncls;
-                for (int j = lane; j < nvalid * ncls; j += 32) dst[j] = sout[(j / ncls) * MAX_CLS + (j % ncls)];
-                __syncwarp();
-            }
-        };
-        if (n_my > 0) epi_a(0);
-        for (int i = 0; i < n_my; ++i) {
-            if (i + 1 < n_my) epi_a(i + 1);
-            if (half == 0) epi_b(i, blockIdx.x + i * (int)gridDim.x);
         }
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc::tc_fence_after();
-        tc::tmem_dealloc(tmem_base, 512);
     }
 }
 
@@ -264,7 +183,7 @@ int launch_occ_head_tc(const bf16* vox, const bf16* w1cat, const bf16* w2cat, co
                        int ncls, int64_t nvox, float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64,
                        cudaStream_t stream)
 {
-    OCC_CHECK(ncls + 2 <= NOUT && ncls + 2 <= MAX_CLS, "occ_head_tc: at most 17 classes");
+    OCC_CHECK(ncls + 2 <= MAX_CLS, "occ_head_tc: at most 17 classes");
     CUtensorMap tmA, tmW1, tmW2;
     {
         const uint64_t dims[2] = {32, (uint64_t)nvox}, strides[1] = {64};
@@ -281,8 +200,7 @@ int launch_occ_head_tc(const bf16* vox, const bf16* w1cat, const bf16* w2cat, co
         const uint32_t box[2] = {64, NOUT};
         if (make_tensor_map_bf16(&tmW2, w2cat, 2, dims, strides, box, 128)) return 1;
     }
-    const int smem = 1024 + W1_BYTES + 2 * W2_CHUNK_BYTES + A_STAGES * A_BYTES + 4 * H_CHUNK_BYTES +
-                     4 * 32 * MAX_CLS * 4 + (HID + NOUT) * 4 + 64 + 256;
+    const int smem = 1024 + W1_BYTES + 2 * W2_CHUNK_BYTES + A_STAGES * A_BYTES + 4 * H_CHUNK_BYTES + (HID + NOUT) * 4 + 64 + 256;
     const int num_sms = sm_count_current_device();
     const int tiles = (int)((nvox + BLOCK_M - 1) / BLOCK_M);
     const int grid = tiles < num_sms ? tiles : num_sms;

@@ -1,4 +1,4 @@
-// Multi-scale deformable attention for sm_100a: the operator-boundary kernel (mmcv `_ext` ABI
+// Multi-scale deformable attention for sm_90a: the operator-boundary kernel (mmcv `_ext` ABI
 // semantics) and the two fused BEVFormer variants.
 //
 //   msda_forward_kernel  <- mmcv._ext.ms_deform_attn_forward, called from
@@ -21,8 +21,8 @@
 //        memory; the gather loop reads them with one broadcast LDS.128 per sample and issues the
 //        loads of sample i+1 before the FMAs of sample i.  4 warps per CTA, 6 CTAs per SM.
 // Sampling offsets / logits arrive as fp32 or (tensor-core path) fp16.
-// Measured bound (ncu, profiles/README.md): the L1 data path -- every 128-bit warp load touches 6-8
-// different 128-byte lines and replays once per line -- not HBM (11 % dram) or instruction issue (50 %).
+// Design bound: the L1 data path -- every 128-bit warp load touches 6-8 different 128-byte lines and replays once per
+// line -- rather than HBM or instruction issue.
 #include <cuda_fp16.h>
 
 #include <cstdlib>
@@ -93,15 +93,11 @@ __device__ __forceinline__ SamplePrep prep_sample(float h_im, float w_im, float 
     return s;
 }
 
-// acc(2 lanes) += a * w using the packed fp32x2 FMA of sm_100
+// acc(2 lanes) += a * w  (two round-to-nearest FMAs)
 __device__ __forceinline__ void ffma2(float2& acc, float a0, float a1, float w)
 {
-    unsigned long long d = *reinterpret_cast<unsigned long long*>(&acc);
-    const float2 av = make_float2(a0, a1), wv = make_float2(w, w);
-    asm("fma.rn.f32x2 %0, %1, %2, %0;"
-        : "+l"(d)
-        : "l"(*reinterpret_cast<const unsigned long long*>(&av)), "l"(*reinterpret_cast<const unsigned long long*>(&wv)));
-    acc = *reinterpret_cast<float2*>(&d);
+    acc.x = fmaf(a0, w, acc.x);
+    acc.y = fmaf(a1, w, acc.y);
 }
 
 template <typename T>
@@ -121,20 +117,16 @@ __device__ __forceinline__ void gather_sample(const T* __restrict__ base, int W,
     }
 }
 
-// ---- bf16 value path: Blackwell's mixed-precision FMA (PTX fma.rn.f32.bf16 -> SASS FHFMA.BF16) multiplies two bf16
-// operands exactly and accumulates in fp32, and it can read either 16-bit half of a register: the bf16 -> fp32
-// unpack disappears.  The four corner weights travel as two packed bf16 pairs (3 shuffles per sample, not 5).
+// ---- bf16 value path: the product of two bf16 operands is exact in fp32, so unpacking both halves (a shift / a mask) and one
+// fp32 FMA gives the mixed-precision multiply-add bit for bit.  The four corner weights travel as two packed bf16 pairs
+// (3 shuffles per sample, not 5).
 __device__ __forceinline__ float fhfma_lo(float acc, uint32_t v, uint32_t w_lo16)
 {
-    const unsigned short a = (unsigned short)(v & 0xffffu), b = (unsigned short)(w_lo16 & 0xffffu);
-    asm("fma.rn.f32.bf16 %0, %1, %2, %0;" : "+f"(acc) : "h"(a), "h"(b));
-    return acc;
+    return fmaf(__uint_as_float(v << 16), __uint_as_float(w_lo16 << 16), acc);
 }
 __device__ __forceinline__ float fhfma_hi(float acc, uint32_t v, uint32_t w_lo16)
 {
-    const unsigned short a = (unsigned short)(v >> 16), b = (unsigned short)(w_lo16 & 0xffffu);
-    asm("fma.rn.f32.bf16 %0, %1, %2, %0;" : "+f"(acc) : "h"(a), "h"(b));
-    return acc;
+    return fmaf(__uint_as_float(v & 0xffff0000u), __uint_as_float(w_lo16 << 16), acc);
 }
 __device__ __forceinline__ void fma_word4(float (&acc)[8], const uint4& v, uint32_t w)
 {
@@ -143,7 +135,7 @@ __device__ __forceinline__ void fma_word4(float (&acc)[8], const uint4& v, uint3
     acc[4] = fhfma_lo(acc[4], v.z, w); acc[5] = fhfma_hi(acc[5], v.z, w);
     acc[6] = fhfma_lo(acc[6], v.w, w); acc[7] = fhfma_hi(acc[7], v.w, w);
 }
-// accumulator abstraction: bf16 values -> float[8] + FHFMA; fp32 values -> float2[4] + FFMA2
+// accumulator abstraction: bf16 values -> float[8]; fp32 values -> float2[4]
 template <typename T> struct Acc;
 template <> struct Acc<bf16> {
     float a[8];
@@ -387,8 +379,8 @@ sca_pipe_kernel(const bf16* __restrict__ value, const QT* __restrict__ qproj, Sc
 }
 
 // ------------------------------------------------------------------------------------------
-// SM-tiled persistent variant (EXPERIMENT, off by default: measured slower, see launch_sca_fused).  Hypothesis: the gather is
-// bound by L2 -> L1 traffic (ncu, linear mapping: 1.48 GB per launch over the crossbar at 6.5 TB/s, L1 hit rate 47 %, DRAM 8 %):
+// SM-tiled persistent variant (EXPERIMENT, off by default, see launch_sca_fused).  Hypothesis: the gather is
+// bound by L2 -> L1 traffic:
 // neighbouring BEV queries project onto overlapping image regions, but consecutive CTAs of a linear grid land on DIFFERENT SMs,
 // so the 24 warps resident on an SM work on 6 unrelated strips.
 // Here every SM works on ONE compact BEV tile (TW x TH = 8 x 3 queries = 6 units of 4 x-consecutive queries) at a time:
@@ -400,7 +392,6 @@ sca_pipe_kernel(const bf16* __restrict__ value, const QT* __restrict__ qproj, Sc
 //        otherwise                        -> another CTA of this SM is fetching: retry
 //     All-zero words (one cudaMemsetAsync per launch) are the initial state.  Balance is dynamic at tile granularity and no
 //     assumption is made about which / how many CTAs the hardware places on an SM.
-//   * tools/dev/sca_l1_sim.py (LRU model of the bench geometry): L2 -> L1 bytes 1.16 GB -> 0.5-0.6 GB per launch.
 constexpr int SCA_TILE_W = 8, SCA_TILE_H = 3, SCA_TILE_UNITS = (SCA_TILE_W / 4) * SCA_TILE_H;
 constexpr unsigned SCA_TILE_DONE = 0xffffu;
 
@@ -457,13 +448,13 @@ sca_tile_kernel(const bf16* __restrict__ value, const QT* __restrict__ qproj, Sc
 }
 
 // ------------------------------------------------------------------------------------------
-// Pair-fetch variant of the production gather (head-major value maps, written by the value_proj GEMM's TMA-store epilogue):
+// Pair-fetch variant of the production gather (head-major value maps, written by the value_proj GEMM's head-major epilogue):
 //   value_hm [8 heads][T = num_cams * Nv tokens][32] bf16 -- one 64-byte row per (head, token), so the two x-neighbours of a
 //   bilinear sample are ADJACENT: 8 lanes fetch the 128 contiguous bytes {left pixel | right pixel} of one (head, row) with
 //   one 128-bit load each, and a warp instruction covers 4 heads x 128 B.  A sample costs 2 such instructions per head group
 //   (upper row, lower row) instead of 4 corner instructions of 8 x 64 B: the same bytes in half as many 128-byte lines when
 //   the pair is line-aligned (even token), three quarters on average -- the row-major layout touched one line per (head,
-//   corner), and the kernel is bound by L1 lines per request (profiles/README.md).
+//   corner), and the kernel is bound by L1 lines per request.
 //   Lane map in phase 2: hl = lane / 8 (head within the group of 4), j = lane % 8: side = j / 4 (left / right pixel),
 //   slice = j % 4 (8 channels).  Two head groups -> 2 x 8 accumulators per lane; left and right partial sums are combined
 //   with one shuffle per accumulator at the end.  Phase 1 (descriptors) is the row-major kernel's.
@@ -930,9 +921,9 @@ static int num_sms_here()                                            // per devi
 {
     static int cache[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     if (cache[dev] == 0) cudaDeviceGetAttribute(&cache[dev], cudaDevAttrMultiProcessorCount, dev);
-    return cache[dev] > 0 ? cache[dev] : 148;
+    return cache[dev] > 0 ? cache[dev] : 132;
 }
 
 template <typename T>
@@ -946,11 +937,9 @@ int launch_sca_fused(const T* value, const void* qproj_v, bool q_half, const Sca
     const dim3 grid(ceil_div(Nq, 8));
     if constexpr (sizeof(T) == 2) {
         // production bf16 kernel: descriptor-staged gather, 4 warps per CTA, 6 CTAs per SM (OCC_SCA_PIPE=0: the
-        // shuffle-broadcast kernel that is also the fp32 path; measured variants: profiles/README.md)
+        // shuffle-broadcast kernel that is also the fp32 path)
         static const int pipe = getenv("OCC_SCA_PIPE") ? atoi(getenv("OCC_SCA_PIPE")) : 416;
-        // OCC_SCA_TILED=6|5: the SM-tiled persistent kernel (6 / 5 CTAs per SM).  MEASURED SLOWER than the linear mapping although it
-        // does what it was built for (ncu, r2 calls 5-6: L1 hit rate 47 -> 64 %, L2->L1 bytes 1.48 -> 1.03 GB, shared-memory
-        // wavefronts -44 %): 268-282 us vs 225 us per launch -- the gather is not bound by L2->L1 bytes (profiles/README.md).
+        // OCC_SCA_TILED=6|5: the SM-tiled persistent kernel (6 / 5 CTAs per SM), an experiment next to the linear mapping
         static const int tiled = getenv("OCC_SCA_TILED") ? atoi(getenv("OCC_SCA_TILED")) : 0;
         if (tiled && sched != nullptr && sp.bev_w % 4 == 0) {
             // SM-tiled persistent kernel: one word per SM (indexed by %smid, < SCA_SCHED_WORDS - 1) + the global tile counter
@@ -1012,7 +1001,7 @@ int launch_sca_pair(const bf16* value_hm, const void* qproj_v, bool q_half, cons
     const int Nq = sp.bev_h * sp.bev_w;
     const long long T = (long long)sp.num_cams * Nv;
     // 6 CTAs/SM caps the kernel at 80 registers (a few spills outside the gather loop); OCC_SCA_PAIR_MINB=5 trades occupancy
-    // for none (measured variants: profiles/README.md)
+    // for none
     static const int minb = getenv("OCC_SCA_PAIR_MINB") ? atoi(getenv("OCC_SCA_PAIR_MINB")) : 6;
     static const int hack = getenv("OCC_PAIR_HACK") ? atoi(getenv("OCC_PAIR_HACK")) : 0;     // timing experiments only
     if (q_half) {

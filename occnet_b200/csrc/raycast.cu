@@ -1,4 +1,4 @@
-// Ray-casting metric for sm_100a (SURVEY rows a14 / a15).
+// Ray-casting metric for sm_90a (SURVEY rows a14 / a15).
 //   render_forward_kernel <- tools/ray_iou/lib/dvr/dvr.cu:69-319 ("test" phase) + host wrapper :329-388
 //   ray_metric_kernel     <- datasets/ray_metrics.py process_one_sample :89-143 + calc_metrics :146-189
 // The traversal arithmetic is double precision with the reference's comparison order, so voxel

@@ -18,7 +18,7 @@ Everything here is a behavioural restatement of the published mmcv 1.x / mmdet 2
 semantics (parameter names, init rules, forward arithmetic), written from scratch.
 `install_as_mmcv()` additionally registers these objects under the `mmcv.*` / `mmdet.*`
 module names; only `tests/golden/gen_golden.py` uses that, to import the *unmodified*
-reference modules from /root/reference and pin the oracle against them.
+reference modules from the reference tree and pin the oracle against them.
 """
 from __future__ import annotations
 

@@ -12,7 +12,7 @@ configured by projects/configs/bevformer/bevformer_base_occ.py:48-66:
     img_neck     = FPN(in_channels=[512,1024,2048], out_channels=256, start_level=0,
                        add_extra_convs='on_output', num_outs=4, relu_before_extra_convs=True)
 
-Both are THIRD-PARTY mmdet modules (mmdet is absent from /root/reference; BEVFormer's install page pins
+Both are THIRD-PARTY mmdet modules (mmdet is absent from the reference tree; BEVFormer's install page pins
 mmdet 2.14.0), so the algorithm is restated from its published form:
 
   * ResNet-50, bottleneck blocks, style='pytorch' (the stride-2 convolution is the 3x3 one, i.e. torchvision's

@@ -2,18 +2,17 @@
 
 Plain-torch CPU restatement of the reference's camera->occupancy hot path, function by
 function (SURVEY section 8a rows a1-a13).  Each function cites the reference lines it
-follows (paths relative to /root/reference/projects/mmdet3d_plugin/bevformer/).  All
+follows (paths relative to projects/mmdet3d_plugin/bevformer/ of the reference tree).  All
 arithmetic is fp32, eval mode (dropout = identity, BatchNorm uses running statistics).
 
 Parameters travel in a flat dict keyed exactly like the reference's
 `pts_bbox_head.state_dict()` (e.g. 'transformer.encoder.layers.0.attentions.1.output_proj.weight'),
 so a reference checkpoint can be fed to the oracle and to the CUDA path unchanged.
 
-Third-party pieces restated from their published semantics (absent from /root/reference):
+Third-party pieces restated from their published semantics (absent from the reference tree):
 mmcv FFN / LayerNorm / ConvModule, mmdet LearnedPositionalEncoding, mmcv MSDA (oracle/msda.py).
 
-Parity status: pinned against the UNMODIFIED reference modules imported in this container
-through an mmcv stand-in (tests/golden/gen_golden.py -> tests/golden/ref_*.npz); the
+Parity status: pinned against the UNMODIFIED reference modules, imported through an mmcv stand-in (tests/golden/gen_golden.py -> tests/golden/ref_*.npz); the
 reference itself ships no golden vectors, so there is no upstream pin beyond that.
 """
 import math

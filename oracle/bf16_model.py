@@ -2,7 +2,7 @@
 
 Storage-rounding restatement of the reference's camera->occupancy hot path: the SAME algorithm as
 `oracle/bevformer_occ.py` (which follows the reference file by file), with every tensor that the
-B200 bf16 / tcgen05 configuration keeps in 16 bits rounded at exactly those storage points
+bf16 / tensor-core configuration keeps in 16 bits rounded at exactly those storage points
 (DESIGN.md section 3), and fp32 everywhere else.  It exists so that the parity test of the
 throughput configuration can use a tight tolerance: against the fp32 oracle that configuration can
 only be held to ~1e-2 (8-bit mantissas), which would hide real bugs; against this model the only

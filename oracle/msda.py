@@ -1,7 +1,7 @@
 """ORACLE (test infrastructure only -- never imported by the product path).
 
 CPU restatement of the multi-scale deformable attention operator that the reference
-reaches through `mmcv` (third-party, NOT vendored under /root/reference, version
+reaches through `mmcv` (third-party, NOT vendored in the reference tree, version
 unpinned by the repo; BEVFormer's install page names mmcv-full 1.4.0):
 
   * `mmcv.ops.multi_scale_deform_attn.multi_scale_deformable_attn_pytorch`

@@ -1,7 +1,7 @@
 /* ORACLE (test infrastructure only -- never linked into the product library).
  *
  * Plain-C restatement of the reference's ray-casting kernel in "test" phase:
- *   /root/reference/tools/ray_iou/lib/dvr/dvr.cu:69-319  (render_forward_cuda_kernel)
+ *   tools/ray_iou/lib/dvr/dvr.cu:69-319 of the reference tree  (render_forward_cuda_kernel)
  *   host wrapper dvr.cu:329-388 (outputs pre-filled with -1 / 0)
  * One call == one `dvr.render_forward(sigma, origin, points, tindex, grid, "test")`
  * with N == 1.  All traversal arithmetic is double, exactly as in the kernel; inputs
@@ -13,7 +13,7 @@
  * cannot change the result) but the walk still continues to the exit so that `d[count-1]`
  * (the no-hit answer) and the MAX_STEP cut-off behave identically.
  *
- * Parity status: validated on the GPU box against the reference kernel itself
+ * Parity status: validated on the GPU against the reference kernel itself
  * (oracle/_ref/dvr_ref*.so, built from the reference sources by oracle/build_ref.py).
  */
 #include <float.h>

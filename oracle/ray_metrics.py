@@ -1,13 +1,13 @@
 """ORACLE (test infrastructure only -- never imported by the product path).
 
 Restatement of the reference's Ray-mIoU / mAVE metric (SURVEY rows a14, a15):
-  /root/reference/projects/mmdet3d_plugin/datasets/ray_metrics.py
+  projects/mmdet3d_plugin/datasets/ray_metrics.py (reference tree)
      generate_lidar_rays :63-86, process_one_sample :89-143, calc_metrics :146-197, main :200-257
 The voxel traversal is the C restatement in oracle/ray_dda.c (of tools/ray_iou/lib/dvr/dvr.cu:69-319).
 
-Parity status: python logic pinned against the unmodified reference functions imported in this
-container (tests/golden/gen_golden.py -> tests/golden/ref_metric.npz); DDA pinned on the GPU box
-against the reference kernel (oracle/_ref).
+Parity status: python logic pinned against the unmodified reference functions
+(tests/golden/gen_golden.py -> tests/golden/ref_metric.npz); DDA pinned on the GPU against the
+reference kernel's outputs (tests/golden/ref_dvr.npz, and oracle/_ref when it is built).
 """
 import ctypes
 import math

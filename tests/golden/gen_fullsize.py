@@ -62,7 +62,9 @@ def pack_outputs(out, d):
         d[k + '_shape'] = np.asarray(out[k].shape)
     cls = out['occ'].argmax(-1)[0].numpy().astype(np.uint8)
     d['occ_cls'] = cls
-    d['flow_f16'] = out['flow'][0].numpy().astype(np.float16)
+    # the metric reads the reference flow only at voxels whose class carries flow (ray_metrics.py:26-29, 178-185): stored there
+    flow = out['flow'][0].numpy()
+    d['flow_f16'] = np.where(cls[..., None] < ORM.FLOW_CLASSES, flow, 0).astype(np.float16)
     d['counters'], fin = ray_counters(cls, out['flow'][0].numpy())
     d['miou'], d['mave'] = fin['miou'], fin['mave']
     return fin

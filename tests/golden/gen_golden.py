@@ -1,16 +1,15 @@
-"""Generate tests/golden/ref_*.npz by running the UNMODIFIED reference modules in this container.
+"""Generate tests/golden/ref_*.npz by running the UNMODIFIED reference modules.
 
-The reference's hot-path modules (`/root/reference/projects/mmdet3d_plugin/bevformer/...`) import
+The reference's hot-path modules (`projects/mmdet3d_plugin/bevformer/...` of the reference tree) import
 mmcv / mmdet at module scope; those are absent here, so `occnet_b200.mmcv_shim.install_as_mmcv()`
 provides stand-ins for the third-party pieces (registries, BaseModule, FFN, ConvModule,
 LearnedPositionalEncoding, `multi_scale_deformable_attn_pytorch` restated in oracle/msda.py).
 Everything else -- BEVFormerEncoder.point_sampling, SpatialCrossAttention's rebatch loops,
 TemporalSelfAttention, MSDeformableAttention3D, TransformerOcc, BEVFormerOccHead, and the metric's
 generate_lidar_rays / process_one_sample / calc_metrics -- is the reference's own code, executed
-from where it lies.  The outputs are committed as small fixtures; /root/reference does not exist
-on the GPU box, so nothing else reads it at test time.
+from where it lies.  The outputs are committed as small fixtures, so nothing reads the reference tree at test time.
 
-Run (CPU, ~1 min):  python tests/golden/gen_golden.py
+Run (CPU, ~1 min):  OCC_REFERENCE_ROOT=<reference tree> python tests/golden/gen_golden.py
 """
 import importlib
 import os
@@ -22,7 +21,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF = '/root/reference'
+REF = os.environ['OCC_REFERENCE_ROOT']
 OUT = os.path.join(ROOT, 'tests', 'golden')
 
 from occnet_b200 import fixtures, mmcv_shim          # noqa: E402

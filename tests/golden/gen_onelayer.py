@@ -1,11 +1,11 @@
-"""One-encoder-layer goldens at FULL size (6 cams, 200x200 BEV, 200x200x16 voxels) for the bf16 / tcgen05 configuration.
+"""One-encoder-layer goldens at FULL size (6 cams, 200x200 BEV, 200x200x16 voxels) for the bf16 / tensor-core configuration.
 
     python tests/golden/gen_onelayer.py          # ~20 s; writes full1_bf16.npz, full1_prev_bf16.npz
 
 Why: over SIX layers the bf16 path is chaotic in the rounding sense -- a 1-ulp difference in an fp32 accumulation order flips a
 bf16 rounding somewhere, and that flip propagates as bf16-sized noise -- so against the storage-rounding model
-(oracle/bf16_model.py) a six-layer engine run can only agree to about the model's own distance from the fp32 oracle
-(measured: 2.0e-2 max / 2.9e-3 mean, profiles/r2_parity_report.json).  After ONE layer few roundings have happened, so the
+(oracle/bf16_model.py) a six-layer engine run can only agree to about the model's own distance from the fp32 oracle.
+After ONE layer few roundings have happened, so the
 same comparison is tight and a wrong constant / index / layout in the fused path cannot hide behind the 6e-2 bar.
 Both files hold seeded subsamples (tests/golden/sampling.py) of bev_embed / occ / flow from the fp32 oracle AND the model.
 """
@@ -23,9 +23,7 @@ sys.path.insert(0, HERE)
 from occnet_b200 import fixtures                    # noqa: E402
 from oracle import bevformer_occ as O               # noqa: E402
 from oracle import bf16_model as B                  # noqa: E402
-from sampling import sub_idx                        # noqa: E402
-
-N1 = 40000
+from sampling import N1, sub_idx                    # noqa: E402
 
 
 def case(prev):

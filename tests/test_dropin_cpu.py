@@ -1,4 +1,5 @@
 """CPU suite: the drop-in surface (config loading, registries, state_dict key contract) and the data-parallel host logic."""
+import json
 import os
 import subprocess
 import sys
@@ -11,7 +12,13 @@ from occnet_b200 import fixtures
 from occnet_b200.mmcv_shim import Config, build_detector, build_head
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_CFG = '/root/reference/projects/configs/bevformer/bevformer_base_occ.py'
+# the shipped config (projects/configs/bevformer/bevformer_base_occ.py with its `_base_` files) as Config.fromfile merges it:
+# plugin, model and dist_params, stored by tests/golden/gen_config.py
+CFG_GOLDEN = os.path.join(ROOT, 'tests', 'golden', 'ref_config_base_occ.json')
+
+
+def shipped_config():
+    return Config(json.load(open(CFG_GOLDEN)), filename=CFG_GOLDEN)
 
 
 head_cfg = fixtures.head_cfg          # registry config of the head for a fixture geometry (shared with bench.py)
@@ -28,12 +35,11 @@ def test_plugin_state_dict_keys_equal_reference(golden_dir):
     head.load_state_dict(fixtures.init_params(cfg, seed=2), strict=True)
 
 
-@pytest.mark.skipif(not os.path.exists(REF_CFG), reason='reference tree not present (GPU box)')
 def test_shipped_config_loads_and_builds_unchanged():
     import projects.mmdet3d_plugin  # noqa: F401
-    cfg = Config.fromfile(REF_CFG)
+    cfg = shipped_config()
     assert cfg.plugin and cfg.plugin_dir == 'projects/mmdet3d_plugin/'
-    assert cfg.model.type == 'BEVFormerOcc' and cfg.dist_params.backend == 'nccl'          # `_base_` merge works
+    assert cfg.model.type == 'BEVFormerOcc' and cfg.dist_params.backend == 'nccl'          # from the `_base_` files
     assert cfg.model.pts_bbox_head.transformer.encoder.num_layers == 4
     det = build_detector(cfg.model)
     head = det.pts_bbox_head
@@ -45,7 +51,18 @@ def test_shipped_config_loads_and_builds_unchanged():
         head([torch.zeros(1, 6, 256, h, w) for h, w in fixtures.CFG_FULL['level_shapes']], fixtures.make_img_metas(fixtures.CFG_FULL))
 
 
-@pytest.mark.skipif(not os.path.exists(REF_CFG), reason='reference tree not present (GPU box)')
+def test_config_fromfile_merges_base_files(tmp_path):
+    """Config.fromfile's `_base_` inheritance (mmcv semantics): nested dicts merge key by key, the child wins, `_delete_`
+    replaces a dict, lists are replaced whole."""
+    (tmp_path / 'base.py').write_text("model = dict(type='A', head=dict(n=1, m=2), opt=dict(lr=1))\nlayers = [1, 2]\nname = 'base'\n")
+    (tmp_path / 'child.py').write_text("_base_ = ['./base.py']\nmodel = dict(head=dict(n=3), opt=dict(_delete_=True, wd=5))\n"
+                                       "layers = [7]\n")
+    cfg = Config.fromfile(str(tmp_path / 'child.py'))
+    assert cfg.model.type == 'A' and cfg.model.head.n == 3 and cfg.model.head.m == 2
+    assert dict(cfg.model.opt) == {'wd': 5}
+    assert list(cfg.layers) == [7] and cfg.name == 'base'
+
+
 def test_backbone_neck_containers_have_reference_keys():
     """img_backbone / img_neck of the shipped config build as parameter containers whose keys are the reference's
     (mmdet ResNet == torchvision resnet50 minus fc; mmdet FPN lateral_convs / fpn_convs) and accept the oracle's
@@ -53,7 +70,7 @@ def test_backbone_neck_containers_have_reference_keys():
     import projects.mmdet3d_plugin  # noqa: F401
     from torchvision.models import resnet50
     from oracle import backbone as OB
-    det = build_detector(Config.fromfile(REF_CFG).model)
+    det = build_detector(shipped_config().model)
     sd = det.state_dict()
     bk = {k[len('img_backbone.'):] for k in sd if k.startswith('img_backbone.')}
     assert bk == {k for k in resnet50(weights=None).state_dict() if not k.startswith('fc.')}
