@@ -88,6 +88,7 @@ struct GemmProb {
     CUtensorMap tmA, tmA2, tmW;
     const float* bias; const float* residual; void* C;
     const float* res_t32;                                     // optional fp32 epilogue constant [M,N] in the T32 block layout
+                                                              // (never together with residual: the epilogue loads one of them)
     long long ldc, nblk_stride;                               // C offset of (row, column c of n-block b): b * nblk_stride + row * ldc + c
     int head_major;                                           // value maps [n-block][column/32][M][32] (one 64-byte row per (head, token))
     int M, N, BN, nk, nk1, act, w_resident, stages;
@@ -206,33 +207,50 @@ gemm_tc_kernel(const __grid_constant__ GemmProbs probs, LnArgs ln)
         if constexpr (LN) {
             tc::ln_epilogue(acc, r0, row_end, quad_col, cvec, residual, ln.pos, ln.y_f32, ln.y_bf16, ln.y_pos_bf16);
         } else {
+            // Column cl = ns * 64 + 8 j + quad_col lies in 32-column block 2 ns + j / 4 at offset 8 (j % 4) + quad_col, so every
+            // address below is a per-row base plus a compile-time multiple of a per-launch stride.  The fp32 epilogue operand
+            // (res_t32 or residual, never both) of a row is loaded in full before its first use: the loads are in flight
+            // together instead of one latency per column pair.  Per element the arithmetic is unchanged.
+            const bool has_t32 = res_t32 != nullptr, has_res = residual != nullptr, relu = act == ACT_RELU;
+            const float* __restrict__ qsrc = has_t32 ? res_t32 : residual;
+            const int q_blk = has_t32 ? 1024 : 32, q_j = has_t32 ? 256 : 8;           // operand offset per 32 / per 8 columns
+            const size_t o_blk = P.head_major ? (size_t)M * 32 : 32;                 // output offset per 32 columns
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = r0 + 8 * h;
                 if (row >= row_end) continue;
+                const float* const qrow =
+                    qsrc + (has_t32 ? ((((size_t)(row >> 5) * (N >> 5) + n_blk * (BN >> 5)) * 256 + (quad_col >> 2) * 32 + (row & 31)) << 2) +
+                                          (quad_col & 3)
+                                    : (size_t)row * N + n_blk * BN + quad_col);
+                float2 q[4][8];
+                if (qsrc) {
+#pragma unroll
+                    for (int ns = 0; ns < 4; ++ns) {
+                        if (ns >= nsubs) break;
+#pragma unroll
+                        for (int j = 0; j < 8; ++j)
+                            q[ns][j] = __ldg(reinterpret_cast<const float2*>(qrow + (2 * ns + j / 4) * q_blk + (j & 3) * q_j));
+                    }
+                }
+                TC* const orow = reinterpret_cast<TC*>(P.C) +
+                                 (P.head_major ? ((size_t)n_blk * (BN >> 5) * M + row) * 32 + quad_col
+                                               : (size_t)n_blk * P.nblk_stride + (size_t)row * P.ldc + quad_col);
 #pragma unroll
                 for (int ns = 0; ns < 4; ++ns) {
                     if (ns >= nsubs) break;
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
-                        const int cl = ns * 64 + 8 * j + quad_col, col = n_blk * BN + cl;
+                        const int cl = ns * 64 + 8 * j + quad_col;
                         float x0 = acc[ns][4 * j + 2 * h] + cvec[cl], x1 = acc[ns][4 * j + 2 * h + 1] + cvec[cl + 1];
-                        if (res_t32) {
-                            const float2 q = __ldg(reinterpret_cast<const float2*>(res_t32 + tc::t32_index(row, col, N)));
-                            x0 += q.x; x1 += q.y;
-                        }
-                        if (act == ACT_RELU) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-                        if (residual) {
-                            const float2 q = __ldg(reinterpret_cast<const float2*>(residual + (size_t)row * N + col));
-                            x0 += q.x; x1 += q.y;
-                        }
-                        const size_t o = P.head_major
-                                             ? ((size_t)(n_blk * (BN >> 5) + (cl >> 5)) * M + row) * 32 + (cl & 31)
-                                             : (size_t)n_blk * P.nblk_stride + (size_t)row * P.ldc + cl;
+                        if (has_t32) { x0 += q[ns][j].x; x1 += q[ns][j].y; }
+                        if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                        if (has_res) { x0 += q[ns][j].x; x1 += q[ns][j].y; }
+                        TC* const o = orow + (2 * ns + j / 4) * o_blk + 8 * (j & 3);
                         if constexpr (sizeof(TC) == 4)
-                            *reinterpret_cast<float2*>(reinterpret_cast<float*>(P.C) + o) = make_float2(x0, x1);
+                            *reinterpret_cast<float2*>(o) = make_float2(x0, x1);
                         else
-                            *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(P.C) + o) = tc::pack_16(x0, x1, out_half);
+                            *reinterpret_cast<uint32_t*>(o) = tc::pack_16(x0, x1, out_half);
                     }
                 }
             }
