@@ -57,6 +57,7 @@ int occb200_ms_deform_attn_backward(const float* value, const int64_t* spatial_s
  * spatial cross-attention, FFN), the Conv3d voxel decoder and the occupancy / flow heads.
  */
 typedef struct occb200_engine occb200_engine;
+typedef struct occb200_backbone occb200_backbone;   /* image backbone + neck, declared below */
 
 typedef struct occb200_config {
     int bev_h, bev_w;              /* BEV grid (200 x 200)                     bevformer_base_occ.py:41-42   */
@@ -106,8 +107,18 @@ int occb200_engine_set_prev_rotation(occb200_engine* e, const int32_t* map_host)
 /* Element type / layout of the feature levels handed to _forward / _forward_host / _submit_host from now on (pointers
  * travel through the same arguments): 0 = fp32 [num_cams, C, h, w] (default, the reference's), 1 = bf16, same layout
  * (half the PCIe bytes for host pipelines that hold bf16 features), 2 = bf16 channels-last [num_cams, h, w, C] -- the
- * native output of occb200_backbone_forward_nhwc_bf16, so images -> voxels never leaves the device or transposes. */
+ * native output of occb200_backbone_forward_nhwc_bf16, so images -> voxels never leaves the device or transposes.
+ * 3 = uint8 camera frames: feats[0] is the frame buffer [num_cams, src_h, src_w, 3] of the attached backbone's frame format
+ * (occb200_engine_attach_backbone) and feats[1..3] are ignored; a device pointer for _forward, a host pointer for
+ * _forward_host / _submit_host.  The backbone runs first, on the same stream; with both precisions bf16 its FPN writes
+ * channels-last bf16 levels into engine-owned buffers (code 2's hand-over), otherwise fp32 NCHW levels.  The backbone's
+ * workspace and those level buffers are shared by both _submit_host slots: every frame records an event after its last read
+ * of them and the next frame's backbone waits for it, so switching streams between submits stays correct.
+ * occb200_engine_launches_per_frame then counts the backbone's kernels too. */
 int occb200_engine_set_input_dtype(occb200_engine* e, int feats_bf16);
+/* Borrowed; NULL detaches.  bb must be finalized, with num_images == num_cams, level shapes equal to the engine's, and a
+ * frame format set.  It must outlive the engine's use of it (detach before destroying it). */
+int occb200_engine_attach_backbone(occb200_engine* e, occb200_backbone* bb);
 
 /* One frame, DEVICE buffers.
  *   feats[l]   dev f32 [num_cams, C, h_l, w_l]  (FPN outputs of one batch item, NCHW)
@@ -144,7 +155,8 @@ int occb200_engine_copy_tap(occb200_engine* e, int which, int layer, float* dst_
 
 /* Row a2 on its own: reference_points_cam dev f32 [num_cams, Nq, D, 2], bev_mask dev u8 [num_cams, Nq, D]. */
 int occb200_engine_project_pillars(occb200_engine* e, float* ref_cam, uint8_t* mask, void* stream);
-/* number of kernels one forward launches (for the benchmark's gpu_launches claim) */
+/* number of kernels one forward launches (for the benchmark's gpu_launches claim); with input dtype 3 (camera frames) the
+ * attached backbone's kernels are included */
 int occb200_engine_launches_per_frame(const occb200_engine* e);
 /* Per-kernel-category device timing with CUDA events on the launch stream (benchmark roofline).
  * Categories: 0 pack/prepare, 1 dense GEMM, 2 TSA gather, 3 SCA gather, 4 LayerNorm, 5 bev->voxel, 6 conv3d,
@@ -196,7 +208,6 @@ int occb200_gemm_bf16_tc(const void* A_bf16, const void* W_bf16, const float* bi
  *   running_mean", "img_neck.lateral_convs.0.conv.bias", ... (HOST fp32; `num_batches_tracked` is not a parameter).
  *   forward: img dev f32 [num_images, 3, H, W] (mean/std-normalised, padded) -> out_l dev f32 [num_images, 256, h_l, w_l]
  *   (any out may be NULL), the layout `extract_img_feat` hands to the head after its view(B, N, C, h, w). */
-typedef struct occb200_backbone occb200_backbone;
 occb200_backbone* occb200_backbone_create(int num_images, int img_h, int img_w, int precision, int use_tensor_cores);
 void occb200_backbone_destroy(occb200_backbone* e);
 int occb200_backbone_load_param(occb200_backbone* e, const char* key, const float* data, int64_t numel);
@@ -208,6 +219,19 @@ int occb200_backbone_forward(occb200_backbone* e, const float* img, float* out0,
  * the last convolutions (no NCHW fp32 copy): the layout occb200_engine_set_input_dtype(e, 2) consumes. */
 int occb200_backbone_forward_nhwc_bf16(occb200_backbone* e, const float* img, void* out0, void* out1, void* out2, void* out3,
                                        void* stream);
+/* Camera frames as the loader produces them: uint8 [num_images, src_h, src_w, 3] (mmcv.imread order, BGR), normalised
+ * (to_rgb swap first, then (x - mean[c]) * (1/std[c]) in fp32) and padded bottom/right with 0 to the backbone's H x W
+ * inside the stem (NormalizeMultiviewImage + PadMultiViewImage + DefaultFormatBundle3D). src_h <= H, src_w <= W, std != 0.
+ * mean / std are indexed in the order of the normalised channels (RGB when to_rgb); 1/std is rounded from double, as
+ * mmcv.imnormalize computes it.  Host-side, synchronous; the stem of forward_frames then writes the same im2col operand
+ * that _forward writes from the fp32 images the host pipeline would produce, so the outputs are bit-identical to it. */
+int occb200_backbone_set_frame_format(occb200_backbone* e, int src_h, int src_w, const float mean[3], const float std[3],
+                                      int to_rgb);
+/* frames: dev u8 [num_images, src_h, src_w, 3] contiguous (16-byte aligned rows are read with vector loads).
+ * out_layout 0: fp32 NCHW (as occb200_backbone_forward, any out may be NULL); 1: bf16 channels-last (as _forward_nhwc_bf16,
+ * precision 1 only).  Without a frame format set, or with an out-of-range argument, it returns an error and launches nothing. */
+int occb200_backbone_forward_frames(occb200_backbone* e, const uint8_t* frames, void* out0, void* out1, void* out2,
+                                    void* out3, int out_layout, void* stream);
 
 #ifdef __cplusplus
 }

@@ -33,6 +33,7 @@ SIGNATURES = {
     'occb200_engine_finalize': (_i, [_vp]),
     'occb200_engine_set_cameras': (_i, [_vp, _vp, _vp, _i, _i]),
     'occb200_engine_set_input_dtype': (_i, [_vp, _i]),
+    'occb200_engine_attach_backbone': (_i, [_vp, _vp]),
     'occb200_engine_set_prev_rotation': (_i, [_vp, _vp]),
     'occb200_engine_forward': (_i, [_vp, ctypes.POINTER(_vp), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'occb200_engine_forward_host': (_i, [_vp, ctypes.POINTER(_vp), _vp, _vp, _vp]),
@@ -56,6 +57,8 @@ SIGNATURES = {
     'occb200_backbone_level_shape': (_i, [_vp, _i, ctypes.POINTER(_i), ctypes.POINTER(_i)]),
     'occb200_backbone_forward': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'occb200_backbone_forward_nhwc_bf16': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'occb200_backbone_set_frame_format': (_i, [_vp, _i, _i, _vp, _vp, _i]),
+    'occb200_backbone_forward_frames': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
 }
 
 _lib = None

@@ -69,6 +69,51 @@ class BackboneEngine:
             _lib.check(self.lib.occb200_backbone_forward(self._h, _lib.ptr(img), *[_lib.ptr(o) for o in outs], _lib.stream_ptr()))
         return outs
 
+    def set_frame_format(self, src_hw, mean, std, to_rgb):
+        """Frames for `forward_frames` are uint8 (num_images, src_h, src_w, 3) in BGR order (as decoded by mmcv.imread); the
+        stem normalises them like NormalizeMultiviewImage(mean, std, to_rgb) (swap first, then (x - mean[c]) * (1/std[c]) in
+        fp32, mean / std in the normalised channel order) and pads them with 0 at the bottom / right to the engine's H x W
+        like PadMultiViewImage(pad_val=0)."""
+        src_h, src_w = int(src_hw[0]), int(src_hw[1])
+        m = np.ascontiguousarray(np.asarray(mean, np.float32).reshape(3))
+        s = np.ascontiguousarray(np.asarray(std, np.float32).reshape(3))
+        _lib.check(self.lib.occb200_backbone_set_frame_format(self._h, src_h, src_w, _lib.ptr(m), _lib.ptr(s), int(bool(to_rgb))))
+        self.frame_hw = (src_h, src_w)
+
+    def check_frames(self, frames, cuda=True):
+        """Host-side contract of a frame buffer: a wrong tensor would be an out-of-bounds read on the device."""
+        hw = getattr(self, 'frame_hw', None)
+        if hw is None:
+            raise RuntimeError('BackboneEngine: call set_frame_format() before passing camera frames')
+        want = (self.num_images, hw[0], hw[1], 3)
+        if not isinstance(frames, torch.Tensor):
+            raise TypeError('frames must be a torch.Tensor')
+        if frames.dtype != torch.uint8:
+            raise ValueError(f'frames must be uint8, got {frames.dtype}')
+        if tuple(frames.shape) != want:
+            raise ValueError(f'frames shape {tuple(frames.shape)} != {want} (num_images, src_h, src_w, 3)')
+        if not frames.is_contiguous():
+            raise ValueError('frames must be contiguous (num_images, src_h, src_w, 3)')
+        if frames.is_cuda != cuda:
+            raise ValueError(f'frames must be a {"CUDA" if cuda else "CPU (pinned)"} tensor')
+
+    def forward_frames(self, frames, channels_last_bf16=False):
+        """frames (num_images, src_h, src_w, 3) CUDA uint8, contiguous -> the same 4 levels as `forward` returns for the
+        normalised, padded fp32 images, bit for bit (see `set_frame_format`)."""
+        self.check_frames(frames, cuda=True)
+        if channels_last_bf16 and self.precision != 'bf16':
+            raise RuntimeError('channels_last_bf16 output needs a bf16 backbone engine')
+        with torch.cuda.device(frames.device):
+            if channels_last_bf16:
+                outs = [torch.empty((self.num_images, h, w, 256), dtype=torch.bfloat16, device=frames.device) for h, w in self.level_shapes]
+                _lib.check(self.lib.occb200_backbone_forward_frames(self._h, _lib.ptr(frames), *[_lib.ptr(o) for o in outs], 1,
+                                                                    _lib.stream_ptr()))
+                return [o.permute(0, 3, 1, 2) for o in outs]
+            outs = [torch.empty((self.num_images, 256, h, w), dtype=torch.float32, device=frames.device) for h, w in self.level_shapes]
+            _lib.check(self.lib.occb200_backbone_forward_frames(self._h, _lib.ptr(frames), *[_lib.ptr(o) for o in outs], 0,
+                                                                _lib.stream_ptr()))
+        return outs
+
     def __del__(self):
         h = getattr(self, '_h', None)
         if h:

@@ -58,6 +58,10 @@ struct occb200_backbone {
     struct Block { ConvW c1, c2, c3, down; bool has_down = false; int stride = 1; };
     std::vector<Block> blocks[4];
     ConvW lateral[3], fpnc[4];
+    // occb200_backbone_set_frame_format: normalisation + padding of uint8 camera frames (forward_frames)
+    bool frames_set = false;
+    FrameNorm fn{};
+    int launches = 0;                // kernels the last forward launched
     // workspace
     Buf img_nhwc, col, ping[2], t1, t2, t3, idn, stage_out[3], lat[3], fo[4];
     size_t elt() const { return precision ? 2 : 4; }
@@ -165,6 +169,7 @@ int conv(occb200_backbone* e, const T* in, int N, int H, int W, const ConvW& c, 
         if (e->use_tc && implicit_enabled() && c.wh.p && c.stride == 1 && c.kpad == c.kh * c.kw * c.cin &&
             conv2d_tc_supported(c.cin, c.cout, c.kh, c.kw) && (c.kh == 3 || residual != nullptr)) {
             if (fused_residual) *fused_residual = residual != nullptr;
+            e->launches++;
             return conv2d_tc(reinterpret_cast<const bf16*>(in), c.wh.as<bf16>(), c.b.as<float>(),
                              reinterpret_cast<const bf16*>(residual), reinterpret_cast<bf16*>(out), N, H, W, c.cin, c.cout,
                              c.kh, c.kw, c.pad, residual ? ACT_RELU : act, st);
@@ -174,23 +179,41 @@ int conv(occb200_backbone* e, const T* in, int N, int H, int W, const ConvW& c, 
     if (!(c.kh == 1 && c.kw == 1 && c.stride == 1 && c.kpad == c.cin)) {
         OCC_CHECK((size_t)M * c.kpad * sizeof(T) <= e->col.bytes, "backbone: im2col workspace too small");
         if (launch_im2col_nhwc<T>(in, e->col.as<T>(), N, H, W, c.cin, c.kh, c.kw, c.stride, c.pad, Ho, Wo, c.kpad, st)) return 2;
+        e->launches++;
         A = e->col.as<T>();
     }
+    e->launches++;
     return conv_gemm<T>(e, A, M, c, out, act, st);
 }
 
+// Input: fp32 images `img` [N, 3, H, W], or uint8 camera frames `frames` [N, src_h, src_w, 3] (img == nullptr) that the stem's
+// im2col normalises and pads itself (occb200_backbone_set_frame_format).
 // nhwc_out != nullptr (bf16 only): the FPN output convolutions write the caller's channels-last buffers directly
 template <typename T>
-int forward_impl(occb200_backbone* e, const float* img, float* const* outs, cudaStream_t st, void* const* nhwc_out = nullptr)
+int forward_impl(occb200_backbone* e, const float* img, const uint8_t* frames, float* const* outs, cudaStream_t st,
+                 void* const* nhwc_out = nullptr)
 {
     const int N = e->num_images;
     int H = e->H, W = e->W, Ho, Wo;
-    if (launch_nchw_to_nhwc_small<T>(img, e->img_nhwc.as<T>(), N, 3, H, W, st)) return 2;
+    e->launches = 0;
     // stem: conv 7x7 s2 p3 + BN + ReLU, MaxPool 3x3 s2 p1 (mmdet ResNet.forward / torchvision resnet50)
-    if (conv<T>(e, e->img_nhwc.as<T>(), N, H, W, e->stem, e->ping[0].as<T>(), ACT_RELU, Ho, Wo, st)) return 2;
+    if (img) {
+        if (launch_nchw_to_nhwc_small<T>(img, e->img_nhwc.as<T>(), N, 3, H, W, st)) return 2;
+        e->launches++;
+        if (conv<T>(e, e->img_nhwc.as<T>(), N, H, W, e->stem, e->ping[0].as<T>(), ACT_RELU, Ho, Wo, st)) return 2;
+    } else {
+        const ConvW& c = e->stem;
+        Ho = out_size(H, c.kh, c.stride, c.pad);
+        Wo = out_size(W, c.kw, c.stride, c.pad);
+        if (launch_im2col_frames<T>(frames, e->col.as<T>(), e->fn, N, H, W, c.kh, c.kw, c.stride, c.pad, Ho, Wo, c.kpad, st))
+            return 2;
+        e->launches += 2;
+        if (conv_gemm<T>(e, e->col.as<T>(), (int64_t)N * Ho * Wo, c, e->ping[0].as<T>(), ACT_RELU, st)) return 2;
+    }
     H = Ho; W = Wo;
     const int Hp = out_size(H, 3, 2, 1), Wp = out_size(W, 3, 2, 1);
     if (launch_maxpool3x3s2_nhwc<T>(e->ping[0].as<T>(), e->ping[1].as<T>(), N, H, W, 64, Hp, Wp, st)) return 2;
+    e->launches++;
     H = Hp; W = Wp;
     const T* cur = e->ping[1].as<T>();
     int sh[3], sw[3];
@@ -217,6 +240,7 @@ int forward_impl(occb200_backbone* e, const float* img, float* const* outs, cuda
             if (!fused) {
                 if (conv<T>(e, e->t2.as<T>(), N, h2, w2, blk.c3, e->t3.as<T>(), ACT_NONE, h3, w3, st)) return 2;
                 if (launch_add_relu<T>(e->t3.as<T>(), identity, dst, (int64_t)N * h3 * w3 * blk.c3.cout, st)) return 2;
+                e->launches++;
             }
             cur = dst; H = h3; W = w3;
         }
@@ -231,6 +255,7 @@ int forward_impl(occb200_backbone* e, const float* img, float* const* outs, cuda
     for (int i = 2; i >= 1; --i)
         if (launch_upsample_add_nhwc<T>(e->lat[i - 1].as<T>(), e->lat[i].as<T>(), N, lh[i - 1], lw[i - 1], lh[i], lw[i],
                                         e->out_channels, st)) return 2;
+    e->launches += 2;
     int oh[4], ow[4];
     T* fo[4];
     for (int i = 0; i < 4; ++i) fo[i] = (nhwc_out && nhwc_out[i]) ? reinterpret_cast<T*>(nhwc_out[i]) : e->fo[i].as<T>();
@@ -238,8 +263,11 @@ int forward_impl(occb200_backbone* e, const float* img, float* const* outs, cuda
         if (conv<T>(e, e->lat[i].as<T>(), N, lh[i], lw[i], e->fpnc[i], fo[i], ACT_NONE, oh[i], ow[i], st)) return 2;
     if (conv<T>(e, fo[2], N, oh[2], ow[2], e->fpnc[3], fo[3], ACT_NONE, oh[3], ow[3], st)) return 2;
     if (nhwc_out) return 0;
-    for (int i = 0; i < 4; ++i)
-        if (outs[i] && launch_nhwc_to_nchw_f32<T>(e->fo[i].as<T>(), outs[i], N, oh[i] * ow[i], e->out_channels, st)) return 2;
+    for (int i = 0; i < 4; ++i) {
+        if (!outs[i]) continue;
+        if (launch_nhwc_to_nchw_f32<T>(e->fo[i].as<T>(), outs[i], N, oh[i] * ow[i], e->out_channels, st)) return 2;
+        e->launches++;
+    }
     return 0;
 }
 
@@ -366,8 +394,8 @@ int occb200_backbone_forward(occb200_backbone* e, const float* img, float* out0,
     OCC_CHECK(e && img, "null pointer");
     OCC_CHECK(e->finalized, "backbone_finalize() has not been called");
     float* outs[4] = {out0, out1, out2, out3};
-    return e->precision ? forward_impl<bf16>(e, img, outs, (cudaStream_t)stream)
-                        : forward_impl<float>(e, img, outs, (cudaStream_t)stream);
+    return e->precision ? forward_impl<bf16>(e, img, nullptr, outs, (cudaStream_t)stream)
+                        : forward_impl<float>(e, img, nullptr, outs, (cudaStream_t)stream);
 }
 
 int occb200_backbone_forward_nhwc_bf16(occb200_backbone* e, const float* img, void* out0, void* out1, void* out2, void* out3,
@@ -377,7 +405,51 @@ int occb200_backbone_forward_nhwc_bf16(occb200_backbone* e, const float* img, vo
     OCC_CHECK(e->finalized, "backbone_finalize() has not been called");
     OCC_CHECK(e->precision == 1, "backbone_forward_nhwc_bf16 needs a bf16 backbone (precision 1)");
     void* outs[4] = {out0, out1, out2, out3};
-    return forward_impl<bf16>(e, img, nullptr, (cudaStream_t)stream, outs);
+    return forward_impl<bf16>(e, img, nullptr, nullptr, (cudaStream_t)stream, outs);
+}
+
+int occb200_backbone_set_frame_format(occb200_backbone* e, int src_h, int src_w, const float mean[3], const float std[3],
+                                      int to_rgb)
+{
+    OCC_CHECK(e && mean && std, "null pointer");
+    OCC_CHECK(src_h >= 1 && src_w >= 1 && src_h <= e->H && src_w <= e->W,
+              "backbone_set_frame_format: frames of " + std::to_string(src_h) + "x" + std::to_string(src_w) +
+                  " do not fit the backbone's " + std::to_string(e->H) + "x" + std::to_string(e->W));
+    for (int c = 0; c < 3; ++c)
+        OCC_CHECK(std::isfinite(mean[c]) && std::isfinite(std[c]) && std[c] != 0.f,
+                  "backbone_set_frame_format: mean / std must be finite and std non-zero");
+    FrameNorm fn{};
+    for (int c = 0; c < 3; ++c) {
+        fn.mean[c] = mean[c];
+        fn.inv_std[c] = (float)(1.0 / (double)std[c]);          // mmcv.imnormalize: stdinv = 1 / np.float64(std)
+    }
+    fn.src_h = src_h; fn.src_w = src_w; fn.to_rgb = to_rgb ? 1 : 0;
+    e->fn = fn;
+    e->frames_set = true;
+    return 0;
+}
+
+int occb200_backbone_forward_frames(occb200_backbone* e, const uint8_t* frames, void* out0, void* out1, void* out2,
+                                    void* out3, int out_layout, void* stream)
+{
+    OCC_CHECK(e && frames, "null pointer");
+    OCC_CHECK(e->finalized, "backbone_finalize() has not been called");
+    OCC_CHECK(e->frames_set, "backbone_forward_frames: call occb200_backbone_set_frame_format first");
+    OCC_CHECK(out_layout == 0 || out_layout == 1, "backbone_forward_frames: out_layout must be 0 (fp32 NCHW) or 1 (bf16 NHWC)");
+    void* outs[4] = {out0, out1, out2, out3};
+    if (out_layout == 1) {
+        OCC_CHECK(e->precision == 1, "backbone_forward_frames: out_layout 1 needs a bf16 backbone (precision 1)");
+        OCC_CHECK(out0 && out1 && out2 && out3, "null pointer");
+        return forward_impl<bf16>(e, nullptr, frames, nullptr, (cudaStream_t)stream, outs);
+    }
+    float* fo[4] = {(float*)out0, (float*)out1, (float*)out2, (float*)out3};
+    return e->precision ? forward_impl<bf16>(e, nullptr, frames, fo, (cudaStream_t)stream)
+                        : forward_impl<float>(e, nullptr, frames, fo, (cudaStream_t)stream);
 }
 
 }  // extern "C"
+
+occ::BackboneInfo occ::backbone_info(const occb200_backbone* e)
+{
+    return {e->num_images, e->H, e->W, e->precision, e->finalized, e->frames_set, e->fn.src_h, e->fn.src_w, e->launches};
+}

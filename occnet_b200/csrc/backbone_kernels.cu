@@ -92,6 +92,29 @@ __global__ void im2col_nhwc_any_kernel(const T* __restrict__ in, T* __restrict__
 // 16-byte chunks (8 consecutive k) of the output rows from shared memory and writes them coalesced (855 MB of im2col rows for
 // 6 x 928 x 1600 images: an element-per-thread gather from global memory was the slowest step of the backbone).
 constexpr int STEM_TW = 128, STEM_MAX_KH = 7, STEM_MAX_SPAN = 1024;
+
+// Write phase shared by the stem im2col kernels: the CTA's output rows [128 pixels, Kpad] from the KH staged input rows.
+template <typename T>
+__device__ __forceinline__ void stem_write_rows(const T (&rows)[STEM_MAX_KH][STEM_MAX_SPAN], T* __restrict__ out, int n,
+                                                int yo, int x0, int C, int KH, int KW, int stride, int Ho, int Wo, int Kpad)
+{
+    const int kv = Kpad / 8, kwc = KW * C, ktot = KH * kwc;
+    const int64_t m0 = ((int64_t)n * Ho + yo) * Wo + x0;
+    for (int id = threadIdx.x; id < STEM_TW * kv; id += 256) {
+        const int px = id / kv, k0 = (id - px * kv) * 8;
+        if (x0 + px >= Wo) break;
+        int ky = k0 / kwc, r = k0 - ky * kwc;
+        const int base = px * stride * C;
+        float v[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            v[j] = (k0 + j < ktot) ? to_f32(rows[ky][base + r]) : 0.f;
+            if (++r == kwc) { r = 0; ++ky; }
+        }
+        store8(out + (m0 + px) * Kpad + k0, v);
+    }
+}
+
 template <typename T>
 __global__ void __launch_bounds__(256)
 im2col_smallc_kernel(const T* __restrict__ in, T* __restrict__ out, int N, int H, int W, int C, int KH, int KW, int stride,
@@ -110,21 +133,64 @@ im2col_smallc_kernel(const T* __restrict__ in, T* __restrict__ out, int N, int H
         }
     }
     __syncthreads();
-    const int kv = Kpad / 8, kwc = KW * C, ktot = KH * kwc;
-    const int64_t m0 = ((int64_t)n * Ho + yo) * Wo + x0;
-    for (int id = threadIdx.x; id < STEM_TW * kv; id += 256) {
-        const int px = id / kv, k0 = (id - px * kv) * 8;
-        if (x0 + px >= Wo) break;
-        int ky = k0 / kwc, r = k0 - ky * kwc;
-        const int base = px * stride * C;
-        float v[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            v[j] = (k0 + j < ktot) ? to_f32(rows[ky][base + r]) : 0.f;
-            if (++r == kwc) { r = 0; ++ky; }
+    stem_write_rows<T>(rows, out, n, yo, x0, C, KH, KW, stride, Ho, Wo, Kpad);
+}
+
+// The same stem im2col straight from uint8 camera frames [N, src_h, src_w, 3] (BGR, as decoded), fusing what the reference's
+// test pipeline does on the host: NormalizeMultiviewImage (optional BGR->RGB swap first, then (x - mean[c]) * (1/std[c]) in
+// fp32, the two operations kept separate: no FMA contraction), PadMultiViewImage (pad_val 0 at the bottom / right up to the
+// backbone's H x W) and the HWC->CHW transpose of DefaultFormatBundle3D (the im2col reads channels-last anyway).  Staging is
+// two passes: the raw bytes of the KH rows (16-byte loads when every row starts 16-byte aligned, bytes otherwise), then
+// the normalised values in the storage type.  Padded pixels hold 0, never a normalised 0, and so does the convolution's own
+// padding.  The rows are then bit-identical to what nchw_to_nhwc_small + im2col_smallc stage from the fp32 images the host
+// pipeline produces, and the write phase is shared, so the operand is byte-identical.
+constexpr int STEM_MAX_RAW = STEM_MAX_SPAN + 32;               // span + alignment slack at both ends
+
+template <typename T>
+__global__ void __launch_bounds__(256)
+im2col_frames_kernel(const uint8_t* __restrict__ frames, T* __restrict__ out, FrameNorm fn, int KH, int KW, int stride,
+                     int pad, int Ho, int Wo, int Kpad, int vec)
+{
+    constexpr int C = 3;
+    __shared__ T rows[STEM_MAX_KH][STEM_MAX_SPAN];
+    __shared__ __align__(16) uint8_t raw[STEM_MAX_KH][STEM_MAX_RAW];
+    const int x0 = blockIdx.x * STEM_TW, yo = blockIdx.y, n = blockIdx.z;
+    const int span = ((STEM_TW - 1) * stride + KW) * C;
+    const int gx0 = (x0 * stride - pad) * C;
+    const int row_bytes = fn.src_w * C;
+    const int b0 = max(gx0, 0), b1 = min(gx0 + span, row_bytes);  // bytes of the source row inside the span (whole pixels)
+    const int a0 = vec ? (b0 & ~15) : b0;                         // raw[ky][0] holds source byte a0
+    for (int ky = 0; ky < KH; ++ky) {
+        const int y = yo * stride + ky - pad;
+        if (y < 0 || y >= fn.src_h || b1 <= b0) continue;
+        const uint8_t* src = frames + ((int64_t)n * fn.src_h + y) * row_bytes;
+        if (vec) {                                                // row_bytes % 16 == 0: the last chunk ends inside the row
+            const int nchunk = (b1 - a0 + 15) >> 4;
+            for (int i = threadIdx.x; i < nchunk; i += 256)
+                *reinterpret_cast<uint4*>(&raw[ky][i * 16]) = __ldg(reinterpret_cast<const uint4*>(src + a0) + i);
+        } else {
+            for (int i = threadIdx.x; i < b1 - b0; i += 256) raw[ky][i] = src[b0 + i];
         }
-        store8(out + (m0 + px) * Kpad + k0, v);
     }
+    __syncthreads();
+    for (int ky = 0; ky < KH; ++ky) {
+        const int y = yo * stride + ky - pad;
+        const bool row_in = y >= 0 && y < fn.src_h;
+        for (int e = threadIdx.x; e < span; e += 256) {
+            const int g = gx0 + e;
+            float v = 0.f;
+            if (row_in && g >= b0 && g < b1) {
+                const int c = g % C;                              // output channel (RGB order when to_rgb)
+                const int sc = fn.to_rgb ? C - 1 - c : c;         // its byte in the BGR frame
+                const float mean = c == 0 ? fn.mean[0] : (c == 1 ? fn.mean[1] : fn.mean[2]);
+                const float inv = c == 0 ? fn.inv_std[0] : (c == 1 ? fn.inv_std[1] : fn.inv_std[2]);
+                v = __fmul_rn(__fsub_rn((float)raw[ky][g - c + sc - a0], mean), inv);
+            }
+            rows[ky][e] = from_f32<T>(v);
+        }
+    }
+    __syncthreads();
+    stem_write_rows<T>(rows, out, n, yo, x0, C, KH, KW, stride, Ho, Wo, Kpad);
 }
 
 // MaxPool2d(kernel 3, stride 2, padding 1) on NHWC, 8 channels per thread (padding behaves as -inf)
@@ -245,6 +311,21 @@ int launch_im2col_nhwc(const T* in, T* out, int N, int H, int W, int C, int KH, 
 }
 
 template <typename T>
+int launch_im2col_frames(const uint8_t* frames, T* out, const FrameNorm& fn, int N, int H, int W, int KH, int KW, int stride,
+                         int pad, int Ho, int Wo, int Kpad, cudaStream_t stream)
+{
+    OCC_CHECK(Kpad >= KH * KW * 3 && Kpad % 8 == 0, "im2col_frames: Kpad must cover KH*KW*3 and be a multiple of 8");
+    OCC_CHECK(KH <= STEM_MAX_KH && ((STEM_TW - 1) * stride + KW) * 3 <= STEM_MAX_SPAN && N <= 65535 && Ho <= 65535,
+              "im2col_frames: convolution shape outside the shared-memory stem kernel");
+    OCC_CHECK(fn.src_h >= 1 && fn.src_w >= 1 && fn.src_h <= H && fn.src_w <= W, "im2col_frames: frames must fit in H x W");
+    const int vec = (fn.src_w * 3) % 16 == 0 && (reinterpret_cast<uintptr_t>(frames) & 15) == 0;
+    dim3 grid(ceil_div(Wo, STEM_TW), Ho, N);
+    im2col_frames_kernel<T><<<grid, 256, 0, stream>>>(frames, out, fn, KH, KW, stride, pad, Ho, Wo, Kpad, vec);
+    OCC_CUDA(cudaGetLastError());
+    return 0;
+}
+
+template <typename T>
 int launch_maxpool3x3s2_nhwc(const T* in, T* out, int N, int H, int W, int C, int Ho, int Wo, cudaStream_t stream)
 {
     OCC_CHECK(C % 8 == 0, "maxpool: C must be a multiple of 8");
@@ -285,6 +366,8 @@ int launch_nhwc_to_nchw_f32(const T* src, float* dst, int N, int HW, int C, cuda
 #define OCC_INST(T)                                                                                                       \
     template int launch_nchw_to_nhwc_small<T>(const float*, T*, int, int, int, int, cudaStream_t);                       \
     template int launch_im2col_nhwc<T>(const T*, T*, int, int, int, int, int, int, int, int, int, int, int, cudaStream_t); \
+    template int launch_im2col_frames<T>(const uint8_t*, T*, const FrameNorm&, int, int, int, int, int, int, int, int,    \
+                                         int, int, cudaStream_t);                                                         \
     template int launch_maxpool3x3s2_nhwc<T>(const T*, T*, int, int, int, int, int, int, cudaStream_t);                  \
     template int launch_add_relu<T>(const T*, const T*, T*, int64_t, cudaStream_t);                                      \
     template int launch_upsample_add_nhwc<T>(T*, const T*, int, int, int, int, int, int, cudaStream_t);                  \

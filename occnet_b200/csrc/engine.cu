@@ -71,6 +71,12 @@ struct occb200_engine {
     DevBuf rot_map;                     // occb200_engine_set_prev_rotation: source row of every BEV cell (int32, -1 = outside)
     bool rot_set = false;
     int feats_bf16 = 0;                 // occb200_engine_set_input_dtype: feature levels arrive as bf16 instead of fp32
+    // input dtype 3 (uint8 camera frames): the attached backbone (borrowed), the levels it hands over (shared by both host
+    // slots, like its workspace) and the event after the last frame that read them
+    occb200_backbone* bb = nullptr;
+    DevBuf bb_levels[4];
+    cudaEvent_t bb_free = nullptr;
+    bool bb_free_recorded = false;
     std::map<std::string, std::vector<float>> host_params;
     std::vector<LayerW> layers;
     DevBuf bev_queries, pos, pos_t32, cams_embeds, level_embeds;
@@ -617,6 +623,61 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
     return 0;
 }
 
+// A backbone the engine can drive for input dtype 3: finalized, one image per camera, the engine's level shapes, frames set.
+int check_backbone(const occb200_engine* e, const occb200_backbone* bb)
+{
+    const BackboneInfo bi = backbone_info(bb);
+    OCC_CHECK(bi.finalized, "attach_backbone: backbone_finalize() has not been called");
+    OCC_CHECK(bi.num_images == e->cfg.num_cams, "attach_backbone: backbone num_images " + std::to_string(bi.num_images) +
+                                                    " != engine num_cams " + std::to_string(e->cfg.num_cams));
+    for (int l = 0; l < 4; ++l) {
+        int h = 0, w = 0;
+        if (occb200_backbone_level_shape(bb, l, &h, &w)) return 1;
+        OCC_CHECK(h == e->lg.h[l] && w == e->lg.w[l],
+                  "attach_backbone: backbone level " + std::to_string(l) + " is " + std::to_string(h) + "x" +
+                      std::to_string(w) + ", the engine's is " + std::to_string(e->lg.h[l]) + "x" + std::to_string(e->lg.w[l]));
+    }
+    OCC_CHECK(bi.frames_set, "attach_backbone: backbone has no frame format (occb200_backbone_set_frame_format)");
+    return 0;
+}
+
+// uint8 frames [num_cams, src_h, src_w, 3] of the attached backbone
+size_t frame_bytes(const occb200_engine* e)
+{
+    const BackboneInfo bi = backbone_info(e->bb);
+    return (size_t)e->cfg.num_cams * bi.src_h * bi.src_w * 3;
+}
+
+template <typename T>
+int forward_frames_impl(occb200_engine* e, const uint8_t* frames, const float* prev_bev, float* bev_embed, float* occ_logits,
+                        float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st)
+{
+    const BackboneInfo bi = backbone_info(e->bb);
+    const bool cl = e->cfg.precision == 1 && bi.precision == 1;   // bf16 -> bf16: channels-last hand-over (input dtype 2)
+    void* lv[4];
+    for (int l = 0; l < 4; ++l) {
+        const size_t n = (size_t)e->cfg.num_cams * 256 * e->lg.h[l] * e->lg.w[l] * (cl ? 2 : 4);
+        if (e->bb_levels[l].bytes != n && e->bb_levels[l].alloc(n)) return 2;
+        lv[l] = e->bb_levels[l].p;
+    }
+    if (!e->bb_free) OCC_CUDA(cudaEventCreateWithFlags(&e->bb_free, cudaEventDisableTiming));
+    // the backbone workspace and the level buffers are shared by every stream the frames arrive on
+    if (e->bb_free_recorded) OCC_CUDA(cudaStreamWaitEvent(st, e->bb_free, 0));
+    int rc = occb200_backbone_forward_frames(e->bb, frames, lv[0], lv[1], lv[2], lv[3], cl ? 1 : 0, st);
+    if (rc) return rc;
+    const int bb_launches = backbone_info(e->bb).launches;
+    const float* feats[4] = {(const float*)lv[0], (const float*)lv[1], (const float*)lv[2], (const float*)lv[3]};
+    const int code = e->feats_bf16;
+    e->feats_bf16 = cl ? 2 : 0;
+    rc = forward_impl<T>(e, feats, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st);
+    e->feats_bf16 = code;
+    if (rc) return rc;
+    OCC_CUDA(cudaEventRecord(e->bb_free, st));
+    e->bb_free_recorded = true;
+    e->launches += bb_launches;
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -705,8 +766,9 @@ void occb200_engine_destroy(occb200_engine* e)
                      &e->q_pos_t, &e->q0_t, &e->prev_t, &e->tsa_value, &e->tsa_value_prev, &e->qproj, &e->attn_out,
                      &e->x_f32, &e->ffn_h, &e->vox0, &e->vox1, &e->vox2, &e->hits, &e->tap_layer, &e->tap_tsa,
                      &e->tap_sca, &e->feats_dev[0], &e->feats_dev[1], &e->feats_dev[2], &e->feats_dev[3],
-                     &e->occ_i64_dev, &e->flow_dev};
+                     &e->occ_i64_dev, &e->flow_dev, &e->bb_levels[0], &e->bb_levels[1], &e->bb_levels[2], &e->bb_levels[3]};
     for (DevBuf* b : all) b->release();
+    if (e->bb_free) cudaEventDestroy(e->bb_free);
     for (auto& sl : e->slots) {
         for (auto& f : sl.feats) f.release();
         sl.occ.release(); sl.flow.release();
@@ -1001,8 +1063,17 @@ int occb200_engine_forward(occb200_engine* e, const float* const* feats, const f
     OCC_CHECK(e && feats, "null pointer");
     OCC_CHECK(e->finalized, "engine_finalize() has not been called");
     OCC_CHECK(e->cameras_set, "engine_set_cameras() has not been called");
-    for (int l = 0; l < e->cfg.num_levels; ++l) OCC_CHECK(feats[l] != nullptr, "null feature level");
     cudaStream_t st = (cudaStream_t)stream;
+    if (e->feats_bf16 == 3) {
+        OCC_CHECK(e->bb != nullptr, "input dtype 3 (camera frames) needs an attached backbone (occb200_engine_attach_backbone)");
+        OCC_CHECK(feats[0] != nullptr, "null frame buffer");
+        if (check_backbone(e, e->bb)) return 1;
+        const uint8_t* frames = reinterpret_cast<const uint8_t*>(feats[0]);
+        if (e->cfg.precision == 0)
+            return forward_frames_impl<float>(e, frames, prev_bev, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64, st);
+        return forward_frames_impl<bf16>(e, frames, prev_bev, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64, st);
+    }
+    for (int l = 0; l < e->cfg.num_levels; ++l) OCC_CHECK(feats[l] != nullptr, "null feature level");
     if (e->cfg.precision == 0)
         return forward_impl<float>(e, feats, prev_bev, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64, st);
     return forward_impl<bf16>(e, feats, prev_bev, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64, st);
@@ -1013,12 +1084,14 @@ int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_hos
 {
     OCC_CHECK(e && feats_host && occ_cls_i64_host && flow_host, "null pointer");
     OCC_CHECK(e->finalized && e->cameras_set, "engine not finalized / cameras not set");
+    if (e->feats_bf16 == 3) OCC_CHECK(e->bb != nullptr && feats_host[0] != nullptr, "input dtype 3 needs an attached backbone and a frame buffer");
     const occb200_config& c = e->cfg;
     cudaStream_t st = (cudaStream_t)stream;
     const size_t nvox = (size_t)c.bev_w * c.bev_h * c.pillar_h;
-    const float* dev_feats[4];
-    for (int l = 0; l < 4; ++l) {
-        const size_t n = (size_t)c.num_cams * 256 * e->lg.h[l] * e->lg.w[l] * (e->feats_bf16 ? 2 : 4);
+    const float* dev_feats[4] = {nullptr, nullptr, nullptr, nullptr};
+    for (int l = 0; l < (e->feats_bf16 == 3 ? 1 : 4); ++l) {
+        const size_t n = e->feats_bf16 == 3 ? frame_bytes(e)
+                                            : (size_t)c.num_cams * 256 * e->lg.h[l] * e->lg.w[l] * (e->feats_bf16 ? 2 : 4);
         if (e->feats_dev[l].bytes != n && e->feats_dev[l].alloc(n)) return 2;
         OCC_CUDA(cudaMemcpyAsync(e->feats_dev[l].p, feats_host[l], n, cudaMemcpyHostToDevice, st));
         dev_feats[l] = e->feats_dev[l].as<float>();
@@ -1040,6 +1113,7 @@ int occb200_engine_submit_host(occb200_engine* e, int slot, const float* const* 
     OCC_CHECK(e && feats_host && occ_cls_i64_host && flow_host, "null pointer");
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
     OCC_CHECK(e->finalized && e->cameras_set, "engine not finalized / cameras not set");
+    if (e->feats_bf16 == 3) OCC_CHECK(e->bb != nullptr && feats_host[0] != nullptr, "input dtype 3 needs an attached backbone and a frame buffer");
     const occb200_config& c = e->cfg;
     cudaStream_t st = (cudaStream_t)stream;
     occb200_engine::Slot& s = e->slots[slot];
@@ -1061,9 +1135,10 @@ int occb200_engine_submit_host(occb200_engine* e, int slot, const float* const* 
         return n < 1 ? 1 : (n > 4 ? 4 : n);
     }();
     const size_t nvox = (size_t)c.bev_w * c.bev_h * c.pillar_h;
-    const float* dev_feats[4];
-    for (int l = 0; l < 4; ++l) {
-        const size_t n = (size_t)c.num_cams * 256 * e->lg.h[l] * e->lg.w[l] * (e->feats_bf16 ? 2 : 4);
+    const float* dev_feats[4] = {nullptr, nullptr, nullptr, nullptr};
+    for (int l = 0; l < (e->feats_bf16 == 3 ? 1 : 4); ++l) {              // input dtype 3: one buffer, the uint8 frames
+        const size_t n = e->feats_bf16 == 3 ? frame_bytes(e)
+                                            : (size_t)c.num_cams * 256 * e->lg.h[l] * e->lg.w[l] * (e->feats_bf16 ? 2 : 4);
         if (s.feats[l].bytes != n && s.feats[l].alloc(n)) return 2;
         const int pieces = n >= (32u << 20) ? nsplit : 1;
         const size_t chunk = ((n / pieces) + 255) & ~(size_t)255;
@@ -1115,8 +1190,19 @@ int occb200_engine_set_prev_rotation(occb200_engine* e, const int32_t* map_host)
 
 int occb200_engine_set_input_dtype(occb200_engine* e, int feats_bf16)
 {
-    OCC_CHECK(e && feats_bf16 >= 0 && feats_bf16 <= 2, "input dtype must be 0 (fp32 NCHW), 1 (bf16 NCHW) or 2 (bf16 NHWC)");
+    OCC_CHECK(e && feats_bf16 >= 0 && feats_bf16 <= 3,
+              "input dtype must be 0 (fp32 NCHW), 1 (bf16 NCHW), 2 (bf16 NHWC) or 3 (uint8 camera frames)");
     e->feats_bf16 = feats_bf16;
+    return 0;
+}
+
+int occb200_engine_attach_backbone(occb200_engine* e, occb200_backbone* bb)
+{
+    OCC_CHECK(e, "null engine");
+    if (bb && check_backbone(e, bb)) return 1;
+    if (e->bb_free_recorded) OCC_CUDA(cudaEventSynchronize(e->bb_free));   // the previous backbone may still be running
+    e->bb = bb;
+    e->bb_free_recorded = false;
     return 0;
 }
 

@@ -2,6 +2,8 @@
 #pragma once
 #include "common.cuh"
 
+typedef struct occb200_backbone occb200_backbone;
+
 namespace occ {
 
 // Per-frame camera geometry for the fused spatial cross-attention kernel.
@@ -40,6 +42,15 @@ template <typename T> int launch_nchw_to_nhwc_small(const float* src, T* dst, in
 template <typename T>
 int launch_im2col_nhwc(const T* in, T* out, int N, int H, int W, int C, int KH, int KW, int stride, int pad, int Ho, int Wo,
                        int Kpad, cudaStream_t stream);
+// stem im2col straight from uint8 frames [N, src_h, src_w, 3] (BGR): to_rgb swap, (x - mean[c]) * inv_std[c] in fp32, zero pad
+// to H x W (see the kernel's comment); the operand equals launch_im2col_nhwc's on the normalised, padded fp32 images
+struct FrameNorm { float mean[3], inv_std[3]; int src_h, src_w, to_rgb; };
+template <typename T>
+int launch_im2col_frames(const uint8_t* frames, T* out, const FrameNorm& fn, int N, int H, int W, int KH, int KW, int stride,
+                         int pad, int Ho, int Wo, int Kpad, cudaStream_t stream);
+// backbone.cu: what the frame engine checks before it drives an attached backbone (occb200_engine_attach_backbone)
+struct BackboneInfo { int num_images, H, W, precision; bool finalized, frames_set; int src_h, src_w, launches; };
+BackboneInfo backbone_info(const occb200_backbone* e);
 template <typename T> int launch_maxpool3x3s2_nhwc(const T* in, T* out, int N, int H, int W, int C, int Ho, int Wo, cudaStream_t stream);
 template <typename T> int launch_add_relu(const T* a, const T* b, T* out, int64_t n, cudaStream_t stream);
 template <typename T>

@@ -88,15 +88,24 @@ class OccEngine:
         self.vox_shape = (cfg['bev_w'], cfg['bev_h'], cfg['pillar_h'])
         self._pinned = None
         self.feat_dtype, self.feat_channels_last = torch.float32, False
+        self.backbone = None
 
     def set_input_dtype(self, dtype, channels_last=False):
         """Feature levels are handed over as `dtype` from now on (torch.float32, the reference's, or torch.bfloat16);
         `channels_last` (bf16 only): tensors of shape (num_cams, C, h, w) whose MEMORY is (num_cams, h, w, C) -- the
-        backbone engine's native output."""
-        assert dtype in (torch.float32, torch.bfloat16) and not (channels_last and dtype != torch.bfloat16)
-        code = 2 if channels_last else int(dtype == torch.bfloat16)
+        backbone engine's native output.  torch.uint8: each frame is ONE tensor of camera frames (num_cams, src_h, src_w, 3)
+        that the attached backbone (`attach_backbone`) turns into the levels on the device first."""
+        assert dtype in (torch.float32, torch.bfloat16, torch.uint8) and not (channels_last and dtype != torch.bfloat16)
+        code = 3 if dtype == torch.uint8 else (2 if channels_last else int(dtype == torch.bfloat16))
         _lib.check(self.lib.occb200_engine_set_input_dtype(self._h, code))
         self.feat_dtype, self.feat_channels_last = dtype, bool(channels_last)
+
+    def attach_backbone(self, backbone):
+        """`backbone`: a `BackboneEngine` with one image per camera, this engine's level shapes and a frame format
+        (`set_frame_format`), or None to detach.  Borrowed: the engine keeps a reference while it is attached."""
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.occb200_engine_attach_backbone(self._h, None if backbone is None else backbone._h))
+        self.backbone = backbone
 
     def __del__(self):
         h = getattr(self, '_h', None)
@@ -120,6 +129,11 @@ class OccEngine:
 
     def _check_feats(self, feats, cuda):
         """A mismatched tensor would be an out-of-bounds device read in the pack kernel: fail on the host instead."""
+        if self.feat_dtype == torch.uint8:
+            if self.backbone is None:
+                raise RuntimeError('camera-frame input (torch.uint8) needs an attached backbone: call attach_backbone() first')
+            self.backbone.check_frames(feats, cuda=cuda)
+            return
         nc, C = self.cfg['num_cams'], self.cfg['embed_dims']
         if len(feats) != self.cfg['num_levels']:
             raise ValueError(f'expected {self.cfg["num_levels"]} feature levels, got {len(feats)}')
@@ -133,16 +147,17 @@ class OccEngine:
 
     def _feat_ptrs(self, feats):
         arr = (ctypes.c_void_p * 4)()
-        for i, f in enumerate(feats):
+        for i, f in enumerate([feats] if self.feat_dtype == torch.uint8 else feats):
             arr[i] = f.data_ptr()
         return arr
 
     def forward(self, feats, prev_bev=None, want=('bev_embed', 'occ', 'flow', 'occ_cls')):
-        """feats: 4 CUDA fp32 tensors (num_cams, C, h, w) of one frame.  Returns a dict of CUDA tensors."""
+        """feats: 4 CUDA fp32 tensors (num_cams, C, h, w) of one frame, or with `set_input_dtype(torch.uint8)` one CUDA
+        uint8 tensor of camera frames (num_cams, src_h, src_w, 3).  Returns a dict of CUDA tensors."""
         C = self.cfg['embed_dims']
         X, Y, Z = self.vox_shape
         dev = self.device
-        if not self.feat_channels_last:
+        if not self.feat_channels_last and self.feat_dtype != torch.uint8:
             feats = [f.contiguous() for f in feats]
         self._check_feats(feats, cuda=True)
         out = {}
@@ -166,7 +181,8 @@ class OccEngine:
         return out
 
     def forward_host(self, feats_host, occ_out=None, flow_out=None):
-        """feats_host: 4 pinned CPU fp32 tensors (num_cams, C, h, w).  H2D + frame + D2H + sync inside.
+        """feats_host: 4 pinned CPU fp32 tensors (num_cams, C, h, w), or one pinned uint8 tensor of camera frames with
+        `set_input_dtype(torch.uint8)` (25.9 MB per 6 x 900 x 1600 frame).  H2D + frame + D2H + sync inside.
         Returns (occ_cls int64 (X,Y,Z) CPU, flow fp32 (X,Y,Z,2) CPU)."""
         X, Y, Z = self.vox_shape
         if occ_out is None or flow_out is None:
@@ -175,9 +191,7 @@ class OccEngine:
                                 torch.empty((X, Y, Z, 2), dtype=torch.float32).pin_memory())
             occ_out, flow_out = self._pinned
         self._check_feats(feats_host, cuda=False)
-        arr = (ctypes.c_void_p * 4)()
-        for i, f in enumerate(feats_host):
-            arr[i] = f.data_ptr()
+        arr = self._feat_ptrs(feats_host)
         with torch.cuda.device(self.device):
             _lib.check(self.lib.occb200_engine_forward_host(self._h, arr, _lib.ptr(occ_out), _lib.ptr(flow_out),
                                                             _lib.stream_ptr()))
@@ -186,9 +200,7 @@ class OccEngine:
     def submit_host(self, slot, feats_host, occ_out, flow_out):
         """Pipelined host-buffer call (slot 0/1): returns immediately; `wait_host(slot)` completes it."""
         self._check_feats(feats_host, cuda=False)
-        arr = (ctypes.c_void_p * 4)()
-        for i, f in enumerate(feats_host):
-            arr[i] = f.data_ptr()
+        arr = self._feat_ptrs(feats_host)
         with torch.cuda.device(self.device):
             _lib.check(self.lib.occb200_engine_submit_host(self._h, slot, arr, _lib.ptr(occ_out), _lib.ptr(flow_out),
                                                            _lib.stream_ptr()))
@@ -258,4 +270,5 @@ class OccEngine:
 
     @property
     def launches_per_frame(self):
+        """kernels the last forward launched; with camera frames (torch.uint8) the backbone's kernels are included"""
         return int(self.lib.occb200_engine_launches_per_frame(self._h))

@@ -609,12 +609,27 @@ class BEVFormerOcc(BaseModule):
     parameter containers (so reference checkpoints load with their own keys).  Features come from, in this order:
     `img_feats=` handed to forward / simple_test; a `feature_extractor(img)` callable; or the native ResNet-50 + FPN
     (`occnet_b200.backbone.BackboneEngine`, SURVEY 8f rank 1; `native_backbone=False` turns it off) when the config builds
-    `img_backbone` / `img_neck` -- images then go to voxels without leaving the device (bf16: channels-last hand-over)."""
+    `img_backbone` / `img_neck` -- images then go to voxels without leaving the device (bf16: channels-last hand-over).
+
+    `img` may also be the camera frames themselves, uint8 (B, N, h, w, 3) in BGR order as decoded, on CUDA or CPU: the native
+    backbone's stem then does the test pipeline's NormalizeMultiviewImage(**frame_norm_cfg) + PadMultiViewImage(**frame_pad)
+    + DefaultFormatBundle3D on the device (bit-identical to running them on the host in fp32), and copies of the metas get
+    the keys those transforms set.  The defaults are the shipped config's (bevformer_base_occ.py:14-15, 166-171)."""
 
     def __init__(self, pts_bbox_head=None, img_backbone=None, img_neck=None, use_grid_mask=False, video_test_mode=False,
                  train_cfg=None, test_cfg=None, pretrained=None, feature_extractor=None, native_backbone=True,
-                 backbone_precision=None, temporal_test=False, **kwargs):
+                 backbone_precision=None, temporal_test=False,
+                 frame_norm_cfg=dict(mean=[103.530, 116.280, 123.675], std=[1.0, 1.0, 1.0], to_rgb=False),
+                 frame_pad=dict(size_divisor=32), **kwargs):
         super().__init__()
+        self.frame_norm_cfg = dict(mean=[float(v) for v in frame_norm_cfg['mean']],
+                                   std=[float(v) for v in frame_norm_cfg['std']], to_rgb=bool(frame_norm_cfg.get('to_rgb', True)))
+        frame_pad = dict(frame_pad)
+        if frame_pad.pop('pad_val', 0) != 0:
+            raise NotImplementedError('frame_pad: only pad_val=0 (the shipped value and the default) is supported')
+        if (frame_pad.get('size') is None) == (frame_pad.get('size_divisor') is None) or set(frame_pad) - {'size', 'size_divisor'}:
+            raise ValueError(f'frame_pad takes exactly one of size=(H, W) / size_divisor=d, got {frame_pad}')
+        self.frame_pad = dict(size=frame_pad.get('size'), size_divisor=frame_pad.get('size_divisor'))
         if pts_bbox_head is not None:
             pts_bbox_head = dict(pts_bbox_head)
             pts_bbox_head.pop('train_cfg', None); pts_bbox_head.pop('test_cfg', None)
@@ -638,23 +653,89 @@ class BEVFormerOcc(BaseModule):
         self.temporal_test = temporal_test
         self.prev_frame_info = {'prev_bev': None, 'scene_token': None, 'prev_pos': 0, 'prev_angle': 0}
 
+    def _get_backbone_engine(self, device, shape):
+        """the native backbone engine for images of `shape` (B*N, 3, H, W) on `device`, rebuilt when a parameter changes"""
+        from ..backbone import BackboneEngine
+        key = (str(device), tuple(shape), self.backbone_precision,
+               tuple(p._version for p in self.img_backbone.parameters()), tuple(p._version for p in self.img_neck.parameters()))
+        if self._backbone_engine is None or key != self._backbone_key:
+            sd = {k: v for k, v in self.state_dict().items() if k.startswith(('img_backbone.', 'img_neck.'))}
+            self._backbone_engine = BackboneEngine(sd, shape[0], shape[-2:], precision=self.backbone_precision, device=str(device))
+            self._backbone_key = key
+        return self._backbone_engine
+
     def extract_img_feat(self, img, img_metas=None, len_queue=None):
         """reference :66-99 (eval: GridMask is the identity).  img (B, N, 3, H, W) -> list of (B, N, 256, h_l, w_l)."""
-        from ..backbone import BackboneEngine
         if img.dim() == 4:
             img = img.unsqueeze(0)
         B, N = img.shape[:2]
         x = img.reshape(B * N, *img.shape[2:])
-        key = (str(x.device), tuple(x.shape), self.backbone_precision,
-               tuple(p._version for p in self.img_backbone.parameters()), tuple(p._version for p in self.img_neck.parameters()))
-        if self._backbone_engine is None or key != self._backbone_key:
-            sd = {k: v for k, v in self.state_dict().items() if k.startswith(('img_backbone.', 'img_neck.'))}
-            self._backbone_engine = BackboneEngine(sd, B * N, x.shape[-2:], precision=self.backbone_precision, device=str(x.device))
-            self._backbone_key = key
+        be = self._get_backbone_engine(x.device, x.shape)
         cl = self.backbone_precision == 'bf16' and getattr(self.pts_bbox_head, 'precision', 'fp32') == 'bf16'
-        feats = self._backbone_engine.forward(x, channels_last_bf16=cl)        # bf16 head: channels-last hand-over, no copies
+        feats = be.forward(x, channels_last_bf16=cl)                           # bf16 head: channels-last hand-over, no copies
         if len_queue is not None:
             return [f.view(B // len_queue, len_queue, N, *f.shape[1:]) for f in feats]
+        return [f.view(B, N, *f.shape[1:]) for f in feats]
+
+    def frame_shape(self, h, w):
+        """(H, W) that PadMultiViewImage(**frame_pad) pads an h x w frame to"""
+        size, d = self.frame_pad['size'], self.frame_pad['size_divisor']
+        if size is not None:
+            H, W = int(size[0]), int(size[1])
+            if H < h or W < w:
+                raise ValueError(f'frame_pad size {(H, W)} is smaller than the {h}x{w} camera frames')
+            return H, W
+        return -(-h // d) * d, -(-w // d) * d
+
+    @staticmethod
+    def _check_frames(img):
+        if img.dim() == 4:
+            img = img.unsqueeze(0)
+        if img.dim() != 5 or img.shape[-1] != 3:
+            raise ValueError(f'camera frames must be uint8 (B, N, h, w, 3), got shape {tuple(img.shape)}')
+        return img
+
+    def frame_metas(self, img_metas, img):
+        """Copies of `img_metas` with the keys NormalizeMultiviewImage + PadMultiViewImage set for uint8 frames `img`
+        (B, N, h, w, 3): ori_shape (h, w, 3), img_shape = pad_shape (H, W, 3) per camera, pad_fixed_size, pad_size_divisor,
+        img_norm_cfg.  A meta that already carries a different img_shape is an error: the camera projection normalises by
+        it (encoder.py:133-134)."""
+        img = self._check_frames(img)
+        N, h, w = img.shape[1:4]
+        H, W = self.frame_shape(h, w)
+        nc = self.frame_norm_cfg
+        out = []
+        for m in img_metas:
+            have = m.get('img_shape')
+            if have is not None and any(tuple(s[:2]) != (H, W) for s in have):
+                raise ValueError(f"img_metas carry img_shape {list(have)[:1]}... but the {h}x{w} frames pad to {(H, W)}")
+            m = dict(m)
+            m.update(ori_shape=[(h, w, 3)] * N, img_shape=[(H, W, 3)] * N, pad_shape=[(H, W, 3)] * N,
+                     pad_fixed_size=self.frame_pad['size'], pad_size_divisor=self.frame_pad['size_divisor'],
+                     img_norm_cfg=dict(mean=np.asarray(nc['mean'], np.float32), std=np.asarray(nc['std'], np.float32),
+                                       to_rgb=nc['to_rgb']))
+            out.append(m)
+        return out
+
+    def extract_frame_feat(self, img):
+        """uint8 camera frames (B, N, h, w, 3), CUDA or CPU -> list of (B, N, 256, h_l, w_l), normalised and padded by the
+        native backbone's stem."""
+        if not torch.cuda.is_available():
+            raise RuntimeError('BEVFormerOcc: camera frames need a CUDA device (libocc_b200 has no CPU path)')
+        if not (self.native_backbone and hasattr(self, 'img_backbone') and hasattr(self, 'img_neck')):
+            raise RuntimeError('BEVFormerOcc: uint8 camera frames need the native backbone (img_backbone=ResNet, img_neck=FPN)')
+        img = self._check_frames(img)
+        if not img.is_cuda:
+            p = next(self.pts_bbox_head.parameters())
+            dev = p.device if p.is_cuda else torch.device('cuda', torch.cuda.current_device())
+            img = img.to(dev, non_blocking=img.is_pinned())
+        B, N, h, w = img.shape[:4]
+        H, W = self.frame_shape(h, w)
+        be = self._get_backbone_engine(img.device, (B * N, 3, H, W))
+        nc = self.frame_norm_cfg
+        be.set_frame_format((h, w), nc['mean'], nc['std'], nc['to_rgb'])
+        cl = self.backbone_precision == 'bf16' and getattr(self.pts_bbox_head, 'precision', 'fp32') == 'bf16'
+        feats = be.forward_frames(img.reshape(B * N, h, w, 3).contiguous(), channels_last_bf16=cl)
         return [f.view(B, N, *f.shape[1:]) for f in feats]
 
     def extract_feat(self, img, img_metas=None, len_queue=None):
@@ -683,6 +764,9 @@ class BEVFormerOcc(BaseModule):
         return outs['bev_embed'], occ, flow
 
     def simple_test(self, img_metas, img=None, img_feats=None, prev_bev=None, rescale=False, **kwargs):
+        if img_feats is None and isinstance(img, torch.Tensor) and img.dtype == torch.uint8:
+            img_metas = self.frame_metas(img_metas, img)                       # before any launch: shape errors are free
+            return self.simple_test_pts(self.extract_frame_feat(img), img_metas, prev_bev, rescale=rescale)
         feats = img_feats if img_feats is not None else self.extract_feat(img, img_metas)
         return self.simple_test_pts(feats, img_metas, prev_bev, rescale=rescale)
 
