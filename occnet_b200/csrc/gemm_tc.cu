@@ -61,9 +61,6 @@ int make_tensor_map_bf16(CUtensorMap* map, const void* base, int rank, const uin
     return 0;
 }
 
-int cached_map_2d(const void* base, uint64_t inner, uint64_t rows, uint32_t box_inner, uint32_t box_rows, CUtensorMap* out,
-                  uint64_t ld = 0);
-
 namespace {
 
 constexpr int BLOCK_M = 128, BLOCK_K = 64, A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;
@@ -90,7 +87,7 @@ struct GemmProb {
     const float* res_t32;                                     // optional fp32 epilogue constant [M,N] in the T32 block layout
                                                               // (never together with residual: the epilogue loads one of them)
     long long ldc, nblk_stride;                               // C offset of (row, column c of n-block b): b * nblk_stride + row * ldc + c
-    int head_major;                                           // value maps [n-block][column/32][M][32] (one 64-byte row per (head, token))
+    int head_major;                                           // always 0 (see the 16-bit epilogue)
     int M, N, BN, nk, nk1, act, w_resident, stages;
     int out_half;                                             // 16-bit outputs as fp16 instead of bf16 (runtime, per problem)
     int cta_begin, cta_count;
@@ -214,7 +211,9 @@ gemm_tc_kernel(const __grid_constant__ GemmProbs probs, LnArgs ln)
             const bool has_t32 = res_t32 != nullptr, has_res = residual != nullptr, relu = act == ACT_RELU;
             const float* __restrict__ qsrc = has_t32 ? res_t32 : residual;
             const int q_blk = has_t32 ? 1024 : 32, q_j = has_t32 ? 256 : 8;           // operand offset per 32 / per 8 columns
-            const size_t o_blk = P.head_major ? (size_t)M * 32 : 32;                 // output offset per 32 columns
+            // Output offset per 32 columns.  The head_major arm is never taken, but without this run-time select nvcc 12.9 schedules
+            // the epilogue differently and the dense layers got 4-5 % slower on an H100 (400 W); it goes with the epilogue rework.
+            const size_t o_blk = P.head_major ? (size_t)M * 32 : 32;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = r0 + 8 * h;
@@ -295,11 +294,9 @@ struct MapKey {
     bool operator<(const MapKey& o) const { return std::tie(p, d0, d1, ld, b0, b1) < std::tie(o.p, o.d0, o.d1, o.ld, o.b0, o.b1); }
 };
 
-}  // namespace
-
-// row-major bf16 [rows, inner] with a row pitch of `ld` elements (0 = dense)  (also used by gemm_chain.cu)
+// row-major bf16 [rows, inner] with a row pitch of `ld` elements (0 = dense)
 int cached_map_2d(const void* base, uint64_t inner, uint64_t rows, uint32_t box_inner, uint32_t box_rows, CUtensorMap* out,
-                  uint64_t ld)
+                  uint64_t ld = 0)
 {
     static std::map<MapKey, CUtensorMap> cache;
     static std::mutex mu;
@@ -319,12 +316,10 @@ int cached_map_2d(const void* base, uint64_t inner, uint64_t rows, uint32_t box_
     return 0;
 }
 
-namespace {
-
 // Fills one problem (tensor maps, plan, CTA share).  ctas = number of CTAs this problem may use (0: all SMs).
 template <typename TC, bool LN>
 int build_prob(GemmProb& P, int& smem, const bf16* A, const bf16* A2, int K1, const bf16* W, const float* bias, const float* residual,
-               TC* C, int M, int N, int K, int act, bool blocked_out, int lda, int lda2, bool head_major, int ctas, int cta_begin)
+               TC* C, int M, int N, int K, int act, bool blocked_out, int lda, int lda2, int ctas, int cta_begin)
 {
     if (A2 == nullptr) K1 = K;
     const Plan p = make_plan(N, K, LN);
@@ -341,7 +336,7 @@ int build_prob(GemmProb& P, int& smem, const bf16* A, const bf16* A2, int K1, co
     P.bias = bias; P.residual = residual; P.C = C; P.res_t32 = nullptr;
     P.ldc = blocked_out ? (long long)p.BN : (long long)N;
     P.nblk_stride = blocked_out ? (long long)M * p.BN : (long long)p.BN;
-    P.head_major = head_major ? 1 : 0;
+    P.head_major = 0;
     P.M = M; P.N = N; P.BN = p.BN; P.nk = K / BLOCK_K; P.nk1 = K1 / BLOCK_K; P.act = act;
     P.w_resident = p.resident; P.stages = p.stages;
     P.out_half = std::is_same<TC, __half>::value ? 1 : 0;
@@ -370,13 +365,12 @@ int launch_probs(const GemmProbs& probs, int smem, LnArgs ln, cudaStream_t strea
 
 template <typename TC, bool LN>
 int launch(const bf16* A, const bf16* A2, int K1, const bf16* W, const float* bias, const float* residual, TC* C,
-           LnArgs ln, int M, int N, int K, int act, cudaStream_t stream, bool blocked_out = false, int lda = 0, int lda2 = 0,
-           bool head_major = false)
+           LnArgs ln, int M, int N, int K, int act, cudaStream_t stream, bool blocked_out = false, int lda = 0, int lda2 = 0)
 {
     GemmProbs probs;
     probs.n = 1;
     int smem = 0;
-    if (build_prob<TC, LN>(probs.p[0], smem, A, A2, K1, W, bias, residual, C, M, N, K, act, blocked_out, lda, lda2, head_major, 0, 0))
+    if (build_prob<TC, LN>(probs.p[0], smem, A, A2, K1, W, bias, residual, C, M, N, K, act, blocked_out, lda, lda2, 0, 0))
         return 1;
     return launch_probs<TC, LN>(probs, smem, ln, stream);
 }
@@ -396,12 +390,6 @@ int gemm_tc(const bf16* A, const bf16* A2, int K1, const bf16* W, const float* b
     return launch<TC, false>(A, A2, K1, W, bias, residual, C, LnArgs{}, M, N, K, act, stream);
 }
 
-// C = A.W^T + bias, N = 256, written head-major: [8 heads][M][32] bf16 -- TSA value maps
-int gemm_tc_heads256(const bf16* A, const bf16* W, const float* bias, bf16* C, int M, int K, cudaStream_t stream)
-{
-    return launch<bf16, false>(A, nullptr, 0, W, bias, nullptr, C, LnArgs{}, M, 256, K, ACT_NONE, stream, false, 0, 0, true);
-}
-
 // fp32-grade GEMM on the tensor cores: S = [hi | lo] (bf16 split of an fp32 operand, row pitch 2*Ks), W3 = [W_hi | W_hi | W_lo]
 // (N x 3*Ks).  C = hi.W_hi + lo.W_hi + hi.W_lo  (the lo.lo term, 2^-16 relative, is dropped) as ONE GEMM with K' = 3*Ks whose
 // A operand is the concatenation [S (2*Ks columns) | first Ks columns of S again] -- two tensor maps over the same buffer.
@@ -411,12 +399,11 @@ int gemm_tc_split3(const bf16* S, int Ks, const bf16* W3, const float* bias, con
     return launch<float, false>(S, S, 2 * Ks, W3, bias, residual, C, LnArgs{}, M, N, 3 * Ks, act, stream, false, 2 * Ks, 2 * Ks);
 }
 
-int gemm_tc_blocked256(const bf16* A, const bf16* W, const float* bias, bf16* C, int M, int N, int K, cudaStream_t stream,
-                       bool head_major)
+int gemm_tc_blocked256(const bf16* A, const bf16* W, const float* bias, bf16* C, int M, int N, int K, cudaStream_t stream)
 {
     const Plan p = make_plan(N, K, false);
     OCC_CHECK(p.BN == 256 && N % 256 == 0, "gemm_tc_blocked256: N must be a multiple of 256 with 256-wide tiles");
-    return launch<bf16, false>(A, nullptr, 0, W, bias, nullptr, C, LnArgs{}, M, N, K, ACT_NONE, stream, true, 0, 0, head_major);
+    return launch<bf16, false>(A, nullptr, 0, W, bias, nullptr, C, LnArgs{}, M, N, K, ACT_NONE, stream, true);
 }
 
 // residual, y_f32 and pos are in the T32 block layout (elementwise.cu), rows padded to a multiple of 32
@@ -450,7 +437,7 @@ int gemm_tc_tsa_inputs(const bf16* const* Av, int nv, const bf16* Wv, const floa
     int smem = 0, sm = 0, begin = 0;
     for (int i = 0; i < nv; ++i) {
         if (build_prob<bf16, false>(probs.p[i], sm, Av[i], nullptr, 0, Wv, bv, nullptr, Cv[i], M, 256, 256, ACT_NONE, false, 0, 0,
-                                    false, cv, begin)) return 1;
+                                    cv, begin)) return 1;
         begin += probs.p[i].cta_count;
         smem = sm > smem ? sm : smem;
     }
@@ -458,7 +445,7 @@ int gemm_tc_tsa_inputs(const bf16* const* Av, int nv, const bf16* Wv, const floa
     // rq_t32: the epilogue constant in the T32 layout, added before the 16-bit rounding; otherwise the row-major fp32 rq
     const bool t32 = rq_t32 != nullptr && M % 32 == 0;
     if (build_prob<bf16, false>(probs.p[nv], sm, Aq, Aq2, K1q, Wq, bq, t32 ? nullptr : rq, reinterpret_cast<bf16*>(Cq), M, Nq, Kq,
-                                ACT_NONE, false, 0, 0, false, cq, begin)) return 1;
+                                ACT_NONE, false, 0, 0, cq, begin)) return 1;
     probs.p[nv].out_half = 1;
     if (t32) probs.p[nv].res_t32 = rq_t32;
     smem = sm > smem ? sm : smem;
