@@ -195,6 +195,36 @@ int occb200_layernorm_f32(const float* x, const float* gamma, const float* beta,
 /* tensor-core bf16 GEMM self-test entry: C f32 [M,N] = A bf16 [M,K] . W bf16 [N,K]^T (+bias); used by tests */
 int occb200_gemm_bf16_tc(const void* A_bf16, const void* W_bf16, const float* bias, float* C, int M, int N, int K,
                          void* stream);
+/* The tensor-core GEMM (wgmma, bf16 operands, fp32 accumulation) in each of its variants, for operator tests.  Every
+ * operand is a dense row-major device array; bias [N] and residual [M,N] are fp32 and may be NULL.  Unsupported shapes,
+ * bad codes and NULL required pointers return an error before any CUDA call.
+ *   gemm_tc: C [M,N] = act(A . W^T + bias) (+ residual), out_dtype 0 fp32, 1 bf16, 2 fp16; act 0 none / 1 relu.
+ *     A bf16 [M,K], or with A2 != NULL the concatenation [A (M x K1) | A2 (M x (K - K1))] along K.  W bf16 [N,K].
+ *     M > 0, N % 64 == 0, K % 64 == 0; with A2: K1 % 64 == 0 and 0 < K1 < K. */
+int occb200_gemm_tc(const void* A, const void* A2, int K1, const void* W, const float* bias, const float* residual, void* C,
+                    int out_dtype, int M, int N, int K, int act, void* stream);
+/*   gemm_tc_ln: x = A . W^T + bias + residual, N = 256, y = LayerNorm(x) * gamma + beta (eps 1e-5).  residual, pos and y_f32 are
+ *     fp32 in the T32 block layout (32 x 32 blocks of [col % 32 / 4][row % 32][4], rows padded to a multiple of 32); y_bf16 = bf16(y)
+ *     and y_pos_bf16 = bf16(y + pos) are row-major [M,256].  Outputs may be NULL; y_pos_bf16 needs pos. */
+int occb200_gemm_tc_ln(const void* A, const void* W, const float* bias, const float* residual, const float* gamma,
+                       const float* beta, const float* pos, float* y_f32, void* y_bf16, void* y_pos_bf16, int M, int K,
+                       void* stream);
+/*   gemm_tc_blocked256: C = A . W^T + bias with N % 256 == 0, written as N / 256 bf16 matrices [M,256] at C + i * M * 256. */
+int occb200_gemm_tc_blocked256(const void* A, const void* W, const float* bias, void* C, int M, int N, int K, void* stream);
+/*   gemm_tc_tsa_inputs: one launch of nv (1 or 2) value problems Cv[i] = bf16(Av[i] . Wv^T + bv) ([M,256], K = 256) and the
+ *     projection Cq = fp16([Aq | Aq2] . Wq^T + bq + constant) ([M,Nq], K = Kq, split at K1q when Aq2 != NULL).  The fp32 constant
+ *     is rq_t32 (T32 layout) when given and M % 32 == 0, else rq (row-major [M,Nq]); rq_t32 needs rq.  Av, Cv: HOST arrays of nv
+ *     device pointers.  bv, bq, rq may be NULL. */
+int occb200_gemm_tc_tsa_inputs(const void* const* Av, int nv, const void* Wv, const float* bv, void* const* Cv, const void* Aq,
+                               const void* Aq2, int K1q, const void* Wq, const float* bq, const float* rq, const float* rq_t32,
+                               void* Cq, int M, int Nq, int Kq, void* stream);
+/*   gemm_tc_split3: fp32-grade product C f32 [M,N] = act(S_hi . W_hi^T + S_lo . W_hi^T + S_hi . W_lo^T + bias) (+ residual) from
+ *     S = [hi | lo] bf16 [M, 2 Ks] and W3 = [W_hi | W_hi | W_lo] bf16 [N, 3 Ks]; Ks % 64 == 0.
+ *   split_bf16: S [rows, 2 (Ka + Kb)] bf16, row r = [hi(a[r]) hi(b[r]) | lo(a[r]) lo(b[r])], hi = bf16(x), lo = bf16(x - hi);
+ *     a f32 [rows, Ka], b f32 [rows, Kb] or NULL with Kb = 0; Ka, Kb multiples of 8. */
+int occb200_gemm_tc_split3(const void* S, int Ks, const void* W3, const float* bias, const float* residual, float* C, int M, int N,
+                           int act, void* stream);
+int occb200_split_bf16(const float* a, int Ka, const float* b, int Kb, int64_t rows, void* S, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Image backbone + neck (SURVEY 8f rank 1, the step immediately BEFORE the hot path); parity vs its oracle:

@@ -1214,4 +1214,72 @@ int occb200_gemm_bf16_tc(const void* A, const void* W, const float* bias, float*
                           C, M, N, K, ACT_NONE, (cudaStream_t)stream);
 }
 
+// ---- tensor-core GEMM variants for kernel tests: argument checks only, every rejection before the first CUDA call
+int occb200_gemm_tc(const void* A, const void* A2, int K1, const void* W, const float* bias, const float* residual, void* C,
+                    int out_dtype, int M, int N, int K, int act, void* stream)
+{
+    OCC_CHECK(A && W && C, "null pointer");
+    OCC_CHECK(out_dtype >= 0 && out_dtype <= 2, "out_dtype must be 0 (fp32), 1 (bf16) or 2 (fp16)");
+    OCC_CHECK(act == ACT_NONE || act == ACT_RELU, "act must be 0 (none) or 1 (relu)");
+    OCC_CHECK(K > 0 && (A2 == nullptr || K1 < K) && gemm_tc_supported(M, N, K, A2 ? K1 : K),
+              "shape not supported by the tensor-core GEMM (M > 0, N % 64, K % 64, K1 % 64, 0 < K1 < K)");
+    const bf16 *a = reinterpret_cast<const bf16*>(A), *a2 = reinterpret_cast<const bf16*>(A2), *w = reinterpret_cast<const bf16*>(W);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (out_dtype == 0) return gemm_tc<float>(a, a2, K1, w, bias, residual, reinterpret_cast<float*>(C), M, N, K, act, st);
+    if (out_dtype == 1) return gemm_tc<bf16>(a, a2, K1, w, bias, residual, reinterpret_cast<bf16*>(C), M, N, K, act, st);
+    return gemm_tc<__half>(a, a2, K1, w, bias, residual, reinterpret_cast<__half*>(C), M, N, K, act, st);
+}
+
+int occb200_gemm_tc_ln(const void* A, const void* W, const float* bias, const float* residual, const float* gamma,
+                       const float* beta, const float* pos, float* y_f32, void* y_bf16, void* y_pos_bf16, int M, int K,
+                       void* stream)
+{
+    OCC_CHECK(A && W && bias && residual && gamma && beta, "null pointer");
+    OCC_CHECK(y_pos_bf16 == nullptr || pos != nullptr, "y_pos_bf16 needs pos");
+    OCC_CHECK(M > 0 && K > 0 && K % 64 == 0, "shape not supported by the LayerNorm GEMM (M > 0, K % 64)");
+    return gemm_tc_ln(reinterpret_cast<const bf16*>(A), reinterpret_cast<const bf16*>(W), bias, residual, gamma, beta, pos, y_f32,
+                      reinterpret_cast<bf16*>(y_bf16), reinterpret_cast<bf16*>(y_pos_bf16), M, K, (cudaStream_t)stream);
+}
+
+int occb200_gemm_tc_blocked256(const void* A, const void* W, const float* bias, void* C, int M, int N, int K, void* stream)
+{
+    OCC_CHECK(A && W && C, "null pointer");
+    OCC_CHECK(K > 0 && N % 256 == 0 && gemm_tc_supported(M, N, K, K), "shape not supported (M > 0, N % 256, K % 64)");
+    return gemm_tc_blocked256(reinterpret_cast<const bf16*>(A), reinterpret_cast<const bf16*>(W), bias, reinterpret_cast<bf16*>(C),
+                              M, N, K, (cudaStream_t)stream);
+}
+
+int occb200_gemm_tc_tsa_inputs(const void* const* Av, int nv, const void* Wv, const float* bv, void* const* Cv, const void* Aq,
+                               const void* Aq2, int K1q, const void* Wq, const float* bq, const float* rq, const float* rq_t32,
+                               void* Cq, int M, int Nq, int Kq, void* stream)
+{
+    OCC_CHECK(nv >= 1 && nv <= 2, "nv must be 1 or 2");
+    OCC_CHECK(Av && Cv && Wv && Aq && Wq && Cq, "null pointer");
+    for (int i = 0; i < nv; ++i) OCC_CHECK(Av[i] && Cv[i], "null value operand / output");
+    OCC_CHECK(rq_t32 == nullptr || rq != nullptr, "rq_t32 needs the row-major rq (used when M % 32 != 0)");
+    OCC_CHECK(gemm_tc_supported(M, 256, 256, 256), "shape not supported (M > 0)");
+    OCC_CHECK(Kq > 0 && (Aq2 == nullptr || K1q < Kq) && gemm_tc_supported(M, Nq, Kq, Aq2 ? K1q : Kq),
+              "projection shape not supported (Nq % 64, Kq % 64, K1q % 64, 0 < K1q < Kq)");
+    return gemm_tc_tsa_inputs(reinterpret_cast<const bf16* const*>(Av), nv, reinterpret_cast<const bf16*>(Wv), bv,
+                              reinterpret_cast<bf16* const*>(Cv), reinterpret_cast<const bf16*>(Aq), reinterpret_cast<const bf16*>(Aq2), K1q, reinterpret_cast<const bf16*>(Wq), bq, rq, rq_t32,
+                              reinterpret_cast<__half*>(Cq), M, Nq, Kq, (cudaStream_t)stream);
+}
+
+int occb200_gemm_tc_split3(const void* S, int Ks, const void* W3, const float* bias, const float* residual, float* C, int M, int N,
+                           int act, void* stream)
+{
+    OCC_CHECK(S && W3 && C, "null pointer");
+    OCC_CHECK(act == ACT_NONE || act == ACT_RELU, "act must be 0 (none) or 1 (relu)");
+    OCC_CHECK(Ks > 0 && gemm_tc_supported(M, N, 3 * Ks, 2 * Ks), "shape not supported (M > 0, N % 64, Ks % 64)");
+    return gemm_tc_split3(reinterpret_cast<const bf16*>(S), Ks, reinterpret_cast<const bf16*>(W3), bias, residual, C, M, N, act,
+                          (cudaStream_t)stream);
+}
+
+int occb200_split_bf16(const float* a, int Ka, const float* b, int Kb, int64_t rows, void* S, void* stream)
+{
+    OCC_CHECK(a && S && (Kb == 0 || b), "null pointer");
+    OCC_CHECK(rows >= 0 && Ka > 0 && Kb >= 0 && Ka % 8 == 0 && Kb % 8 == 0, "Ka, Kb must be multiples of 8");
+    return launch_split_bf16(a, Ka, b, Kb, rows, reinterpret_cast<bf16*>(S), (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -4,7 +4,7 @@
 
 namespace occ {
 
-// shapes the tensor-core kernel handles: K % 64 == 0 (and the split point K1 % 64 == 0), N % 16 == 0, N <= 256 per pass
+// shapes the tensor-core kernel handles: K % 64 == 0 (and the split point K1 % 64 == 0), N % 64 == 0, N <= 256 per pass
 bool gemm_tc_supported(int M, int N, int K, int K1);
 
 template <typename TC>

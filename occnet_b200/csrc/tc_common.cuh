@@ -170,9 +170,11 @@ __device__ __forceinline__ uint32_t pack_16(float a, float b, bool half)
 
 // LayerNorm epilogue of a 64 x 256 warpgroup tile (acc: 4 x wgmma.m64n64 fragments; rows r0 and r0 + 8 of this thread, columns
 // 8 j + quad_col (+ 1) of every 64-column sub-tile).  x = acc + bias + residual (T32), y = LN(x) over the 256 columns of a row,
-// whose statistics are reduced over the 4 threads of a quad; cvec = [bias | gamma | beta] in shared memory.  Writes y (fp32 T32),
+// whose statistics are reduced over the 4 threads of a quad (one pass, or two where the mean is large against the spread);
+// cvec = [bias | gamma | beta] in shared memory.  Writes y (fp32 T32),
 // bf16 y and bf16 y + pos (row-major [M, 256]) where the pointers are set.  The residual is read with plain (coherent) loads:
 // it may have been written earlier in the same launch.
+constexpr float LN_ONE_PASS_R2 = 16.f;
 __device__ __forceinline__ void ln_epilogue(float (&acc)[4][32], int r0, int row_end, int quad_col, const float* cvec,
                                             const float* residual, const float* pos, float* y_f32, bf16* y_bf16, bf16* y_pos_bf16)
 {
@@ -201,7 +203,25 @@ __device__ __forceinline__ void ln_epilogue(float (&acc)[4][32], int r0, int row
         sum += __shfl_xor_sync(0xffffffffu, sum, 1); sum += __shfl_xor_sync(0xffffffffu, sum, 2);
         sumsq += __shfl_xor_sync(0xffffffffu, sumsq, 1); sumsq += __shfl_xor_sync(0xffffffffu, sumsq, 2);
         mean[h] = sum * (1.f / 256.f);
-        const float var = fmaxf(sumsq * (1.f / 256.f) - mean[h] * mean[h], 0.f);
+        float var = fmaxf(sumsq * (1.f / 256.f) - mean[h] * mean[h], 0.f);
+        // The one-pass variance cancels when |mean| >> std: its relative error grows like (mean / std)^2.  Rows with
+        // mean^2 > 16 var take a second pass over the registers, sum((x - mean)^2) as layernorm256 computes it; below that
+        // bound the one-pass error stays under 3e-5 relative.  The branch is warp-uniform (the quad shuffles need the whole
+        // warp), so warps without such a row skip the second pass.
+        const bool two_pass = mean[h] * mean[h] > LN_ONE_PASS_R2 * var;
+        if (__any_sync(0xffffffffu, two_pass)) {
+            float ss = 0.f;
+#pragma unroll
+            for (int ns = 0; ns < 4; ++ns) {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const float d0 = acc[ns][4 * j + 2 * h] - mean[h], d1 = acc[ns][4 * j + 2 * h + 1] - mean[h];
+                    ss = fmaf(d0, d0, fmaf(d1, d1, ss));
+                }
+            }
+            ss += __shfl_xor_sync(0xffffffffu, ss, 1); ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+            if (two_pass) var = ss * (1.f / 256.f);
+        }
         rstd[h] = rsqrtf(var + 1e-5f);
     }
 #pragma unroll
