@@ -101,7 +101,10 @@ int occb200_engine_set_cameras(occb200_engine* e, const float* cam_mat, const fl
  * rotate(prev_bev as (C,H,W), can_bus[-1] degrees, center=rotate_center), nearest, zero fill).  A nearest-neighbour
  * rotation is a row permutation of the (Nq, C) BEV: map_host[q] (HOST int32 [Nq]) = source BEV cell of output cell q,
  * -1 = outside (zeros).  The engine applies it while casting prev_bev to the GEMM operand type -- prev_bev is then
- * passed UN-rotated to occb200_engine_forward.  NULL clears it (prev_bev is taken as already rotated).  Synchronous. */
+ * passed UN-rotated to occb200_engine_forward.  NULL clears it (prev_bev is taken as already rotated).  Synchronous.
+ * The map lives in ONE engine-global device buffer written by a blocking copy: a frame still queued on a non-blocking
+ * stream may read the new map, so change it only when no frame is in flight.  The video calls below ignore it (they take a
+ * map per frame). */
 int occb200_engine_set_prev_rotation(occb200_engine* e, const int32_t* map_host);
 
 /* Element type / layout of the feature levels handed to _forward / _forward_host / _submit_host from now on (pointers
@@ -145,6 +148,40 @@ int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_hos
 int occb200_engine_submit_host(occb200_engine* e, int slot, const float* const* feats_host, int64_t* occ_cls_i64_host,
                                float* flow_host, void* stream);
 int occb200_engine_wait_host(occb200_engine* e, int slot);
+
+/* Temporal (video) inference with the BEV history kept inside the engine (BEVFormer's prev_bev, transformer_occ.py:189-205).
+ *
+ * _set_history(e, 1) allocates the history: ONE [Nq, 256] row-major buffer in the storage precision (bf16; fp32 for
+ * precision 0), 20.5 MB / 41 MB at 200 x 200.  _set_history(e, 0) frees it.  Both wait for queued video frames first, and
+ * both start a new scene.  Synchronous.
+ *
+ * Only _forward_video and _submit_host_video read or write the history; _forward, _forward_host and _submit_host never touch
+ * it.  A video frame
+ *   - runs in self mode (prev_bev = None) when scene_start != 0 or no video frame has run since _set_history(e, 1): bit-identical
+ *     to occb200_engine_forward(prev_bev = NULL);
+ *   - otherwise takes prev_bev = the history gathered through the rotation map (NULL = no rotation): bit-identical to
+ *     occb200_engine_forward(prev_bev = the previous video frame's bev_embed) after occb200_engine_set_prev_rotation(map).
+ *     The history holds the last LayerNorm's storage-type copy of bev_embed, which is exactly what that call's gather makes
+ *     of the fp32 bev_embed;
+ *   - leaves its own final BEV in the history, whether or not bev_embed is requested;
+ *   - waits for the previous video frame's history write (an event), so the caller may switch streams between frames.
+ * The map is the per-frame form of occb200_engine_set_prev_rotation's (source cell of every cell, -1 = outside); the
+ * engine-global map of that call is ignored here.
+ *
+ * _forward_video: device buffers, the outputs of occb200_engine_forward (any may be NULL).  rot_map_dev: dev int32 [Nq] or
+ *   NULL; it is not checked on the host, so an entry outside [-1, Nq) is read as -1 (a row of zeros), never out of bounds.
+ * _submit_host_video: the pipelined host-buffer call (occb200_engine_submit_host), completed by occb200_engine_wait_host.
+ *   rot_map_host: HOST int32 [Nq] or NULL, checked like occb200_engine_set_prev_rotation's, then staged in a slot-owned pinned
+ *   buffer and uploaded on the slot's copy stream: the caller may reuse its array as soon as the call returns.
+ * All four input dtypes work (set_input_dtype).  A call without _set_history(e, 1), with a NULL pointer, a bad or busy slot or an
+ * out-of-range host map returns 1 before any CUDA call and leaves the history unchanged.  occb200_engine_launches_per_frame
+ * counts the video frame's launches. */
+int occb200_engine_set_history(occb200_engine* e, int enable);
+int occb200_engine_forward_video(occb200_engine* e, const float* const* feats, const int32_t* rot_map_dev, int scene_start,
+                                 float* bev_embed, float* occ_logits, float* flow, uint8_t* occ_cls_u8, int64_t* occ_cls_i64,
+                                 void* stream);
+int occb200_engine_submit_host_video(occb200_engine* e, int slot, const float* const* feats_host, const int32_t* rot_map_host,
+                                     int scene_start, int64_t* occ_cls_i64_host, float* flow_host, void* stream);
 
 /* Intermediate taps for parity tests (dev f32, valid after a forward; NULL if not produced):
  *   which: 0 = layer output [Nq,C] of layer `layer`; 1 = TSA output (pre-norm, with residual); 2 = SCA output

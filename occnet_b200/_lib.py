@@ -39,6 +39,9 @@ SIGNATURES = {
     'occb200_engine_forward_host': (_i, [_vp, ctypes.POINTER(_vp), _vp, _vp, _vp]),
     'occb200_engine_submit_host': (_i, [_vp, _i, ctypes.POINTER(_vp), _vp, _vp, _vp]),
     'occb200_engine_wait_host': (_i, [_vp, _i]),
+    'occb200_engine_set_history': (_i, [_vp, _i]),
+    'occb200_engine_forward_video': (_i, [_vp, ctypes.POINTER(_vp), _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'occb200_engine_submit_host_video': (_i, [_vp, _i, ctypes.POINTER(_vp), _vp, _i, _vp, _vp, _vp]),
     'occb200_engine_enable_taps': (_i, [_vp, _i]),
     'occb200_engine_copy_tap': (_i, [_vp, _i, _i, _vp, _vp]),
     'occb200_engine_project_pillars': (_i, [_vp, _vp, _vp, _vp]),

@@ -374,6 +374,34 @@ int launch_gather_rows(const float* src, const int32_t* map, int rows, int C, T*
 }
 template int launch_gather_rows<float>(const float*, const int32_t*, int, int, float*, float*, cudaStream_t);
 template int launch_gather_rows<bf16>(const float*, const int32_t*, int, int, bf16*, float*, cudaStream_t);
+
+// ---- the same rotation from the engine-owned BEV history, already in the storage type: a pure row permutation (16 bytes
+//      per thread, no conversion).  The map may come straight from the caller's device memory, so an entry outside
+//      [-1, rows) reads as -1 (zeros) instead of out of bounds.
+namespace {
+__global__ void gather_rows16_kernel(const uint4* __restrict__ src, const int32_t* __restrict__ map, int rows, int per_row,
+                                     uint4* __restrict__ dst)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (int64_t)rows * per_row) return;
+    const int r = (int)(i / per_row), c = (int)(i % per_row);
+    const int sr = map ? __ldg(map + r) : r;
+    dst[i] = (sr >= 0 && sr < rows) ? __ldg(src + (int64_t)sr * per_row + c) : make_uint4(0u, 0u, 0u, 0u);
+}
+}  // namespace
+template <typename T>
+int launch_gather_rows_stored(const T* src, const int32_t* map, int rows, int C, T* dst, cudaStream_t stream)
+{
+    OCC_CHECK((C * sizeof(T)) % 16 == 0, "gather_rows_stored: rows must be a multiple of 16 bytes");
+    const int per_row = (int)(C * sizeof(T) / 16);
+    const int64_t n = (int64_t)rows * per_row;
+    gather_rows16_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(src), map, rows, per_row,
+                                                                reinterpret_cast<uint4*>(dst));
+    OCC_CUDA(cudaGetLastError());
+    return 0;
+}
+template int launch_gather_rows_stored<float>(const float*, const int32_t*, int, int, float*, cudaStream_t);
+template int launch_gather_rows_stored<bf16>(const bf16*, const int32_t*, int, int, bf16*, cudaStream_t);
 }  // namespace occ
 
 // ---- feature packing from channels-last bf16 levels [num_cams, h, w, C] (what occb200_backbone_forward_nhwc_bf16 writes):

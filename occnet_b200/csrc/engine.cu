@@ -67,6 +67,12 @@ struct occb200_engine {
     bool cameras_set = false, finalized = false, taps = false;
     DevBuf rot_map;                     // occb200_engine_set_prev_rotation: source row of every BEV cell (int32, -1 = outside)
     bool rot_set = false;
+    // occb200_engine_set_history: the last video frame's final BEV [Nq, 256] in the storage type (the bf16 / fp32 copy the last
+    // LayerNorm writes), read and written only by the video calls; hist_done is recorded after every video frame
+    DevBuf hist;
+    bool hist_valid = false;            // a video frame has written it since set_history(e, 1)
+    cudaEvent_t hist_done = nullptr;
+    bool hist_recorded = false;
     int feats_bf16 = 0;                 // occb200_engine_set_input_dtype: feature levels arrive as bf16 instead of fp32
     // input dtype 3 (uint8 camera frames): the attached backbone (borrowed), the levels it hands over (shared by both host
     // slots, like its workspace) and the event after the last frame that read them
@@ -86,9 +92,12 @@ struct occb200_engine {
     DevBuf conv_w[2], conv_b[2], conv_wh[2];
     DevBuf conv_wh_hi[2], conv_wh_lo[2], vox_split;      // fp32 storage + tensor cores: bf16 hi / lo split of the folded conv weights, [hi | lo] voxel operand
     DevBuf sca_v_all_wh, sca_v_all_b, sca_value_all;     // value_proj of every layer, concatenated (tensor-core path)
+    // TSA queue 1 with a previous BEV (encoder.py:204-209 stacks the layer-0 query once): value_proj_l(bev_queries) of every
+    // layer, [L][Nq,256] in the storage type -- parameters only, computed at finalize by the frame path's own GEMM
+    DevBuf tsa_v_query;
     DevBuf hw1, hb1, hw2, hb2, fw1, fb1, fw2, fb2, head_w1h, head_w2h, head_b1c, head_b2c;
     // workspace
-    DevBuf tokens, sca_value, q_f32, q_t, q_pos_t, q0_t, prev_t, tsa_value, tsa_value_prev, qproj, attn_out, x_f32,
+    DevBuf tokens, sca_value, q_f32, q_t, q_pos_t, prev_t, tsa_value, qproj, attn_out, x_f32,
         ffn_h, vox0, vox1, vox2, hits;
     DevBuf tap_layer, tap_tsa, tap_sca;
     // fp32-grade tensor-core configuration (precision 0 + use_tensor_cores): bf16 [hi | lo] splits of the GEMM operands
@@ -98,6 +107,8 @@ struct occb200_engine {
     // pipelined host-buffer variant: 2 slots, copies on their own streams, compute on the caller's stream
     struct Slot {
         DevBuf feats[4], occ, flow;
+        DevBuf rot;                     // _submit_host_video: the frame's rotation map, uploaded from rot_pinned on h2d_stream[0]
+        int32_t* rot_pinned = nullptr;
         cudaEvent_t h2d_done[4] = {nullptr, nullptr, nullptr, nullptr}, compute_done = nullptr, d2h_done = nullptr;
         bool busy = false;
     } slots[2];
@@ -228,11 +239,39 @@ int gemm_ln_fused(occb200_engine* e, const bf16* A, const void* Wh, const float*
     return gemm_tc_ln(A, reinterpret_cast<const bf16*>(Wh), bias, residual, gamma, beta, pos, y_f32, y_t, y_pos_t, M, K, st);
 }
 
+// TSA's queue-1 value maps value_proj_l(bev_queries) for every layer, with the GEMM the frame path would run on the same
+// operand (bf16 tensor cores: rows do not depend on how problems share a launch, so they equal the merged TSA-input launch's)
+template <typename T>
+int build_tsa_query_values(occb200_engine* e)
+{
+    const int Nq = e->Nq, C = 256;
+    DevBuf q0;
+    if (q0.alloc((size_t)Nq * C * sizeof(T)) || e->tsa_v_query.alloc((size_t)e->cfg.num_layers * Nq * C * sizeof(T))) return 2;
+    if (launch_cast<T>(e->bev_queries.as<float>(), q0.as<T>(), (int64_t)Nq * C, 0)) return 2;
+    for (int l = 0; l < e->cfg.num_layers; ++l) {
+        LayerW& w = e->layers[l];
+        if (gemm<T, T>(e, q0.as<T>(), nullptr, 0, w.tsa_v_w.as<float>(), w.tsa_v_wh.p, w.tsa_v_b.as<float>(), nullptr,
+                       e->tsa_v_query.as<T>() + (size_t)l * Nq * C, Nq, C, C, ACT_NONE, 0)) return 2;
+    }
+    OCC_CUDA(cudaDeviceSynchronize());
+    q0.release();
+    return 0;
+}
+
 enum { MODE_FRAME = 0, MODE_L0_TSA_ONLY = 1 };
+
+// A video frame (occb200_engine_forward_video / _submit_host_video): with `prev`, the previous BEV is the engine history
+// gathered through `map` (NULL = no rotation) instead of a caller's fp32 prev_bev; either way the frame's last LayerNorm
+// writes its storage-type copy of the final BEV into the history.
+struct VideoArgs {
+    bool prev = false;
+    const int32_t* map = nullptr;
+};
 
 template <typename T>
 int forward_impl(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed,
-                 float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, int mode = MODE_FRAME)
+                 float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, int mode = MODE_FRAME,
+                 const VideoArgs* video = nullptr)
 {
     const occb200_config& c = e->cfg;
     const int Nq = e->Nq, Nv = e->Nv, C = 256, ncam = c.num_cams;
@@ -284,23 +323,20 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
         q_f32 = x_f32;
         x_f32 = (old == cbuf) ? spare_f32 : old;
     };
-    const bool has_prev = prev_bev != nullptr;
-    const T* q0_t = nullptr;
+    const bool from_hist = video != nullptr && video->prev;
+    const bool has_prev = prev_bev != nullptr || from_hist;
     if (has_prev) {
         // encoder.py:204-209: value = stack([prev_bev, bev_query]) built ONCE before the layer loop, so
         // queue 1 keeps seeing the layer-0 query in every layer.
         // (transformer_occ.py:195-205) the rotation of prev_bev about rotate_center is a nearest-neighbour row permutation:
-        // applied here, fused with the operand cast, from the index map set by occb200_engine_set_prev_rotation
-        if (launch_gather_rows<T>(prev_bev, e->rot_set ? e->rot_map.as<int32_t>() : nullptr, Nq, C, e->prev_t.as<T>(), nullptr, st))
+        // applied here, fused with the operand cast, from the index map set by occb200_engine_set_prev_rotation.  The
+        // history already holds the operand rounding of the previous bev_embed, so gathering it gives the same operand.
+        if (from_hist) {
+            if (launch_gather_rows_stored<T>(e->hist.as<T>(), video->map, Nq, C, e->prev_t.as<T>(), st)) return 2;
+        } else if (launch_gather_rows<T>(prev_bev, e->rot_set ? e->rot_map.as<int32_t>() : nullptr, Nq, C, e->prev_t.as<T>(),
+                                         nullptr, st))
             return 2;
         e->launches++;
-        if (const_q) {
-            q0_t = e->qc_t.as<T>();
-        } else {
-            if (launch_cast<T>(e->bev_queries.as<float>(), e->q0_t.as<T>(), (int64_t)Nq * C, st)) return 2;
-            e->launches++;
-            q0_t = e->q0_t.as<T>();
-        }
     }
     // sampling offsets / attention logits: fp16 on the tensor-core path (half the bytes between the projection GEMM and
     // the gather kernel; |offset| is a few pixels, so fp16's 11-bit mantissa keeps locations to < 0.01 px), fp32 otherwise
@@ -334,22 +370,25 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
             q_t_in = e->l0_q_t.as<T>();
             q_in = q_t; q_pos_in = q_pos_t;
         } else {
-            T* v_cur = e->tsa_value.as<T>();
-            T* v_prev = has_prev ? e->tsa_value_prev.as<T>() : v_cur;
-            // value_proj of every queue entry + the sampling projection are independent GEMMs over [Nq,256] operands: ONE
-            // launch on disjoint CTA ranges on the fused tensor-core path, one launch each otherwise
+            // one value map per layer and frame: the current query's in self mode (queue 0 = queue 1), prev_bev's with a
+            // previous BEV, whose queue-1 map value_proj_l(bev_queries) was computed once at finalize
+            const T* a_v = has_prev ? e->prev_t.as<T>() : q_in;
+            T* v_prev = e->tsa_value.as<T>();
+            const T* v_cur = has_prev ? e->tsa_v_query.as<T>() + (size_t)l * Nq * C : v_prev;
+            // the value map + the sampling projection are independent GEMMs over [Nq,256] operands: ONE launch on disjoint
+            // CTA ranges on the fused tensor-core path, one launch each otherwise
             const bool tsa_merge = sizeof(T) == 2 && fuse_ln && q_half && w.tsa_v_wh.p != nullptr;
             if (tsa_merge) {
                 if constexpr (sizeof(T) == 2) {
-                    const bf16* Av[2] = {reinterpret_cast<const bf16*>(has_prev ? q0_t : q_in), e->prev_t.as<bf16>()};
-                    bf16* Cv[2] = {reinterpret_cast<bf16*>(v_cur), reinterpret_cast<bf16*>(v_prev)};
+                    const bf16* Av[1] = {reinterpret_cast<const bf16*>(a_v)};
+                    bf16* Cv[1] = {reinterpret_cast<bf16*>(v_prev)};
                     e->launches++;
                     ProfScope ps(e, st, CAT_GEMM);
                     const int rc = fold_pos
                         ? gemm_tc_tsa_inputs(Av, 1, w.tsa_v_wh.as<bf16>(), w.tsa_v_b.as<float>(), Cv, reinterpret_cast<const bf16*>(q_in),
                                              nullptr, C, w.tsa_q_wh_fold.as<bf16>(), nullptr, w.tsa_q_const.as<float>(),
                                              w.tsa_q_const_t32.as<float>(), (__half*)qproj, Nq, nq_tsa, C, st)
-                        : gemm_tc_tsa_inputs(Av, has_prev ? 2 : 1, w.tsa_v_wh.as<bf16>(), w.tsa_v_b.as<float>(), Cv,
+                        : gemm_tc_tsa_inputs(Av, 1, w.tsa_v_wh.as<bf16>(), w.tsa_v_b.as<float>(), Cv,
                                              reinterpret_cast<const bf16*>(has_prev ? e->prev_t.as<T>() : q_in),
                                              reinterpret_cast<const bf16*>(q_pos_in), C, w.tsa_q_wh.as<bf16>(), w.tsa_q_b.as<float>(),
                                              nullptr, nullptr, (__half*)qproj, Nq, nq_tsa, 2 * C, st);
@@ -360,8 +399,7 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
                     return gemm<T, T>(e, a, nullptr, 0, w.tsa_v_w.as<float>(), w.tsa_v_wh.p, w.tsa_v_b.as<float>(), nullptr, dst,
                                       Nq, C, C, ACT_NONE, st);
                 };
-                if (value_gemm(has_prev ? q0_t : q_in, v_cur)) return 2;
-                if (has_prev && value_gemm(e->prev_t.as<T>(), v_prev)) return 2;
+                if (value_gemm(a_v, v_prev)) return 2;
                 const T* qa = has_prev ? e->prev_t.as<T>() : q_in;
                 const int rc = q_half ? gemm<T, __half>(e, qa, q_pos_in, C, w.tsa_q_w.as<float>(), w.tsa_q_wh.p, w.tsa_q_b.as<float>(),
                                                         nullptr, (__half*)qproj, Nq, nq_tsa, 2 * C, ACT_NONE, st)
@@ -433,10 +471,12 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
         // ---- FFN (mmcv FFN: x + W2 relu(W1 x))
         if (gemm<T, T>(e, q_t, nullptr, 0, w.ffn1_w.as<float>(), w.ffn1_wh.p, w.ffn1_b.as<float>(), nullptr,
                        e->ffn_h.as<T>(), Nq, c.ffn_dim, C, ACT_RELU, st)) return 2;
+        // a video frame's last LayerNorm writes its storage-type copy straight into the history (q_t is not read afterwards)
+        T* y_t = video != nullptr && l == c.num_layers - 1 ? e->hist.as<T>() : q_t;
         if (fuse_ln) {
             const bool need_qpos = !fold_pos;                // only the unfolded TSA query projection reads q + pos
             if (gemm_ln_fused(e, e->ffn_h.as<bf16>(), w.ffn2_wh.p, w.ffn2_b.as<float>(), q_f32, w.ln_g[2].as<float>(),
-                              w.ln_b[2].as<float>(), need_qpos ? e->pos_t32.as<float>() : nullptr, x_f32, (bf16*)q_t,
+                              w.ln_b[2].as<float>(), need_qpos ? e->pos_t32.as<float>() : nullptr, x_f32, (bf16*)y_t,
                               need_qpos ? (bf16*)q_pos_t : nullptr, Nq, c.ffn_dim, st))
                 return 2;
             advance();
@@ -445,7 +485,7 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
                                q_f32, x_f32, Nq, C, c.ffn_dim, ACT_NONE, st)) return 2;
             {
                 ProfScope ps(e, st, CAT_LN);
-                if (launch_layernorm<T>(x_f32, w.ln_g[2].as<float>(), w.ln_b[2].as<float>(), pos, Nq, C, q_f32, q_t,
+                if (launch_layernorm<T>(x_f32, w.ln_g[2].as<float>(), w.ln_b[2].as<float>(), pos, Nq, C, q_f32, y_t,
                                         q_pos_t, st)) return 2;
             }
             e->launches++;
@@ -547,7 +587,7 @@ size_t frame_bytes(const occb200_engine* e)
 
 template <typename T>
 int forward_frames_impl(occb200_engine* e, const uint8_t* frames, const float* prev_bev, float* bev_embed, float* occ_logits,
-                        float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st)
+                        float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video)
 {
     const BackboneInfo bi = backbone_info(e->bb);
     const bool cl = e->cfg.precision == 1 && bi.precision == 1;   // bf16 -> bf16: channels-last hand-over (input dtype 2)
@@ -566,12 +606,57 @@ int forward_frames_impl(occb200_engine* e, const uint8_t* frames, const float* p
     const float* feats[4] = {(const float*)lv[0], (const float*)lv[1], (const float*)lv[2], (const float*)lv[3]};
     const int code = e->feats_bf16;
     e->feats_bf16 = cl ? 2 : 0;
-    rc = forward_impl<T>(e, feats, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st);
+    rc = forward_impl<T>(e, feats, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, MODE_FRAME, video);
     e->feats_bf16 = code;
     if (rc) return rc;
     OCC_CUDA(cudaEventRecord(e->bb_free, st));
     e->bb_free_recorded = true;
     e->launches += bb_launches;
+    return 0;
+}
+
+// Host-side checks of a device-buffer frame: error 1, nothing enqueued.
+int check_frame(const occb200_engine* e, const float* const* feats)
+{
+    OCC_CHECK(e->finalized, "engine_finalize() has not been called");
+    OCC_CHECK(e->cameras_set, "engine_set_cameras() has not been called");
+    if (e->feats_bf16 == 3) {
+        OCC_CHECK(e->bb != nullptr, "input dtype 3 (camera frames) needs an attached backbone (occb200_engine_attach_backbone)");
+        OCC_CHECK(feats[0] != nullptr, "null frame buffer");
+        return check_backbone(e, e->bb) ? 1 : 0;
+    }
+    for (int l = 0; l < e->cfg.num_levels; ++l) OCC_CHECK(feats[l] != nullptr, "null feature level");
+    return 0;
+}
+
+int run_frame(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed, float* occ_logits,
+              float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video = nullptr)
+{
+    if (e->feats_bf16 == 3) {
+        const uint8_t* frames = reinterpret_cast<const uint8_t*>(feats[0]);
+        if (e->cfg.precision == 0)
+            return forward_frames_impl<float>(e, frames, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, video);
+        return forward_frames_impl<bf16>(e, frames, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, video);
+    }
+    if (e->cfg.precision == 0)
+        return forward_impl<float>(e, feats, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, MODE_FRAME, video);
+    return forward_impl<bf16>(e, feats, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, MODE_FRAME, video);
+}
+
+// One video frame on device buffers, after every host-side check has passed.  The frame waits for the previous video
+// frame (on whatever stream that ran) before it reads the history, and records hist_done after it has written it.
+int run_video_frame(occb200_engine* e, const float* const* feats, const int32_t* map_dev, int scene_start, float* bev_embed,
+                    float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st)
+{
+    VideoArgs v;
+    v.prev = scene_start == 0 && e->hist_valid;
+    v.map = map_dev;
+    if (e->hist_recorded) OCC_CUDA(cudaStreamWaitEvent(st, e->hist_done, 0));
+    const int rc = run_frame(e, feats, nullptr, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, &v);
+    if (rc) return rc;
+    OCC_CUDA(cudaEventRecord(e->hist_done, st));
+    e->hist_recorded = true;
+    e->hist_valid = true;
     return 0;
 }
 
@@ -656,19 +741,21 @@ void occb200_engine_destroy(occb200_engine* e)
                          &w.tsa_q_wh_fold, &w.tsa_q_const, &w.tsa_q_const_t32};
         for (DevBuf* b : all) b->release();
     }
-    DevBuf* all[] = {&e->rot_map, &e->split_ws, &e->tokens_split, &e->l0_x_f32, &e->l0_q_t, &e->pos_bf, &e->qc_f32, &e->qc_t, &e->qc_pos_t, &e->bev_queries, &e->pos, &e->pos_t32, &e->cams_embeds, &e->level_embeds, &e->conv_w[0], &e->conv_w[1],
+    DevBuf* all[] = {&e->rot_map, &e->hist, &e->split_ws, &e->tokens_split, &e->l0_x_f32, &e->l0_q_t, &e->pos_bf, &e->qc_f32, &e->qc_t, &e->qc_pos_t, &e->bev_queries, &e->pos, &e->pos_t32, &e->cams_embeds, &e->level_embeds, &e->conv_w[0], &e->conv_w[1],
                      &e->conv_b[0], &e->conv_b[1], &e->conv_wh[0], &e->conv_wh[1], &e->conv_wh_hi[0], &e->conv_wh_hi[1], &e->conv_wh_lo[0],
                      &e->conv_wh_lo[1], &e->vox_split, &e->sca_v_all_wh, &e->sca_v_all_b, &e->sca_value_all, &e->hw1, &e->hb1, &e->hw2, &e->hb2,
                      &e->fw1, &e->fb1, &e->fw2, &e->fb2, &e->head_w1h, &e->head_w2h, &e->head_b1c, &e->head_b2c, &e->tokens, &e->sca_value, &e->q_f32, &e->q_t,
-                     &e->q_pos_t, &e->q0_t, &e->prev_t, &e->tsa_value, &e->tsa_value_prev, &e->qproj, &e->attn_out,
+                     &e->q_pos_t, &e->prev_t, &e->tsa_value, &e->tsa_v_query, &e->qproj, &e->attn_out,
                      &e->x_f32, &e->ffn_h, &e->vox0, &e->vox1, &e->vox2, &e->hits, &e->tap_layer, &e->tap_tsa,
                      &e->tap_sca, &e->feats_dev[0], &e->feats_dev[1], &e->feats_dev[2], &e->feats_dev[3],
                      &e->occ_i64_dev, &e->flow_dev, &e->bb_levels[0], &e->bb_levels[1], &e->bb_levels[2], &e->bb_levels[3]};
     for (DevBuf* b : all) b->release();
     if (e->bb_free) cudaEventDestroy(e->bb_free);
+    if (e->hist_done) cudaEventDestroy(e->hist_done);
     for (auto& sl : e->slots) {
         for (auto& f : sl.feats) f.release();
-        sl.occ.release(); sl.flow.release();
+        sl.occ.release(); sl.flow.release(); sl.rot.release();
+        if (sl.rot_pinned) cudaFreeHost(sl.rot_pinned);
         if (sl.compute_done) {
             for (cudaEvent_t ev : sl.h2d_done) cudaEventDestroy(ev);
             cudaEventDestroy(sl.compute_done); cudaEventDestroy(sl.d2h_done);
@@ -898,9 +985,9 @@ int occb200_engine_finalize(occb200_engine* e)
     int maxq = 8 * c.num_levels * c.sca_points * 3;
     const size_t nq_pad = ((size_t)Nq + 127) / 128 * 128;
     if (e->tokens.alloc(ntok * C * es) || e->sca_value.alloc(ntok * C * es) || e->q_f32.alloc(nq_pad * C * 4) ||
-        e->q_t.alloc((size_t)Nq * C * es) || e->q_pos_t.alloc((size_t)Nq * C * es) || e->q0_t.alloc((size_t)Nq * C * es) ||
+        e->q_t.alloc((size_t)Nq * C * es) || e->q_pos_t.alloc((size_t)Nq * C * es) ||
         e->prev_t.alloc((size_t)Nq * C * es) || e->tsa_value.alloc((size_t)Nq * C * es) ||
-        e->tsa_value_prev.alloc((size_t)Nq * C * es) || e->qproj.alloc((size_t)Nq * maxq * 4) ||
+        e->qproj.alloc((size_t)Nq * maxq * 4) ||
         e->attn_out.alloc((size_t)Nq * C * es) || e->x_f32.alloc(nq_pad * C * 4) ||
         e->ffn_h.alloc((size_t)Nq * F * es) || e->vox0.alloc(nvox * mid * es) || e->vox1.alloc(nvox * od * es) ||
         e->vox2.alloc(nvox * od * es) || e->hits.alloc(Nq)) return 2;
@@ -912,6 +999,7 @@ int occb200_engine_finalize(occb200_engine* e)
         if (c.pillar_h == 16 && e->vox_split.alloc(nvox * 2 * od * 2)) return 2;
     }
     e->host_params.clear();
+    if ((c.precision == 0 ? build_tsa_query_values<float>(e) : build_tsa_query_values<bf16>(e))) return 2;
     e->l0_ready = false;
     if (tc && e->qc_f32.p != nullptr && getenv("OCC_NO_L0_FOLD") == nullptr) {
         // Layer 0's TemporalSelfAttention (value_proj, query projection over [bev_queries | pos], gather, output_proj) and
@@ -953,22 +1041,36 @@ int occb200_engine_forward(occb200_engine* e, const float* const* feats, const f
                            float* occ_logits, float* flow, uint8_t* occ_cls_u8, int64_t* occ_cls_i64, void* stream)
 {
     OCC_CHECK(e && feats, "null pointer");
-    OCC_CHECK(e->finalized, "engine_finalize() has not been called");
-    OCC_CHECK(e->cameras_set, "engine_set_cameras() has not been called");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (e->feats_bf16 == 3) {
-        OCC_CHECK(e->bb != nullptr, "input dtype 3 (camera frames) needs an attached backbone (occb200_engine_attach_backbone)");
-        OCC_CHECK(feats[0] != nullptr, "null frame buffer");
-        if (check_backbone(e, e->bb)) return 1;
-        const uint8_t* frames = reinterpret_cast<const uint8_t*>(feats[0]);
-        if (e->cfg.precision == 0)
-            return forward_frames_impl<float>(e, frames, prev_bev, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64, st);
-        return forward_frames_impl<bf16>(e, frames, prev_bev, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64, st);
+    if (check_frame(e, feats)) return 1;
+    return run_frame(e, feats, prev_bev, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64, (cudaStream_t)stream);
+}
+
+int occb200_engine_set_history(occb200_engine* e, int enable)
+{
+    OCC_CHECK(e, "null engine");
+    if (e->hist_recorded) OCC_CUDA(cudaEventSynchronize(e->hist_done));   // a queued video frame may still use the buffer
+    e->hist_recorded = false;
+    e->hist_valid = false;
+    if (!enable) {
+        e->hist.release();
+        return 0;
     }
-    for (int l = 0; l < e->cfg.num_levels; ++l) OCC_CHECK(feats[l] != nullptr, "null feature level");
-    if (e->cfg.precision == 0)
-        return forward_impl<float>(e, feats, prev_bev, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64, st);
-    return forward_impl<bf16>(e, feats, prev_bev, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64, st);
+    const size_t n = (size_t)e->Nq * 256 * e->elt();
+    if (e->hist.bytes != n && e->hist.alloc(n)) return 2;
+    if (!e->hist_done) OCC_CUDA(cudaEventCreateWithFlags(&e->hist_done, cudaEventDisableTiming));
+    return 0;
+}
+
+int occb200_engine_forward_video(occb200_engine* e, const float* const* feats, const int32_t* rot_map_dev, int scene_start,
+                                 float* bev_embed, float* occ_logits, float* flow, uint8_t* occ_cls_u8, int64_t* occ_cls_i64,
+                                 void* stream)
+{
+    OCC_CHECK(feats, "null pointer");
+    OCC_CHECK(e, "null engine");
+    OCC_CHECK(e->hist.p != nullptr, "history not enabled: call occb200_engine_set_history(e, 1) first");
+    if (check_frame(e, feats)) return 1;
+    return run_video_frame(e, feats, rot_map_dev, scene_start, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64,
+                           (cudaStream_t)stream);
 }
 
 int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_host, int64_t* occ_cls_i64_host,
@@ -999,8 +1101,9 @@ int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_hos
     return 0;
 }
 
-int occb200_engine_submit_host(occb200_engine* e, int slot, const float* const* feats_host, int64_t* occ_cls_i64_host,
-                               float* flow_host, void* stream)
+// _submit_host and _submit_host_video: `video` selects the history path, with the frame's host rotation map (or NULL)
+static int submit_frame(occb200_engine* e, int slot, const float* const* feats_host, int64_t* occ_cls_i64_host, float* flow_host,
+                        void* stream, bool video, const int32_t* rot_map_host, int scene_start)
 {
     OCC_CHECK(e && feats_host && occ_cls_i64_host && flow_host, "null pointer");
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
@@ -1010,6 +1113,13 @@ int occb200_engine_submit_host(occb200_engine* e, int slot, const float* const* 
     cudaStream_t st = (cudaStream_t)stream;
     occb200_engine::Slot& s = e->slots[slot];
     OCC_CHECK(!s.busy, "slot still in flight: call occb200_engine_wait_host first");
+    if (video) {                                                    // every rejection before the first CUDA call
+        OCC_CHECK(e->hist.p != nullptr, "history not enabled: call occb200_engine_set_history(e, 1) first");
+        if (check_frame(e, feats_host)) return 1;
+        if (rot_map_host)
+            for (int q = 0; q < e->Nq; ++q)
+                OCC_CHECK(rot_map_host[q] >= -1 && rot_map_host[q] < e->Nq, "rotation map entry out of range");
+    }
     if (!e->d2h_stream) {
         for (cudaStream_t& hs : e->h2d_stream) OCC_CUDA(cudaStreamCreateWithFlags(&hs, cudaStreamNonBlocking));
         OCC_CUDA(cudaStreamCreateWithFlags(&e->d2h_stream, cudaStreamNonBlocking));
@@ -1018,6 +1128,15 @@ int occb200_engine_submit_host(occb200_engine* e, int slot, const float* const* 
         for (cudaEvent_t& ev : s.h2d_done) OCC_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
         OCC_CUDA(cudaEventCreateWithFlags(&s.compute_done, cudaEventDisableTiming));
         OCC_CUDA(cudaEventCreateWithFlags(&s.d2h_done, cudaEventDisableTiming));
+    }
+    if (rot_map_host) {
+        // staged in the slot's pinned buffer so that the caller may reuse its array on return; h2d_done[0] covers the upload
+        const size_t mb = (size_t)e->Nq * 4;
+        if (!s.rot_pinned) OCC_CUDA(cudaMallocHost(&s.rot_pinned, mb));
+        if (s.rot.bytes != mb && s.rot.alloc(mb)) return 2;
+        OCC_CUDA(cudaEventSynchronize(s.h2d_done[0]));             // the slot's previous upload has left the staging buffer
+        memcpy(s.rot_pinned, rot_map_host, mb);
+        OCC_CUDA(cudaMemcpyAsync(s.rot.p, s.rot_pinned, mb, cudaMemcpyHostToDevice, e->h2d_stream[0]));
     }
     // Levels larger than 32 MB go up in `nsplit` pieces on separate copy streams: one cudaMemcpyAsync stream reached
     // 46 GB/s of the PCIe link on the test box, two reach 50 GB/s (OCC_H2D_SPLIT = 1..4, default 2).
@@ -1047,8 +1166,10 @@ int occb200_engine_submit_host(occb200_engine* e, int slot, const float* const* 
     }
     if (s.occ.bytes != nvox * 8 && s.occ.alloc(nvox * 8)) return 2;
     if (s.flow.bytes != nvox * 8 && s.flow.alloc(nvox * 8)) return 2;
-    int rc = occb200_engine_forward(e, dev_feats, nullptr, nullptr, nullptr, s.flow.as<float>(), nullptr,
-                                    s.occ.as<int64_t>(), stream);
+    int rc = video ? run_video_frame(e, dev_feats, rot_map_host ? s.rot.as<int32_t>() : nullptr, scene_start, nullptr, nullptr,
+                                     s.flow.as<float>(), nullptr, s.occ.as<int64_t>(), st)
+                   : occb200_engine_forward(e, dev_feats, nullptr, nullptr, nullptr, s.flow.as<float>(), nullptr,
+                                            s.occ.as<int64_t>(), stream);
     if (rc) return rc;
     OCC_CUDA(cudaEventRecord(s.compute_done, st));
     OCC_CUDA(cudaStreamWaitEvent(e->d2h_stream, s.compute_done, 0));
@@ -1057,6 +1178,21 @@ int occb200_engine_submit_host(occb200_engine* e, int slot, const float* const* 
     OCC_CUDA(cudaEventRecord(s.d2h_done, e->d2h_stream));
     s.busy = true;
     return 0;
+}
+
+int occb200_engine_submit_host(occb200_engine* e, int slot, const float* const* feats_host, int64_t* occ_cls_i64_host,
+                               float* flow_host, void* stream)
+{
+    return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, false, nullptr, 0);
+}
+
+int occb200_engine_submit_host_video(occb200_engine* e, int slot, const float* const* feats_host, const int32_t* rot_map_host,
+                                     int scene_start, int64_t* occ_cls_i64_host, float* flow_host, void* stream)
+{
+    OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
+    OCC_CHECK(feats_host && occ_cls_i64_host && flow_host, "null pointer");
+    OCC_CHECK(e, "null engine");
+    return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, true, rot_map_host, scene_start);
 }
 
 int occb200_engine_wait_host(occb200_engine* e, int slot)

@@ -81,6 +81,10 @@ int launch_cast(const float* src, T* dst, int64_t n, cudaStream_t stream);
 // dst[r] = map[r] >= 0 ? src[map[r]] : 0  (rows of C floats; map == nullptr: identity) -- prev_bev rotation + operand cast
 template <typename T>
 int launch_gather_rows(const float* src, const int32_t* map, int rows, int C, T* dst, float* dst_f32, cudaStream_t stream);
+// dst[r] = 0 <= map[r] < rows ? src[map[r]] : 0  (rows of C elements already in the storage type T; other entries read as
+// -1, so an unchecked device map cannot read out of bounds) -- the rotation of the engine-owned BEV history
+template <typename T>
+int launch_gather_rows_stored(const T* src, const int32_t* map, int rows, int C, T* dst, cudaStream_t stream);
 
 // ---- decoder_simt.cu
 // bev [Nq = H*W, C = mid*Z] f32 -> vox [X=W][Y=H][Z][mid] T with vox[x][y][z][cm] = bev[y*W+x][cm*Z+z]

@@ -6,6 +6,7 @@ their reference state_dict keys, camera geometry comes from `img_metas` exactly 
 `BEVFormerEncoder.point_sampling` reads it (encoder.py:94-101, 133-134).
 """
 import ctypes
+import numbers
 
 import numpy as np
 import torch
@@ -151,15 +152,10 @@ class OccEngine:
             arr[i] = f.data_ptr()
         return arr
 
-    def forward(self, feats, prev_bev=None, want=('bev_embed', 'occ', 'flow', 'occ_cls')):
-        """feats: 4 CUDA fp32 tensors (num_cams, C, h, w) of one frame, or with `set_input_dtype(torch.uint8)` one CUDA
-        uint8 tensor of camera frames (num_cams, src_h, src_w, 3).  Returns a dict of CUDA tensors."""
+    def _outputs(self, want):
         C = self.cfg['embed_dims']
         X, Y, Z = self.vox_shape
         dev = self.device
-        if not self.feat_channels_last and self.feat_dtype != torch.uint8:
-            feats = [f.contiguous() for f in feats]
-        self._check_feats(feats, cuda=True)
         out = {}
         if 'bev_embed' in want:
             out['bev_embed'] = torch.empty((self.Nq, C), dtype=torch.float32, device=dev)
@@ -171,6 +167,17 @@ class OccEngine:
             out['occ_cls'] = torch.empty((X, Y, Z), dtype=torch.uint8, device=dev)
         if 'occ_cls_i64' in want:
             out['occ_cls_i64'] = torch.empty((X, Y, Z), dtype=torch.int64, device=dev)
+        return out
+
+    def forward(self, feats, prev_bev=None, want=('bev_embed', 'occ', 'flow', 'occ_cls')):
+        """feats: 4 CUDA fp32 tensors (num_cams, C, h, w) of one frame, or with `set_input_dtype(torch.uint8)` one CUDA
+        uint8 tensor of camera frames (num_cams, src_h, src_w, 3).  Returns a dict of CUDA tensors."""
+        C = self.cfg['embed_dims']
+        dev = self.device
+        if not self.feat_channels_last and self.feat_dtype != torch.uint8:
+            feats = [f.contiguous() for f in feats]
+        self._check_feats(feats, cuda=True)
+        out = self._outputs(want)
         if prev_bev is not None:
             prev_bev = prev_bev.to(device=dev, dtype=torch.float32).reshape(self.Nq, C).contiguous()
         with torch.cuda.device(dev):
@@ -211,23 +218,96 @@ class OccEngine:
     def stream_host(self, frames_host):
         """Generator over an iterable of host frames with two frames in flight; yields (occ int64 CPU, flow CPU)
         views of the slot's pinned output buffers (valid until the slot is reused two frames later)."""
+        return self._stream(frames_host, lambda slot, fr, outs: self.submit_host(slot, fr, *outs))
+
+    def _stream(self, items, submit):
         X, Y, Z = self.vox_shape
         if getattr(self, '_stream_outs', None) is None:              # pinned once: cudaHostAlloc costs milliseconds
             self._stream_outs = [(torch.empty((X, Y, Z), dtype=torch.int64).pin_memory(),
                                   torch.empty((X, Y, Z, 2)).pin_memory()) for _ in range(2)]
         outs = self._stream_outs
         pending = []
-        for i, fr in enumerate(frames_host):
+        for i, item in enumerate(items):
             slot = i & 1
             if len(pending) == 2:
                 s = pending.pop(0)
                 self.wait_host(s)
                 yield outs[s]
-            self.submit_host(slot, fr, *outs[slot])
+            submit(slot, item, outs[slot])
             pending.append(slot)
         for s in pending:
             self.wait_host(s)
             yield outs[s]
+
+    # ---------------------------------------------------------------------------------------- video (temporal) inference
+    def set_history(self, enabled=True):
+        """Keep the BEV history inside the engine for `forward_video` / `submit_host_video`: one (Nq, 256) buffer in the
+        storage precision, allocated (True) or freed (False).  Either way the next video frame starts a new scene."""
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.occb200_engine_set_history(self._h, int(enabled)))
+
+    def _rotation_host(self, rotation):
+        """None, an angle in degrees (can_bus[-1]; the map of `rotation_index_map` about the config's rotate_center) or an
+        index map (Nq,) -> int32 numpy (Nq,) or None.  `submit_host_video` hands the map to the engine, which rejects
+        entries outside [-1, Nq)."""
+        if rotation is None:
+            return None
+        if isinstance(rotation, numbers.Real):
+            return rotation_index_map(self.cfg['bev_h'], self.cfg['bev_w'], float(rotation),
+                                      self.cfg.get('rotate_center', [100, 100]))
+        m = np.ascontiguousarray(rotation.cpu().numpy() if isinstance(rotation, torch.Tensor) else rotation, np.int32)
+        if m.shape != (self.Nq,):
+            raise ValueError(f'rotation map: shape {m.shape} != ({self.Nq},)')
+        return m
+
+    def _rotation_dev(self, rotation):
+        """the same as a CUDA int32 tensor on the current stream.  A CUDA map is used as given (the engine reads entries
+        outside [-1, Nq) as -1); a host map or an angle is range-checked here and uploaded for this frame only: the upload
+        and the frame are ordered on the current stream, so the temporary can be freed when the call returns."""
+        if isinstance(rotation, torch.Tensor) and rotation.is_cuda:
+            if rotation.dtype != torch.int32 or tuple(rotation.shape) != (self.Nq,) or not rotation.is_contiguous() \
+                    or rotation.device != self.device:
+                raise ValueError(f'rotation map: need a contiguous int32 ({self.Nq},) tensor on {self.device}')
+            return rotation
+        m = self._rotation_host(rotation)
+        if m is None:
+            return None
+        if m.min() < -1 or m.max() >= self.Nq:
+            raise ValueError(f'rotation map entry out of range: must be in [-1, {self.Nq})')
+        return torch.from_numpy(m).pin_memory().to(self.device, non_blocking=True)
+
+    def forward_video(self, feats, rotation=None, scene_start=False, want=('bev_embed', 'occ', 'flow', 'occ_cls')):
+        """One frame of a video (needs `set_history()`): `feats` as for `forward`; the previous BEV is the engine's history,
+        rotated by `rotation` (None, an angle in degrees or an index map), unless `scene_start` or this is the first frame
+        since `set_history()` (self mode).  Equals `forward(feats, prev_bev=<previous frame's bev_embed>)` with the same
+        rotation, bit for bit; the frame's BEV stays in the history whether or not 'bev_embed' is in `want`."""
+        if not self.feat_channels_last and self.feat_dtype != torch.uint8:
+            feats = [f.contiguous() for f in feats]
+        self._check_feats(feats, cuda=True)
+        rot = self._rotation_dev(rotation)
+        out = self._outputs(want)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.occb200_engine_forward_video(
+                self._h, self._feat_ptrs(feats), _lib.ptr(rot), int(bool(scene_start)), _lib.ptr(out.get('bev_embed')),
+                _lib.ptr(out.get('occ')), _lib.ptr(out.get('flow')), _lib.ptr(out.get('occ_cls')),
+                _lib.ptr(out.get('occ_cls_i64')), _lib.stream_ptr()))
+        return out
+
+    def submit_host_video(self, slot, feats_host, occ_out, flow_out, rotation=None, scene_start=False):
+        """Pipelined host-buffer video frame (slot 0/1; `submit_host` + the history of `forward_video`): returns
+        immediately, `wait_host(slot)` completes it.  The rotation map is copied before the call returns."""
+        self._check_feats(feats_host, cuda=False)
+        rot = self._rotation_host(rotation)
+        arr = self._feat_ptrs(feats_host)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.occb200_engine_submit_host_video(self._h, slot, arr, _lib.ptr(rot), int(bool(scene_start)),
+                                                                 _lib.ptr(occ_out), _lib.ptr(flow_out), _lib.stream_ptr()))
+
+    def stream_host_video(self, items):
+        """`stream_host` for video: items are (feats_host, rotation, scene_start); two frames in flight, yields
+        (occ int64 CPU, flow CPU) views of the slot's pinned output buffers, frame by frame."""
+        return self._stream(items, lambda slot, it, outs: self.submit_host_video(slot, it[0], *outs, rotation=it[1],
+                                                                                  scene_start=it[2]))
 
     def enable_taps(self, on=True):
         _lib.check(self.lib.occb200_engine_enable_taps(self._h, int(on)))
