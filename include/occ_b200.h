@@ -106,6 +106,20 @@ int occb200_engine_set_cameras(occb200_engine* e, const float* cam_mat, const fl
  * stream may read the new map, so change it only when no frame is in flight.  The video calls below ignore it (they take a
  * map per frame). */
 int occb200_engine_set_prev_rotation(occb200_engine* e, const int32_t* map_host);
+/* The same rotation given by its angle: can_bus[-1] degrees about the config's rotate_center.  No map is built, copied or
+ * uploaded: the gather computes every cell's source cell on the device (occb200_rotation_coeffs, then torchvision's grid and
+ * nearest rounding, bit-identical to the map torchvision's rotate makes of an index image).  The coefficients travel as kernel
+ * arguments of each frame, so there is no in-flight hazard.  Host only, no CUDA call.  Between this call and
+ * occb200_engine_set_prev_rotation(map or NULL) the last call wins.  A non-finite angle returns 1. */
+int occb200_engine_set_prev_rotation_angle(occb200_engine* e, double angle_deg);
+/* The six fp32 grid coefficients of torchvision's rotate(img, angle_deg, center=[cx, cy]) on a bev_h x bev_w image, computed
+ * as torchvision computes them: _get_inverse_affine_matrix(center - size/2, -angle) in double (cos / sin of angle * pi/180),
+ * cast to fp32, divided in fp32 by [bev_w / 2, bev_h / 2].  out[0..2]: g_x = out[0] x + out[1] y + out[2]; out[3..5]: g_y
+ * alike, over the base grid x = j - bev_w/2 + 0.5, y = i - bev_h/2 + 0.5.  Host only, no CUDA call. */
+int occb200_rotation_coeffs(double angle_deg, int bev_h, int bev_w, int cx, int cy, float out[6]);
+/* Debug / test entry: map_dev (dev int32 [Nq]) = the source cell of every BEV cell (-1 = outside) that the rotation gathers
+ * compute for angle_deg, written by one kernel on `stream`. */
+int occb200_engine_rotation_map(occb200_engine* e, double angle_deg, int32_t* map_dev, void* stream);
 
 /* Element type / layout of the feature levels handed to _forward / _forward_host / _submit_host from now on (pointers
  * travel through the same arguments): 0 = fp32 [num_cams, C, h, w] (default, the reference's), 1 = bf16, same layout
@@ -182,6 +196,15 @@ int occb200_engine_forward_video(occb200_engine* e, const float* const* feats, c
                                  void* stream);
 int occb200_engine_submit_host_video(occb200_engine* e, int slot, const float* const* feats_host, const int32_t* rot_map_host,
                                      int scene_start, int64_t* occ_cls_i64_host, float* flow_host, void* stream);
+/* The same two calls with the frame's rotation as an angle (can_bus[-1] degrees about the config's rotate_center) instead of a
+ * map: the history gather computes the source cells on the device (see occb200_engine_set_prev_rotation_angle), so there is
+ * no map to build, stage or upload and the frame launches the same kernels.  Bit-identical to the map calls with the map
+ * torchvision's rotate gives for that angle.  A non-finite angle returns 1 before any CUDA call, like the other rejections. */
+int occb200_engine_forward_video_angle(occb200_engine* e, const float* const* feats, double angle_deg, int scene_start,
+                                       float* bev_embed, float* occ_logits, float* flow, uint8_t* occ_cls_u8,
+                                       int64_t* occ_cls_i64, void* stream);
+int occb200_engine_submit_host_video_angle(occb200_engine* e, int slot, const float* const* feats_host, double angle_deg,
+                                           int scene_start, int64_t* occ_cls_i64_host, float* flow_host, void* stream);
 
 /* Intermediate taps for parity tests (dev f32, valid after a forward; NULL if not produced):
  *   which: 0 = layer output [Nq,C] of layer `layer`; 1 = TSA output (pre-norm, with residual); 2 = SCA output

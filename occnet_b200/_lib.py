@@ -10,6 +10,7 @@ c_f32p = ctypes.c_void_p
 _vp = ctypes.c_void_p
 _i = ctypes.c_int
 _i64 = ctypes.c_int64
+_f64 = ctypes.c_double
 
 
 class OccConfig(ctypes.Structure):
@@ -35,6 +36,9 @@ SIGNATURES = {
     'occb200_engine_set_input_dtype': (_i, [_vp, _i]),
     'occb200_engine_attach_backbone': (_i, [_vp, _vp]),
     'occb200_engine_set_prev_rotation': (_i, [_vp, _vp]),
+    'occb200_engine_set_prev_rotation_angle': (_i, [_vp, _f64]),
+    'occb200_rotation_coeffs': (_i, [_f64, _i, _i, _i, _i, _vp]),
+    'occb200_engine_rotation_map': (_i, [_vp, _f64, _vp, _vp]),
     'occb200_engine_forward': (_i, [_vp, ctypes.POINTER(_vp), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'occb200_engine_forward_host': (_i, [_vp, ctypes.POINTER(_vp), _vp, _vp, _vp]),
     'occb200_engine_submit_host': (_i, [_vp, _i, ctypes.POINTER(_vp), _vp, _vp, _vp]),
@@ -42,6 +46,8 @@ SIGNATURES = {
     'occb200_engine_set_history': (_i, [_vp, _i]),
     'occb200_engine_forward_video': (_i, [_vp, ctypes.POINTER(_vp), _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     'occb200_engine_submit_host_video': (_i, [_vp, _i, ctypes.POINTER(_vp), _vp, _i, _vp, _vp, _vp]),
+    'occb200_engine_forward_video_angle': (_i, [_vp, ctypes.POINTER(_vp), _f64, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'occb200_engine_submit_host_video_angle': (_i, [_vp, _i, ctypes.POINTER(_vp), _f64, _i, _vp, _vp, _vp]),
     'occb200_engine_enable_taps': (_i, [_vp, _i]),
     'occb200_engine_copy_tap': (_i, [_vp, _i, _i, _vp, _vp]),
     'occb200_engine_project_pillars': (_i, [_vp, _vp, _vp, _vp]),

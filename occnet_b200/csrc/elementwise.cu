@@ -345,63 +345,112 @@ int launch_split_bf16(const float* a, int Ka, const float* b, int Kb, int64_t ro
 }  // namespace occ
 
 // ---- prev_bev rotation as a row gather (transformer_occ.py:195-205: torchvision `rotate`, nearest, zero fill): the host
-//      hands over the index map source_row[q] (-1 = outside), this kernel applies it while producing the GEMM operand copy
+//      hands over the index map source_row[q] (-1 = outside), or the rotation's six grid coefficients from which every
+//      thread computes its source row; this kernel applies it while producing the GEMM operand copy
 namespace occ {
 namespace {
-template <typename T>
-__global__ void gather_rows_kernel(const float* __restrict__ src, const int32_t* __restrict__ map, int rows, int C,
-                                   T* __restrict__ dst, float* __restrict__ dst_f32)
+// Source cell of BEV cell q under the rotation `g`, or -1 outside: torchvision's rotate(center=...) with nearest
+// interpolation, operation for operation (_gen_affine_grid + grid_sample(align_corners=False, padding_mode='zeros')):
+//   base grid  x = j - W/2 + 0.5, y = i - H/2 + 0.5                  (half-integers: exact in fp32)
+//   grid       g = (x * r0 + y * r1) + r2 with the y term fused       (the rounding torch's CPU bmm produces)
+//   unnormalise ix = ((g_x + 1) * W - 1) / 2, iy alike with H
+//   nearest    rint (half to even), cells outside the image read the zero fill.
+// Every step is an explicitly rounded intrinsic, so -fmad cannot contract a different rounding into it.
+__device__ __forceinline__ int rotation_source(int q, const RotGrid& g)
+{
+    const int i = q / g.bev_w, j = q - i * g.bev_w;
+    const float x = 0.5f * (float)(2 * j - g.bev_w + 1), y = 0.5f * (float)(2 * i - g.bev_h + 1);
+    const float gx = __fadd_rn(__fmaf_rn(y, g.r[1], __fmul_rn(x, g.r[0])), g.r[2]);
+    const float gy = __fadd_rn(__fmaf_rn(y, g.r[4], __fmul_rn(x, g.r[3])), g.r[5]);
+    const float ix = rintf(__fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), (float)g.bev_w), 1.f), 2.f));
+    const float iy = rintf(__fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), (float)g.bev_h), 1.f), 2.f));
+    if (!(ix >= 0.f && ix < (float)g.bev_w && iy >= 0.f && iy < (float)g.bev_h)) return -1;
+    return (int)iy * g.bev_w + (int)ix;
+}
+
+// kGrid: source rows from rotation_source(grid); otherwise from `map` (host-checked, NULL = identity)
+template <typename T, bool kGrid>
+__global__ void gather_rows_kernel(const float* __restrict__ src, const int32_t* __restrict__ map, RotGrid grid, int rows,
+                                   int C, T* __restrict__ dst, float* __restrict__ dst_f32)
 {
     const int per_row = C >> 3;
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (int64_t)rows * per_row) return;
     const int r = (int)(i / per_row), c = (int)(i % per_row) * 8;
-    const int sr = map ? map[r] : r;
+    const int sr = kGrid ? rotation_source(r, grid) : (map ? map[r] : r);
     float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (sr >= 0) load8(src + (int64_t)sr * C + c, v);
     if (dst) store8(dst + (int64_t)r * C + c, v);
     if (dst_f32) store8(dst_f32 + (int64_t)r * C + c, v);
 }
+
+__global__ void rotation_map_kernel(RotGrid grid, int rows, int32_t* __restrict__ map)
+{
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q < rows) map[q] = rotation_source(q, grid);
+}
 }  // namespace
 template <typename T>
-int launch_gather_rows(const float* src, const int32_t* map, int rows, int C, T* dst, float* dst_f32, cudaStream_t stream)
+int launch_gather_rows(const float* src, const int32_t* map, const RotGrid* grid, int rows, int C, T* dst, float* dst_f32,
+                       cudaStream_t stream)
 {
     OCC_CHECK(C % 8 == 0, "gather_rows: C must be a multiple of 8");
+    OCC_CHECK(grid == nullptr || grid->bev_h * grid->bev_w == rows, "gather_rows: rotation grid size != rows");
     const int64_t n = (int64_t)rows * (C >> 3);
-    gather_rows_kernel<T><<<ceil_div(n, 256), 256, 0, stream>>>(src, map, rows, C, dst, dst_f32);
+    if (grid)
+        gather_rows_kernel<T, true><<<ceil_div(n, 256), 256, 0, stream>>>(src, nullptr, *grid, rows, C, dst, dst_f32);
+    else
+        gather_rows_kernel<T, false><<<ceil_div(n, 256), 256, 0, stream>>>(src, map, RotGrid{}, rows, C, dst, dst_f32);
     OCC_CUDA(cudaGetLastError());
     return 0;
 }
-template int launch_gather_rows<float>(const float*, const int32_t*, int, int, float*, float*, cudaStream_t);
-template int launch_gather_rows<bf16>(const float*, const int32_t*, int, int, bf16*, float*, cudaStream_t);
+template int launch_gather_rows<float>(const float*, const int32_t*, const RotGrid*, int, int, float*, float*, cudaStream_t);
+template int launch_gather_rows<bf16>(const float*, const int32_t*, const RotGrid*, int, int, bf16*, float*, cudaStream_t);
+
+int launch_rotation_map(const RotGrid& grid, int32_t* map, cudaStream_t stream)
+{
+    const int rows = grid.bev_h * grid.bev_w;
+    if (rows == 0) return 0;
+    rotation_map_kernel<<<ceil_div(rows, 256), 256, 0, stream>>>(grid, rows, map);
+    OCC_CUDA(cudaGetLastError());
+    return 0;
+}
 
 // ---- the same rotation from the engine-owned BEV history, already in the storage type: a pure row permutation (16 bytes
 //      per thread, no conversion).  The map may come straight from the caller's device memory, so an entry outside
 //      [-1, rows) reads as -1 (zeros) instead of out of bounds.
 namespace {
-__global__ void gather_rows16_kernel(const uint4* __restrict__ src, const int32_t* __restrict__ map, int rows, int per_row,
-                                     uint4* __restrict__ dst)
+// kGrid: source rows from rotation_source(grid) instead of the map
+template <bool kGrid>
+__global__ void gather_rows16_kernel(const uint4* __restrict__ src, const int32_t* __restrict__ map, RotGrid grid, int rows,
+                                     int per_row, uint4* __restrict__ dst)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (int64_t)rows * per_row) return;
     const int r = (int)(i / per_row), c = (int)(i % per_row);
-    const int sr = map ? __ldg(map + r) : r;
+    const int sr = kGrid ? rotation_source(r, grid) : (map ? __ldg(map + r) : r);
     dst[i] = (sr >= 0 && sr < rows) ? __ldg(src + (int64_t)sr * per_row + c) : make_uint4(0u, 0u, 0u, 0u);
 }
 }  // namespace
 template <typename T>
-int launch_gather_rows_stored(const T* src, const int32_t* map, int rows, int C, T* dst, cudaStream_t stream)
+int launch_gather_rows_stored(const T* src, const int32_t* map, const RotGrid* grid, int rows, int C, T* dst,
+                              cudaStream_t stream)
 {
     OCC_CHECK((C * sizeof(T)) % 16 == 0, "gather_rows_stored: rows must be a multiple of 16 bytes");
+    OCC_CHECK(grid == nullptr || grid->bev_h * grid->bev_w == rows, "gather_rows_stored: rotation grid size != rows");
     const int per_row = (int)(C * sizeof(T) / 16);
     const int64_t n = (int64_t)rows * per_row;
-    gather_rows16_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(src), map, rows, per_row,
-                                                                reinterpret_cast<uint4*>(dst));
+    const uint4* s = reinterpret_cast<const uint4*>(src);
+    uint4* d = reinterpret_cast<uint4*>(dst);
+    if (grid)
+        gather_rows16_kernel<true><<<ceil_div(n, 256), 256, 0, stream>>>(s, nullptr, *grid, rows, per_row, d);
+    else
+        gather_rows16_kernel<false><<<ceil_div(n, 256), 256, 0, stream>>>(s, map, RotGrid{}, rows, per_row, d);
     OCC_CUDA(cudaGetLastError());
     return 0;
 }
-template int launch_gather_rows_stored<float>(const float*, const int32_t*, int, int, float*, cudaStream_t);
-template int launch_gather_rows_stored<bf16>(const bf16*, const int32_t*, int, int, bf16*, cudaStream_t);
+template int launch_gather_rows_stored<float>(const float*, const int32_t*, const RotGrid*, int, int, float*, cudaStream_t);
+template int launch_gather_rows_stored<bf16>(const bf16*, const int32_t*, const RotGrid*, int, int, bf16*, cudaStream_t);
 }  // namespace occ
 
 // ---- feature packing from channels-last bf16 levels [num_cams, h, w, C] (what occb200_backbone_forward_nhwc_bf16 writes):

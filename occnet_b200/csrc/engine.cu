@@ -67,6 +67,8 @@ struct occb200_engine {
     bool cameras_set = false, finalized = false, taps = false;
     DevBuf rot_map;                     // occb200_engine_set_prev_rotation: source row of every BEV cell (int32, -1 = outside)
     bool rot_set = false;
+    RotGrid rot_grid;                   // occb200_engine_set_prev_rotation_angle: the same rotation as grid coefficients
+    bool rot_grid_set = false;          // (at most one of rot_set / rot_grid_set: the last call wins)
     // occb200_engine_set_history: the last video frame's final BEV [Nq, 256] in the storage type (the bf16 / fp32 copy the last
     // LayerNorm writes), read and written only by the video calls; hist_done is recorded after every video frame
     DevBuf hist;
@@ -260,12 +262,45 @@ int build_tsa_query_values(occb200_engine* e)
 
 enum { MODE_FRAME = 0, MODE_L0_TSA_ONLY = 1 };
 
-// A video frame (occb200_engine_forward_video / _submit_host_video): with `prev`, the previous BEV is the engine history
-// gathered through `map` (NULL = no rotation) instead of a caller's fp32 prev_bev; either way the frame's last LayerNorm
-// writes its storage-type copy of the final BEV into the history.
+// torchvision's rotate(img, angle_deg, center=[cx, cy]) of a bev_h x bev_w image as the six grid coefficients its
+// _gen_affine_grid multiplies the base grid with, computed as torchvision computes them: _get_inverse_affine_matrix(center -
+// size / 2, -angle) in double (zero translation and shear, scale 1: [cos, sin, t0; -sin, cos, t1] about the centre), cast to
+// fp32, then divided in fp32 by [W / 2, H / 2].  out = {row x: r0 r1 r2, row y: r3 r4 r5}.  Host only.
+void rotation_coeffs(double angle_deg, int bev_h, int bev_w, int cx, int cy, float out[6])
+{
+    constexpr double kDegToRad = 3.141592653589793 / 180.0;          // math.radians
+    const double rot = -angle_deg * kDegToRad;
+    const double c = std::cos(rot), s = std::sin(rot);
+    const double ccx = (double)cx - (double)bev_w * 0.5, ccy = (double)cy - (double)bev_h * 0.5;
+    double m[6] = {c, s, 0.0, -s, c, 0.0};
+    m[2] += m[0] * -ccx + m[1] * -ccy;                                  // inverse rotation of the centred grid ...
+    m[5] += m[3] * -ccx + m[4] * -ccy;
+    m[2] += ccx;                                                        // ... moved back to the centre
+    m[5] += ccy;
+    const float sx = (float)(0.5 * bev_w), sy = (float)(0.5 * bev_h);
+    for (int k = 0; k < 3; ++k) {
+        out[k] = (float)m[k] / sx;
+        out[3 + k] = (float)m[3 + k] / sy;
+    }
+}
+
+RotGrid rotation_grid(const occb200_engine* e, double angle_deg)
+{
+    RotGrid g;
+    rotation_coeffs(angle_deg, e->cfg.bev_h, e->cfg.bev_w, e->cfg.rotate_center[0], e->cfg.rotate_center[1], g.r);
+    g.bev_h = e->cfg.bev_h;
+    g.bev_w = e->cfg.bev_w;
+    return g;
+}
+
+// A video frame (occb200_engine_forward_video / _submit_host_video and their _angle forms): with `prev`, the previous BEV is
+// the engine history gathered through `map` (NULL = no rotation), or through the source cells computed from `grid` when it is
+// set, instead of a caller's fp32 prev_bev; either way the frame's last LayerNorm writes its storage-type copy of the final
+// BEV into the history.
 struct VideoArgs {
     bool prev = false;
     const int32_t* map = nullptr;
+    const RotGrid* grid = nullptr;
 };
 
 template <typename T>
@@ -329,12 +364,13 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
         // encoder.py:204-209: value = stack([prev_bev, bev_query]) built ONCE before the layer loop, so
         // queue 1 keeps seeing the layer-0 query in every layer.
         // (transformer_occ.py:195-205) the rotation of prev_bev about rotate_center is a nearest-neighbour row permutation:
-        // applied here, fused with the operand cast, from the index map set by occb200_engine_set_prev_rotation.  The
+        // applied here, fused with the operand cast, from the index map set by occb200_engine_set_prev_rotation (or the
+        // source cells each thread computes from the angle of occb200_engine_set_prev_rotation_angle / the _angle calls).  The
         // history already holds the operand rounding of the previous bev_embed, so gathering it gives the same operand.
         if (from_hist) {
-            if (launch_gather_rows_stored<T>(e->hist.as<T>(), video->map, Nq, C, e->prev_t.as<T>(), st)) return 2;
-        } else if (launch_gather_rows<T>(prev_bev, e->rot_set ? e->rot_map.as<int32_t>() : nullptr, Nq, C, e->prev_t.as<T>(),
-                                         nullptr, st))
+            if (launch_gather_rows_stored<T>(e->hist.as<T>(), video->map, video->grid, Nq, C, e->prev_t.as<T>(), st)) return 2;
+        } else if (launch_gather_rows<T>(prev_bev, e->rot_set ? e->rot_map.as<int32_t>() : nullptr,
+                                         e->rot_grid_set ? &e->rot_grid : nullptr, Nq, C, e->prev_t.as<T>(), nullptr, st))
             return 2;
         e->launches++;
     }
@@ -645,12 +681,13 @@ int run_frame(occb200_engine* e, const float* const* feats, const float* prev_be
 
 // One video frame on device buffers, after every host-side check has passed.  The frame waits for the previous video
 // frame (on whatever stream that ran) before it reads the history, and records hist_done after it has written it.
-int run_video_frame(occb200_engine* e, const float* const* feats, const int32_t* map_dev, int scene_start, float* bev_embed,
-                    float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st)
+int run_video_frame(occb200_engine* e, const float* const* feats, const int32_t* map_dev, const RotGrid* grid, int scene_start,
+                    float* bev_embed, float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st)
 {
     VideoArgs v;
     v.prev = scene_start == 0 && e->hist_valid;
     v.map = map_dev;
+    v.grid = grid;
     if (e->hist_recorded) OCC_CUDA(cudaStreamWaitEvent(st, e->hist_done, 0));
     const int rc = run_frame(e, feats, nullptr, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, &v);
     if (rc) return rc;
@@ -1069,7 +1106,21 @@ int occb200_engine_forward_video(occb200_engine* e, const float* const* feats, c
     OCC_CHECK(e, "null engine");
     OCC_CHECK(e->hist.p != nullptr, "history not enabled: call occb200_engine_set_history(e, 1) first");
     if (check_frame(e, feats)) return 1;
-    return run_video_frame(e, feats, rot_map_dev, scene_start, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64,
+    return run_video_frame(e, feats, rot_map_dev, nullptr, scene_start, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64,
+                           (cudaStream_t)stream);
+}
+
+int occb200_engine_forward_video_angle(occb200_engine* e, const float* const* feats, double angle_deg, int scene_start,
+                                       float* bev_embed, float* occ_logits, float* flow, uint8_t* occ_cls_u8,
+                                       int64_t* occ_cls_i64, void* stream)
+{
+    OCC_CHECK(std::isfinite(angle_deg), "rotation angle must be finite");
+    OCC_CHECK(feats, "null pointer");
+    OCC_CHECK(e, "null engine");
+    OCC_CHECK(e->hist.p != nullptr, "history not enabled: call occb200_engine_set_history(e, 1) first");
+    if (check_frame(e, feats)) return 1;
+    const RotGrid g = rotation_grid(e, angle_deg);
+    return run_video_frame(e, feats, nullptr, &g, scene_start, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64,
                            (cudaStream_t)stream);
 }
 
@@ -1101,9 +1152,10 @@ int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_hos
     return 0;
 }
 
-// _submit_host and _submit_host_video: `video` selects the history path, with the frame's host rotation map (or NULL)
+// _submit_host and _submit_host_video(_angle): `video` selects the history path, with the frame's host rotation map (or
+// NULL), or its rotation as grid coefficients (`grid`: nothing to stage or upload)
 static int submit_frame(occb200_engine* e, int slot, const float* const* feats_host, int64_t* occ_cls_i64_host, float* flow_host,
-                        void* stream, bool video, const int32_t* rot_map_host, int scene_start)
+                        void* stream, bool video, const int32_t* rot_map_host, const RotGrid* grid, int scene_start)
 {
     OCC_CHECK(e && feats_host && occ_cls_i64_host && flow_host, "null pointer");
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
@@ -1166,8 +1218,8 @@ static int submit_frame(occb200_engine* e, int slot, const float* const* feats_h
     }
     if (s.occ.bytes != nvox * 8 && s.occ.alloc(nvox * 8)) return 2;
     if (s.flow.bytes != nvox * 8 && s.flow.alloc(nvox * 8)) return 2;
-    int rc = video ? run_video_frame(e, dev_feats, rot_map_host ? s.rot.as<int32_t>() : nullptr, scene_start, nullptr, nullptr,
-                                     s.flow.as<float>(), nullptr, s.occ.as<int64_t>(), st)
+    int rc = video ? run_video_frame(e, dev_feats, rot_map_host ? s.rot.as<int32_t>() : nullptr, grid, scene_start, nullptr,
+                                     nullptr, s.flow.as<float>(), nullptr, s.occ.as<int64_t>(), st)
                    : occb200_engine_forward(e, dev_feats, nullptr, nullptr, nullptr, s.flow.as<float>(), nullptr,
                                             s.occ.as<int64_t>(), stream);
     if (rc) return rc;
@@ -1183,7 +1235,7 @@ static int submit_frame(occb200_engine* e, int slot, const float* const* feats_h
 int occb200_engine_submit_host(occb200_engine* e, int slot, const float* const* feats_host, int64_t* occ_cls_i64_host,
                                float* flow_host, void* stream)
 {
-    return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, false, nullptr, 0);
+    return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, false, nullptr, nullptr, 0);
 }
 
 int occb200_engine_submit_host_video(occb200_engine* e, int slot, const float* const* feats_host, const int32_t* rot_map_host,
@@ -1192,7 +1244,18 @@ int occb200_engine_submit_host_video(occb200_engine* e, int slot, const float* c
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
     OCC_CHECK(feats_host && occ_cls_i64_host && flow_host, "null pointer");
     OCC_CHECK(e, "null engine");
-    return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, true, rot_map_host, scene_start);
+    return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, true, rot_map_host, nullptr, scene_start);
+}
+
+int occb200_engine_submit_host_video_angle(occb200_engine* e, int slot, const float* const* feats_host, double angle_deg,
+                                           int scene_start, int64_t* occ_cls_i64_host, float* flow_host, void* stream)
+{
+    OCC_CHECK(std::isfinite(angle_deg), "rotation angle must be finite");
+    OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
+    OCC_CHECK(feats_host && occ_cls_i64_host && flow_host, "null pointer");
+    OCC_CHECK(e, "null engine");
+    const RotGrid g = rotation_grid(e, angle_deg);
+    return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, true, nullptr, &g, scene_start);
 }
 
 int occb200_engine_wait_host(occb200_engine* e, int slot)
@@ -1208,11 +1271,39 @@ int occb200_engine_wait_host(occb200_engine* e, int slot)
 int occb200_engine_set_prev_rotation(occb200_engine* e, const int32_t* map_host)
 {
     OCC_CHECK(e, "null engine");
-    if (map_host == nullptr) { e->rot_set = false; return 0; }
+    if (map_host == nullptr) { e->rot_set = false; e->rot_grid_set = false; return 0; }
     for (int q = 0; q < e->Nq; ++q) OCC_CHECK(map_host[q] >= -1 && map_host[q] < e->Nq, "rotation map entry out of range");
     if (e->rot_map.bytes != (size_t)e->Nq * 4 && e->rot_map.alloc((size_t)e->Nq * 4)) return 2;
     OCC_CUDA(cudaMemcpy(e->rot_map.p, map_host, (size_t)e->Nq * 4, cudaMemcpyHostToDevice));
     e->rot_set = true;
+    e->rot_grid_set = false;
+    return 0;
+}
+
+int occb200_engine_set_prev_rotation_angle(occb200_engine* e, double angle_deg)
+{
+    OCC_CHECK(std::isfinite(angle_deg), "rotation angle must be finite");
+    OCC_CHECK(e, "null engine");
+    e->rot_grid = rotation_grid(e, angle_deg);
+    e->rot_grid_set = true;
+    e->rot_set = false;
+    return 0;
+}
+
+int occb200_engine_rotation_map(occb200_engine* e, double angle_deg, int32_t* map_dev, void* stream)
+{
+    OCC_CHECK(std::isfinite(angle_deg), "rotation angle must be finite");
+    OCC_CHECK(map_dev, "null pointer");
+    OCC_CHECK(e, "null engine");
+    return launch_rotation_map(rotation_grid(e, angle_deg), map_dev, (cudaStream_t)stream);
+}
+
+int occb200_rotation_coeffs(double angle_deg, int bev_h, int bev_w, int cx, int cy, float out[6])
+{
+    OCC_CHECK(std::isfinite(angle_deg), "rotation angle must be finite");
+    OCC_CHECK(out, "null pointer");
+    OCC_CHECK(bev_h > 0 && bev_w > 0, "bev_h and bev_w must be positive");
+    rotation_coeffs(angle_deg, bev_h, bev_w, cx, cy, out);
     return 0;
 }
 

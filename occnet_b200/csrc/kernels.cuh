@@ -78,13 +78,24 @@ int launch_bev_pos(const float* row_embed, const float* col_embed, int bev_h, in
                    cudaStream_t stream);
 template <typename T>
 int launch_cast(const float* src, T* dst, int64_t n, cudaStream_t stream);
-// dst[r] = map[r] >= 0 ? src[map[r]] : 0  (rows of C floats; map == nullptr: identity) -- prev_bev rotation + operand cast
+// A prev_bev rotation by its grid coefficients (torchvision's theta / [W/2, H/2] in fp32, see rotation_coeffs in engine.cu):
+// g_x = r[0] x + r[1] y + r[2], g_y = r[3] x + r[4] y + r[5] over the base grid of a bev_h x bev_w image
+struct RotGrid {
+    float r[6];
+    int bev_h, bev_w;
+};
+// dst[r] = map[r] >= 0 ? src[map[r]] : 0  (rows of C floats; map == nullptr: identity) -- prev_bev rotation + operand cast.
+// grid != nullptr: the source rows are computed on the device from the rotation instead (map is ignored)
 template <typename T>
-int launch_gather_rows(const float* src, const int32_t* map, int rows, int C, T* dst, float* dst_f32, cudaStream_t stream);
+int launch_gather_rows(const float* src, const int32_t* map, const RotGrid* grid, int rows, int C, T* dst, float* dst_f32,
+                       cudaStream_t stream);
 // dst[r] = 0 <= map[r] < rows ? src[map[r]] : 0  (rows of C elements already in the storage type T; other entries read as
-// -1, so an unchecked device map cannot read out of bounds) -- the rotation of the engine-owned BEV history
+// -1, so an unchecked device map cannot read out of bounds) -- the rotation of the engine-owned BEV history; grid as above
 template <typename T>
-int launch_gather_rows_stored(const T* src, const int32_t* map, int rows, int C, T* dst, cudaStream_t stream);
+int launch_gather_rows_stored(const T* src, const int32_t* map, const RotGrid* grid, int rows, int C, T* dst,
+                              cudaStream_t stream);
+// map[q] = source cell of BEV cell q under `grid` (-1 = outside): the index map both gathers compute, for tests
+int launch_rotation_map(const RotGrid& grid, int32_t* map, cudaStream_t stream);
 
 // ---- decoder_simt.cu
 // bev [Nq = H*W, C = mid*Z] f32 -> vox [X=W][Y=H][Z][mid] T with vox[x][y][z][cm] = bev[y*W+x][cm*Z+z]

@@ -90,6 +90,7 @@ class OccEngine:
         self._pinned = None
         self.feat_dtype, self.feat_channels_last = torch.float32, False
         self.backbone = None
+        self.history = False                                          # set_history(True) has allocated the BEV history
 
     def set_input_dtype(self, dtype, channels_last=False):
         """Feature levels are handed over as `dtype` from now on (torch.float32, the reference's, or torch.bfloat16);
@@ -120,9 +121,14 @@ class OccEngine:
 
     def set_prev_rotation(self, index_map):
         """`index_map` (Nq,) int32 numpy / tensor: source BEV cell of every output cell (-1 = outside), e.g. from
-        `rotation_index_map`; None = prev_bev arrives already rotated."""
+        `rotation_index_map`; a real number: the angle in degrees (can_bus[-1]) about the config's rotate_center, whose
+        source cells the engine computes on the device (the same cells as `rotation_index_map`); None = prev_bev arrives
+        already rotated.  The last call wins."""
         if index_map is None:
             _lib.check(self.lib.occb200_engine_set_prev_rotation(self._h, None))
+            return
+        if isinstance(index_map, numbers.Real):
+            _lib.check(self.lib.occb200_engine_set_prev_rotation_angle(self._h, float(index_map)))
             return
         m = np.ascontiguousarray(index_map.cpu().numpy() if isinstance(index_map, torch.Tensor) else index_map, np.int32)
         assert m.shape == (self.Nq,)
@@ -245,16 +251,21 @@ class OccEngine:
         storage precision, allocated (True) or freed (False).  Either way the next video frame starts a new scene."""
         with torch.cuda.device(self.device):
             _lib.check(self.lib.occb200_engine_set_history(self._h, int(enabled)))
+        self.history = bool(enabled)
+
+    def rotation_map(self, angle_deg):
+        """-> CUDA int32 (Nq,): the source cell of every BEV cell (-1 = outside) that the engine computes on the device for a
+        rotation by `angle_deg` about the config's rotate_center; equal to `rotation_index_map` of the same angle."""
+        m = torch.empty(self.Nq, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.occb200_engine_rotation_map(self._h, float(angle_deg), _lib.ptr(m), _lib.stream_ptr()))
+        return m
 
     def _rotation_host(self, rotation):
-        """None, an angle in degrees (can_bus[-1]; the map of `rotation_index_map` about the config's rotate_center) or an
-        index map (Nq,) -> int32 numpy (Nq,) or None.  `submit_host_video` hands the map to the engine, which rejects
-        entries outside [-1, Nq)."""
+        """None or an index map (Nq,) -> int32 numpy (Nq,) or None.  `submit_host_video` hands the map to the engine, which
+        rejects entries outside [-1, Nq)."""
         if rotation is None:
             return None
-        if isinstance(rotation, numbers.Real):
-            return rotation_index_map(self.cfg['bev_h'], self.cfg['bev_w'], float(rotation),
-                                      self.cfg.get('rotate_center', [100, 100]))
         m = np.ascontiguousarray(rotation.cpu().numpy() if isinstance(rotation, torch.Tensor) else rotation, np.int32)
         if m.shape != (self.Nq,):
             raise ValueError(f'rotation map: shape {m.shape} != ({self.Nq},)')
@@ -262,8 +273,8 @@ class OccEngine:
 
     def _rotation_dev(self, rotation):
         """the same as a CUDA int32 tensor on the current stream.  A CUDA map is used as given (the engine reads entries
-        outside [-1, Nq) as -1); a host map or an angle is range-checked here and uploaded for this frame only: the upload
-        and the frame are ordered on the current stream, so the temporary can be freed when the call returns."""
+        outside [-1, Nq) as -1); a host map is range-checked here and uploaded for this frame only: the upload and the frame
+        are ordered on the current stream, so the temporary can be freed when the call returns."""
         if isinstance(rotation, torch.Tensor) and rotation.is_cuda:
             if rotation.dtype != torch.int32 or tuple(rotation.shape) != (self.Nq,) or not rotation.is_contiguous() \
                     or rotation.device != self.device:
@@ -280,26 +291,37 @@ class OccEngine:
         """One frame of a video (needs `set_history()`): `feats` as for `forward`; the previous BEV is the engine's history,
         rotated by `rotation` (None, an angle in degrees or an index map), unless `scene_start` or this is the first frame
         since `set_history()` (self mode).  Equals `forward(feats, prev_bev=<previous frame's bev_embed>)` with the same
-        rotation, bit for bit; the frame's BEV stays in the history whether or not 'bev_embed' is in `want`."""
+        rotation, bit for bit; the frame's BEV stays in the history whether or not 'bev_embed' is in `want`.  An angle
+        costs no host work: the engine computes the cells of `rotation_index_map(angle)` on the device."""
         if not self.feat_channels_last and self.feat_dtype != torch.uint8:
             feats = [f.contiguous() for f in feats]
         self._check_feats(feats, cuda=True)
-        rot = self._rotation_dev(rotation)
         out = self._outputs(want)
+        outs = (_lib.ptr(out.get('bev_embed')), _lib.ptr(out.get('occ')), _lib.ptr(out.get('flow')),
+                _lib.ptr(out.get('occ_cls')), _lib.ptr(out.get('occ_cls_i64')))
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.occb200_engine_forward_video(
-                self._h, self._feat_ptrs(feats), _lib.ptr(rot), int(bool(scene_start)), _lib.ptr(out.get('bev_embed')),
-                _lib.ptr(out.get('occ')), _lib.ptr(out.get('flow')), _lib.ptr(out.get('occ_cls')),
-                _lib.ptr(out.get('occ_cls_i64')), _lib.stream_ptr()))
+            if isinstance(rotation, numbers.Real):
+                _lib.check(self.lib.occb200_engine_forward_video_angle(
+                    self._h, self._feat_ptrs(feats), float(rotation), int(bool(scene_start)), *outs, _lib.stream_ptr()))
+            else:
+                rot = self._rotation_dev(rotation)
+                _lib.check(self.lib.occb200_engine_forward_video(
+                    self._h, self._feat_ptrs(feats), _lib.ptr(rot), int(bool(scene_start)), *outs, _lib.stream_ptr()))
         return out
 
     def submit_host_video(self, slot, feats_host, occ_out, flow_out, rotation=None, scene_start=False):
         """Pipelined host-buffer video frame (slot 0/1; `submit_host` + the history of `forward_video`): returns
-        immediately, `wait_host(slot)` completes it.  The rotation map is copied before the call returns."""
+        immediately, `wait_host(slot)` completes it.  An index map is copied before the call returns; an angle needs no
+        map at all."""
         self._check_feats(feats_host, cuda=False)
-        rot = self._rotation_host(rotation)
         arr = self._feat_ptrs(feats_host)
         with torch.cuda.device(self.device):
+            if isinstance(rotation, numbers.Real):
+                _lib.check(self.lib.occb200_engine_submit_host_video_angle(
+                    self._h, slot, arr, float(rotation), int(bool(scene_start)), _lib.ptr(occ_out), _lib.ptr(flow_out),
+                    _lib.stream_ptr()))
+                return
+            rot = self._rotation_host(rotation)
             _lib.check(self.lib.occb200_engine_submit_host_video(self._h, slot, arr, _lib.ptr(rot), int(bool(scene_start)),
                                                                  _lib.ptr(occ_out), _lib.ptr(flow_out), _lib.stream_ptr()))
 

@@ -512,14 +512,7 @@ class BEVFormerOccHead(BaseModule):
             eng.set_cameras([img_metas[b] if b == 0 else dict(img_metas[b], ego2lidar=img_metas[0]['ego2lidar'],
                                                               img_shape=img_metas[0]['img_shape'])])
             eng.set_prev_rotation(None if rot_maps is None else rot_maps[b])
-            fb = [f[b] for f in mlvl_feats]
-            # fp32 (the reference's dtype), bf16, or bf16 whose memory is channels-last (the native backbone's output)
-            cl = fb[0].dtype == torch.bfloat16 and all((not f.is_contiguous()) and f.permute(0, 2, 3, 1).is_contiguous() for f in fb)
-            want_dt = torch.bfloat16 if fb[0].dtype == torch.bfloat16 else torch.float32
-            if want_dt != eng.feat_dtype or cl != eng.feat_channels_last:
-                eng.set_input_dtype(want_dt, channels_last=cl)
-            if fb[0].dtype != eng.feat_dtype:
-                fb = [f.float() for f in fb]
+            fb = self._engine_feats(eng, [f[b] for f in mlvl_feats])
             out = eng.forward(fb, prev_bev=None if prev_bev is None else prev_bev[b],
                               want=('bev_embed',) if only_bev else want)
             bevs.append(out['bev_embed'])
@@ -535,6 +528,38 @@ class BEVFormerOccHead(BaseModule):
         # instead of re-reading the 43 MB of logits (reference: softmax(-1).argmax(-1), bevformer_occ_head.py:211-212)
         return {'bev_embed': bev_embed, 'occ': torch.stack(occs) if occs else None, 'flow': torch.stack(flows),
                 'occ_cls': torch.stack(clss)}
+
+    @staticmethod
+    def _engine_feats(eng, fb):
+        """one batch item's levels as the engine takes them: fp32 (the reference's dtype), bf16, or bf16 whose memory is
+        channels-last (the native backbone's output); the engine's input dtype follows them"""
+        cl = fb[0].dtype == torch.bfloat16 and all((not f.is_contiguous()) and f.permute(0, 2, 3, 1).is_contiguous() for f in fb)
+        want_dt = torch.bfloat16 if fb[0].dtype == torch.bfloat16 else torch.float32
+        if want_dt != eng.feat_dtype or cl != eng.feat_channels_last:
+            eng.set_input_dtype(want_dt, channels_last=cl)
+        if fb[0].dtype != eng.feat_dtype:
+            fb = [f.float() for f in fb]
+        return fb
+
+    def forward_video(self, mlvl_feats, img_metas, scene_start):
+        """One video frame of batch 1 with the BEV history kept inside the engine (`OccEngine.forward_video`): the previous
+        frame's BEV never leaves the engine, and the rotation by can_bus[-1] degrees (none when the transformer's
+        rotate_prev_bev is False) is computed on the device.  `scene_start` (or the first frame after the engine is built)
+        runs without a previous BEV.  Bit-identical to `forward(mlvl_feats, img_metas, prev_bev=<previous frame's
+        bev_embed>, test=True)`; the result's 'bev_embed' is None."""
+        _need_cuda(mlvl_feats[0], 'BEVFormerOccHead')
+        if mlvl_feats[0].shape[0] != 1:
+            raise ValueError(f'forward_video takes batch 1, got {mlvl_feats[0].shape[0]}')
+        eng = self._get_engine(mlvl_feats[0].device, [tuple(f.shape[-2:]) for f in mlvl_feats])
+        if not eng.history:
+            eng.set_history(True)
+        eng.set_cameras([img_metas[0]])
+        rotation = float(img_metas[0]['can_bus'][-1]) if self.transformer.rotate_prev_bev else None
+        want = ('occ', 'flow', 'occ_cls_i64') if self.test_logits else ('flow', 'occ_cls_i64')
+        out = eng.forward_video(self._engine_feats(eng, [f[0] for f in mlvl_feats]), rotation=rotation,
+                                scene_start=scene_start, want=want)
+        return {'bev_embed': None, 'occ': out['occ'][None] if 'occ' in out else None, 'flow': out['flow'][None],
+                'occ_cls': out['occ_cls_i64'][None]}
 
     def get_occ(self, preds_dicts, img_metas, rescale=False):
         cls = preds_dicts.get('occ_cls')
@@ -618,7 +643,7 @@ class BEVFormerOcc(BaseModule):
 
     def __init__(self, pts_bbox_head=None, img_backbone=None, img_neck=None, use_grid_mask=False, video_test_mode=False,
                  train_cfg=None, test_cfg=None, pretrained=None, feature_extractor=None, native_backbone=True,
-                 backbone_precision=None, temporal_test=False,
+                 backbone_precision=None, temporal_test=False, engine_history=False,
                  frame_norm_cfg=dict(mean=[103.530, 116.280, 123.675], std=[1.0, 1.0, 1.0], to_rgb=False),
                  frame_pad=dict(size_divisor=32), **kwargs):
         super().__init__()
@@ -651,6 +676,12 @@ class BEVFormerOcc(BaseModule):
         # turns the cache on the way upstream BEVFormer uses it: the previous frame's BEV (kept on the device) feeds the
         # next frame of the SAME scene; a new `scene_token` (or prev_bev_exists=False) resets it (SURVEY 8f rank 3).
         self.temporal_test = temporal_test
+        # engine_history=True (with temporal_test and video_test_mode): batch-1 frames keep that BEV inside the head's frame
+        # engine instead (`BEVFormerOccHead.forward_video`): no fp32 bev_embed round trip and the rotation is computed on
+        # the device.  The outputs are bit-identical to the cache's; `prev_frame_info['prev_bev']` then stays None.
+        # Batch > 1 keeps the cache, and a batch > 1 call in the middle of a scene makes the next batch-1 frame start anew.
+        self.engine_history = engine_history
+        self._engine_history_valid = False
         self.prev_frame_info = {'prev_bev': None, 'scene_token': None, 'prev_pos': 0, 'prev_angle': 0}
 
     def _get_backbone_engine(self, device, shape):
@@ -770,21 +801,46 @@ class BEVFormerOcc(BaseModule):
         feats = img_feats if img_feats is not None else self.extract_feat(img, img_metas)
         return self.simple_test_pts(feats, img_metas, prev_bev, rescale=rescale)
 
+    def simple_test_video(self, img_metas, img=None, img_feats=None, scene_start=False, rescale=False, **kwargs):
+        """`simple_test` of one batch-1 video frame on the head engine's BEV history (`BEVFormerOccHead.forward_video`)
+        -> (occ, flow)"""
+        if img_feats is None and isinstance(img, torch.Tensor) and img.dtype == torch.uint8:
+            img_metas = self.frame_metas(img_metas, img)
+            feats = self.extract_frame_feat(img)
+        else:
+            feats = img_feats if img_feats is not None else self.extract_feat(img, img_metas)
+        outs = self.pts_bbox_head.forward_video(feats, img_metas, scene_start)
+        return self.pts_bbox_head.get_occ(outs, img_metas, rescale=rescale)
+
+    @staticmethod
+    def _batch_size(img, img_feats):
+        if img_feats is not None:
+            return img_feats[0].shape[0]
+        return 1 if img is None or img.dim() == 4 else img.shape[0]
+
     def forward_test(self, img_metas, img=None, img_feats=None, **kwargs):
         metas = img_metas[0] if isinstance(img_metas[0], (list, tuple)) else img_metas
         if isinstance(img, (list, tuple)):
             img = img[0]
         prev_bev = None                                                                             # reference: prev_bev=None
-        if self.temporal_test and self.video_test_mode:
+        video = self.temporal_test and self.video_test_mode
+        if video:
             info = self.prev_frame_info
             tok = metas[0].get('scene_token')
-            if tok != info['scene_token'] or not metas[0].get('prev_bev_exists', True):
+            new_scene = tok != info['scene_token'] or not metas[0].get('prev_bev_exists', True)
+            if new_scene:
                 info['prev_bev'] = None                                                             # first frame of a scene
             info['scene_token'] = tok
             prev_bev = info['prev_bev']
+            if self.engine_history and self._batch_size(img, img_feats) == 1:
+                occ, flow = self.simple_test_video(metas, img, img_feats=img_feats,
+                                                   scene_start=new_scene or not self._engine_history_valid, **kwargs)
+                self._engine_history_valid = True
+                return {'occ_results': occ.cpu(), 'flow_results': flow.cpu()}
         new_prev_bev, occ, flow = self.simple_test(metas, img, img_feats=img_feats, prev_bev=prev_bev, **kwargs)
-        if self.temporal_test and self.video_test_mode:
+        if video:
             self.prev_frame_info['prev_bev'] = new_prev_bev                                         # (B, C, H, W), stays on the device
+            self._engine_history_valid = False
         return {'occ_results': occ.cpu(), 'flow_results': flow.cpu()}
 
     def forward(self, return_loss=False, **kwargs):

@@ -7,18 +7,23 @@ JSON line.
 
 Per run (the variants alternate inside every run):
   device   (CUDA events, features on the device)
-    explicit        : forward(prev_bev = previous bev_embed) with one global rotation map (3 degrees), as bench.py's
-                      temporal_config leg; the caller carries bev_embed
-    video_fixed     : forward_video with the same 3 degrees every frame
-    video_per_frame : forward_video cycling through 8 angles (their index maps come from rotation_index_map's host cache)
-    video_unique    : forward_video with a new angle every frame, as real can_bus[-1] values are: every frame pays the host
-                      torchvision rotate of rotation_index_map and the map upload
-    self_mode       : forward(prev_bev = None): the ceiling, no temporal attention
+    explicit           : forward(prev_bev = previous bev_embed) with one global rotation map (3 degrees), as bench.py's
+                         temporal_config leg; the caller carries bev_embed
+    video_fixed        : forward_video with the host index map of 3 degrees every frame (range-checked and uploaded per frame)
+    video_per_frame    : forward_video cycling through the host maps of 8 angles (rotation_index_map's host cache)
+    video_unique       : forward_video with a new angle every frame, as real can_bus[-1] values are, as a host map: every
+                         frame pays the host torchvision rotate of rotation_index_map and the map upload
+    video_unique_angle : the same new angle every frame handed over as the angle: the engine computes the source cells on
+                         the device inside the history gather (no host work, no upload)
+    self_mode          : forward(prev_bev = None): the ceiling, no temporal attention
   host     (wall clock, ends synchronised; pinned fp32 features, two frames in flight)
-    stream_host_video with the 8 cycling angles, and with a new angle every frame, against stream_host (self mode)
-Also: whether explicit and video paths give byte-identical occ_cls / flow / bev_embed over a frame sequence with per-frame
-angles, and the launches per frame of each variant.  The card's name, power limit and SM clock are read (nvidia-smi queries
-only) in the same call.
+    stream_host_video with the 8 cycling host maps, with a new angle every frame as a host map and as the angle, against
+    stream_host (self mode)
+  detector (wall clock, BEVFormerOcc.forward_test on img_feats, results copied to the host as forward_test returns them)
+    temporal_test with the prev_bev cache (explicit) against engine_history=True, a new angle every frame
+Also: whether explicit and video paths (angles) give byte-identical occ_cls / flow / bev_embed over a frame sequence with
+per-frame angles, and the launches per frame of each variant.  The card's name, power limit and SM clock are read
+(nvidia-smi queries only) in the same call.
 """
 import argparse
 import itertools
@@ -70,6 +75,24 @@ def wall(fn, n):
     return (time.perf_counter() - t0) * 1e3 / n
 
 
+def detector(cfg, params, fr_dev):
+    """BEVFormerOcc(temporal_test=True, video_test_mode=True) with the benchmark engine's configuration and weights; one
+    scene, so every frame after the first has a previous BEV"""
+    import projects.mmdet3d_plugin  # noqa: F401
+    from occnet_b200.mmcv_shim import build_detector
+    det = build_detector(dict(type='BEVFormerOcc', video_test_mode=True, temporal_test=True,
+                              pts_bbox_head=dict(fixtures.head_cfg(cfg), precision='bf16', test_logits=False)))
+    det = det.to(fr_dev[0][0].device).eval()
+    det.pts_bbox_head.load_state_dict(params, strict=True)
+    feats = [[f[None] for f in fr] for fr in fr_dev]
+    metas = []
+    for _ in range(3):
+        m = fixtures.make_img_metas(cfg, bs=1, can_bus_angle=0.0)
+        m[0]['scene_token'] = 'bench'
+        metas.append(m)
+    return det, feats, metas
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--frames', type=int, default=32, help='frames per timed variant')
@@ -94,6 +117,10 @@ def main():
     X, Y, Z = eng.vox_shape
     want_video = ('flow', 'occ_cls')
     fresh = (5.0 + 0.0123 * k for k in itertools.count())          # angles never seen before: no cache hits
+    per_frame_maps = [rotation_index_map(cfg['bev_h'], cfg['bev_w'], a, center) for a in ANGLES]
+
+    def fresh_map():
+        return rotation_index_map(cfg['bev_h'], cfg['bev_w'], next(fresh), center)
     state = {'prev': None}
 
     def explicit(i):
@@ -101,17 +128,22 @@ def main():
 
     variants = {
         'explicit': explicit,
-        'video_fixed': lambda i: eng.forward_video(fr_dev[i % 3], rotation=3.0, want=want_video),
-        'video_per_frame': lambda i: eng.forward_video(fr_dev[i % 3], rotation=ANGLES[i % len(ANGLES)], want=want_video),
-        'video_unique': lambda i: eng.forward_video(fr_dev[i % 3], rotation=next(fresh), want=want_video),
+        'video_fixed': lambda i: eng.forward_video(fr_dev[i % 3], rotation=fixed_map, want=want_video),
+        'video_per_frame': lambda i: eng.forward_video(fr_dev[i % 3], rotation=per_frame_maps[i % len(ANGLES)], want=want_video),
+        'video_unique': lambda i: eng.forward_video(fr_dev[i % 3], rotation=fresh_map(), want=want_video),
+        'video_unique_angle': lambda i: eng.forward_video(fr_dev[i % 3], rotation=next(fresh), want=want_video),
         'self_mode': lambda i: eng.forward(fr_dev[i % 3], want=want_video),
     }
 
     def host_video(n):
-        for _ in eng.stream_host_video((fr_host[i % 3], ANGLES[i % len(ANGLES)], False) for i in range(n)):
+        for _ in eng.stream_host_video((fr_host[i % 3], per_frame_maps[i % len(ANGLES)], False) for i in range(n)):
             pass
 
     def host_video_unique(n):
+        for _ in eng.stream_host_video((fr_host[i % 3], fresh_map(), False) for i in range(n)):
+            pass
+
+    def host_video_unique_angle(n):
         for _ in eng.stream_host_video((fr_host[i % 3], next(fresh), False) for i in range(n)):
             pass
 
@@ -126,7 +158,19 @@ def main():
             fn(i)
     host_video(4)
     host_video_unique(4)
+    host_video_unique_angle(4)
     host_self(4)
+    det, det_feats, det_metas = detector(cfg, params, fr_dev)
+
+    def det_run(engine_history):
+        def run(n):
+            det.engine_history = engine_history
+            for i in range(n):
+                det_metas[i % 3][0]['can_bus'][-1] = next(fresh)
+                det(return_loss=False, img_feats=det_feats[i % 3], img_metas=[det_metas[i % 3]])
+        return run
+    det_run(False)(4)
+    det_run(True)(4)
     torch.cuda.synchronize()
     launches = {}
     for name, fn in variants.items():
@@ -141,7 +185,10 @@ def main():
             r[name + '_ms'] = round(timed(fn, args.frames), 4)
         r['host_video_ms'] = round(wall(host_video, args.frames), 4)
         r['host_video_unique_ms'] = round(wall(host_video_unique, args.frames), 4)
+        r['host_video_unique_angle_ms'] = round(wall(host_video_unique_angle, args.frames), 4)
         r['host_self_ms'] = round(wall(host_self, args.frames), 4)
+        r['detector_explicit_ms'] = round(wall(det_run(False), args.frames), 4)
+        r['detector_engine_history_ms'] = round(wall(det_run(True), args.frames), 4)
         runs.append(r)
     info_after = card()
 
@@ -174,6 +221,9 @@ def main():
         'layers': args.layers, 'frames_per_variant': args.frames, 'runs': runs, 'median_ms': med,
         'video_fixed_vs_explicit_speedup': round(med['explicit_ms'] / med['video_fixed_ms'], 4),
         'video_per_frame_vs_explicit_speedup': round(med['explicit_ms'] / med['video_per_frame_ms'], 4),
+        'video_unique_angle_vs_host_map_speedup': round(med['video_unique_ms'] / med['video_unique_angle_ms'], 4),
+        'host_video_unique_angle_vs_host_map_speedup': round(med['host_video_unique_ms'] / med['host_video_unique_angle_ms'], 4),
+        'detector_engine_history_vs_explicit_speedup': round(med['detector_explicit_ms'] / med['detector_engine_history_ms'], 4),
         'launches_per_frame': launches,
         'outputs_identical_explicit_vs_video': identical, 'outputs_identical_explicit_vs_host_video': host_identical,
         'card_before': info_before, 'card_after': info_after,
