@@ -206,6 +206,30 @@ int occb200_engine_forward_video_angle(occb200_engine* e, const float* const* fe
 int occb200_engine_submit_host_video_angle(occb200_engine* e, int slot, const float* const* feats_host, double angle_deg,
                                            int scene_start, int64_t* occ_cls_i64_host, float* flow_host, void* stream);
 
+/* Ray records: what the Occupancy-and-Flow challenge file holds per frame, {pcd_cls int8, pcd_dist fp16, pcd_flow fp16}
+ * (datasets/nuscenes_occ.py:189-257), cast inside the frame that predicted the volumes.  T <= 8 lidar origins x M rays go
+ * through the predicted 200 x 200 x 16 volume once (ray_metrics.process_one_sample's arithmetic, [R4]); row t * M + m holds the
+ * class of the first occupied voxel (the exit voxel, or voxel (0,0,0) for a ray that never enters the grid), its distance in
+ * metres (-0.4 for such a ray) and its flow, narrowed as numpy's astype does (round to nearest even, overflow to inf, NaN kept).
+ *
+ * _set_rays uploads the constant ray bundle (HOST f32 [M,3], generate_lidar_rays) once.  Synchronous; it also disarms.  Change
+ * the bundle only when no frame is in flight.
+ * _request_rays arms ONE frame: the next frame call of any kind (_forward, _forward_video[_angle], _forward_host,
+ *   _submit_host[_video[_angle]]) that passes its own checks consumes the request and, after its head kernel, launches
+ *   ray_records_kernel on its stream from the volumes it produced: one kernel more than occb200_engine_launches_per_frame
+ *   counts for an unarmed frame.  origins_host: HOST [T,3] f32, or f64 if origin_is_f64 (the arithmetic follows torch's type
+ *   promotion); they are copied into the request and travel as a kernel argument, so the caller may reuse the array at once
+ *   and frames in flight cannot see each other's origins.  Outputs cls_i8 [T*M], dist_f16 [T*M], flow_f16 [T*M,2]: DEVICE
+ *   buffers for the device calls; (pinned) HOST buffers for the host calls, written by the call's device->host copy and
+ *   complete when _forward_host returns / at _wait_host.  Host only, no CUDA call.  T = 0 or NULL origins disarms and returns 0.
+ *   Rejected with error 1, leaving no request armed: NULL engine, T outside 0..8, a NULL output, a non-finite origin, no ray
+ *   bundle set, a grid other than 200 x 200 x 16.  A frame call that is itself rejected leaves the request armed.
+ * With a request armed the host calls accept occ_cls_i64_host == NULL and / or flow_host == NULL and skip that 5.12 MB copy;
+ * without one NULL is rejected as before.  The caller's own outputs are the same bytes with and without a request. */
+int occb200_engine_set_rays(occb200_engine* e, const float* rays_host, int M);
+int occb200_engine_request_rays(occb200_engine* e, const void* origins_host, int origin_is_f64, int T, int8_t* cls_i8,
+                                void* dist_f16, void* flow_f16);
+
 /* Intermediate taps for parity tests (dev f32, valid after a forward; NULL if not produced):
  *   which: 0 = layer output [Nq,C] of layer `layer`; 1 = TSA output (pre-norm, with residual); 2 = SCA output
  *   (pre-norm, with residual); 3 = voxel features [X,Y,Z,out_dim] (converted to fp32 into `dst`);
@@ -216,7 +240,7 @@ int occb200_engine_copy_tap(occb200_engine* e, int which, int layer, float* dst_
 /* Row a2 on its own: reference_points_cam dev f32 [num_cams, Nq, D, 2], bev_mask dev u8 [num_cams, Nq, D]. */
 int occb200_engine_project_pillars(occb200_engine* e, float* ref_cam, uint8_t* mask, void* stream);
 /* number of kernels one forward launches (for the benchmark's gpu_launches claim); with input dtype 3 (camera frames) the
- * attached backbone's kernels are included */
+ * attached backbone's kernels are included; a frame that consumed a ray request launched one kernel more */
 int occb200_engine_launches_per_frame(const occb200_engine* e);
 /* Per-kernel-category device timing with CUDA events on the launch stream (benchmark roofline).
  * Categories: 0 pack/prepare, 1 dense GEMM, 2 TSA gather, 3 SCA gather, 4 LayerNorm, 5 bev->voxel, 6 conv3d,
@@ -243,6 +267,13 @@ int occb200_ray_metric_accumulate(const uint8_t* sem_pred, const float* flow_pre
                                   const float* flow_gt, const void* origins, int origin_is_f64, int T,
                                   const float* rays, int M, double* counters, float* pcd_pred, float* pcd_gt,
                                   void* stream);
+
+/* The ray-record operator on its own (see occb200_engine_request_rays): sem_u8 dev u8 [200,200,16], flow dev f32
+ * [200,200,16,2], origins_host HOST [T,3] (f32, or f64 if origin_is_f64), T in 1..8, rays_dev dev f32 [M,3]; outputs dev
+ * cls_i8 [T*M], dist_f16 [T*M], flow_f16 [T*M,2].  One launch of ray_records_kernel on `stream`.  A NULL pointer, T or M out
+ * of range or a non-finite origin returns 1 before any CUDA call. */
+int occb200_ray_records(const uint8_t* sem_u8, const float* flow, const void* origins_host, int origin_is_f64, int T,
+                        const float* rays_dev, int M, int8_t* cls_i8, void* dist_f16, void* flow_f16, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Building blocks exposed for the module-level API mirror and for kernel tests (dev pointers).

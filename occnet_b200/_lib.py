@@ -48,6 +48,9 @@ SIGNATURES = {
     'occb200_engine_submit_host_video': (_i, [_vp, _i, ctypes.POINTER(_vp), _vp, _i, _vp, _vp, _vp]),
     'occb200_engine_forward_video_angle': (_i, [_vp, ctypes.POINTER(_vp), _f64, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     'occb200_engine_submit_host_video_angle': (_i, [_vp, _i, ctypes.POINTER(_vp), _f64, _i, _vp, _vp, _vp]),
+    'occb200_engine_set_rays': (_i, [_vp, _vp, _i]),
+    'occb200_engine_request_rays': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
+    'occb200_ray_records': (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp]),
     'occb200_engine_enable_taps': (_i, [_vp, _i]),
     'occb200_engine_copy_tap': (_i, [_vp, _i, _i, _vp, _vp]),
     'occb200_engine_project_pillars': (_i, [_vp, _vp, _vp, _vp]),

@@ -104,11 +104,29 @@ struct occb200_engine {
     DevBuf tap_layer, tap_tsa, tap_sca;
     // fp32-grade tensor-core configuration (precision 0 + use_tensor_cores): bf16 [hi | lo] splits of the GEMM operands
     DevBuf split_ws, tokens_split;
+    // ray records (occb200_engine_set_rays / _request_rays): the constant ray bundle, and the request the next frame consumes.
+    // The origins travel inside the request and then as a kernel argument, so nothing is uploaded per frame.
+    DevBuf rays;
+    int rays_M = 0;
+    struct RayRequest {
+        bool armed = false;
+        RayOrigins org;
+        int8_t* cls = nullptr;          // device pointers for the device calls, host pointers for the host calls
+        void *dist = nullptr, *flow = nullptr;
+    } ray_req;
+    // what an armed frame needs beyond the caller's outputs: the u8 class volume / the flow when the caller asked for neither,
+    // and for the host calls the device staging of the three record arrays.  One set for the device calls and _forward_host,
+    // one per _submit_host slot (a slot's device->host copy overlaps the next frame's kernels).
+    struct RayStage {
+        DevBuf sem, flow, cls, dist, rflow;
+        void release() { sem.release(); flow.release(); cls.release(); dist.release(); rflow.release(); }
+    } ray_stage;
     // host-buffer variant
     DevBuf feats_dev[4], occ_i64_dev, flow_dev;
     // pipelined host-buffer variant: 2 slots, copies on their own streams, compute on the caller's stream
     struct Slot {
         DevBuf feats[4], occ, flow;
+        RayStage ray_stage;
         DevBuf rot;                     // _submit_host_video: the frame's rotation map, uploaded from rot_pinned on h2d_stream[0]
         int32_t* rot_pinned = nullptr;
         cudaEvent_t h2d_done[4] = {nullptr, nullptr, nullptr, nullptr}, compute_done = nullptr, d2h_done = nullptr;
@@ -665,8 +683,63 @@ int check_frame(const occb200_engine* e, const float* const* feats)
     return 0;
 }
 
+int ensure(DevBuf& b, size_t n) { return b.bytes != n && b.alloc(n) ? 2 : 0; }
+
+// The host calls hand an armed request device staging for its three record arrays and copy them out after the frame: the
+// request's host pointers are returned in `host`.
+int stage_ray_request(occb200_engine* e, occb200_engine::RayStage& rs, occb200_engine::RayRequest* host)
+{
+    *host = e->ray_req;
+    if (!host->armed) return 0;
+    const size_t n = (size_t)8 * e->rays_M;                        // room for the largest T: no reallocation between frames
+    if (ensure(rs.cls, n) || ensure(rs.dist, n * 2) || ensure(rs.rflow, n * 4)) { e->ray_req.armed = false; return 2; }
+    e->ray_req.cls = rs.cls.as<int8_t>(); e->ray_req.dist = rs.dist.p; e->ray_req.flow = rs.rflow.p;
+    return 0;
+}
+
+int copy_ray_records(const occb200_engine* e, const occb200_engine::RayStage& rs, const occb200_engine::RayRequest& host,
+                     cudaStream_t st)
+{
+    if (!host.armed) return 0;
+    const size_t n = (size_t)host.org.T * e->rays_M;
+    OCC_CUDA(cudaMemcpyAsync(host.cls, rs.cls.p, n, cudaMemcpyDeviceToHost, st));
+    OCC_CUDA(cudaMemcpyAsync(host.dist, rs.dist.p, n * 2, cudaMemcpyDeviceToHost, st));
+    OCC_CUDA(cudaMemcpyAsync(host.flow, rs.rflow.p, n * 4, cudaMemcpyDeviceToHost, st));
+    return 0;
+}
+
+int run_frame_volumes(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed, float* occ_logits,
+                      float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video);
+
+// Every frame call ends up here.  An armed ray request (occb200_engine_request_rays) is consumed by this frame: the head also
+// writes the u8 classes and the flow (into `rs` when the caller did not ask for them) and ray_records_kernel follows it on
+// the frame's stream.
 int run_frame(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed, float* occ_logits,
-              float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video = nullptr)
+              float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video = nullptr,
+              occb200_engine::RayStage* rs = nullptr)
+{
+    const occb200_engine::RayRequest rq = e->ray_req;
+    e->ray_req.armed = false;
+    if (rq.armed) {
+        if (rs == nullptr) rs = &e->ray_stage;
+        const size_t nvox = (size_t)e->cfg.bev_w * e->cfg.bev_h * e->cfg.pillar_h;
+        if (cls_u8 == nullptr) {
+            if (ensure(rs->sem, nvox)) return 2;
+            cls_u8 = rs->sem.as<uint8_t>();
+        }
+        if (flow == nullptr) {
+            if (ensure(rs->flow, nvox * 8)) return 2;
+            flow = rs->flow.as<float>();
+        }
+    }
+    const int rc = run_frame_volumes(e, feats, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, video);
+    if (rc || !rq.armed) return rc;
+    e->launches++;
+    return launch_ray_records(cls_u8, flow, rq.org, e->rays.as<float>(), e->rays_M, rq.cls, rq.dist, rq.flow, st);
+}
+
+int run_frame_volumes(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed, float* occ_logits,
+                      float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video)
 {
     if (e->feats_bf16 == 3) {
         const uint8_t* frames = reinterpret_cast<const uint8_t*>(feats[0]);
@@ -682,14 +755,15 @@ int run_frame(occb200_engine* e, const float* const* feats, const float* prev_be
 // One video frame on device buffers, after every host-side check has passed.  The frame waits for the previous video
 // frame (on whatever stream that ran) before it reads the history, and records hist_done after it has written it.
 int run_video_frame(occb200_engine* e, const float* const* feats, const int32_t* map_dev, const RotGrid* grid, int scene_start,
-                    float* bev_embed, float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st)
+                    float* bev_embed, float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st,
+                    occb200_engine::RayStage* rs = nullptr)
 {
     VideoArgs v;
     v.prev = scene_start == 0 && e->hist_valid;
     v.map = map_dev;
     v.grid = grid;
     if (e->hist_recorded) OCC_CUDA(cudaStreamWaitEvent(st, e->hist_done, 0));
-    const int rc = run_frame(e, feats, nullptr, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, &v);
+    const int rc = run_frame(e, feats, nullptr, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, &v, rs);
     if (rc) return rc;
     OCC_CUDA(cudaEventRecord(e->hist_done, st));
     e->hist_recorded = true;
@@ -785,13 +859,14 @@ void occb200_engine_destroy(occb200_engine* e)
                      &e->q_pos_t, &e->prev_t, &e->tsa_value, &e->tsa_v_query, &e->qproj, &e->attn_out,
                      &e->x_f32, &e->ffn_h, &e->vox0, &e->vox1, &e->vox2, &e->hits, &e->tap_layer, &e->tap_tsa,
                      &e->tap_sca, &e->feats_dev[0], &e->feats_dev[1], &e->feats_dev[2], &e->feats_dev[3],
-                     &e->occ_i64_dev, &e->flow_dev, &e->bb_levels[0], &e->bb_levels[1], &e->bb_levels[2], &e->bb_levels[3]};
+                     &e->occ_i64_dev, &e->flow_dev, &e->rays, &e->bb_levels[0], &e->bb_levels[1], &e->bb_levels[2], &e->bb_levels[3]};
     for (DevBuf* b : all) b->release();
+    e->ray_stage.release();
     if (e->bb_free) cudaEventDestroy(e->bb_free);
     if (e->hist_done) cudaEventDestroy(e->hist_done);
     for (auto& sl : e->slots) {
         for (auto& f : sl.feats) f.release();
-        sl.occ.release(); sl.flow.release(); sl.rot.release();
+        sl.occ.release(); sl.flow.release(); sl.rot.release(); sl.ray_stage.release();
         if (sl.rot_pinned) cudaFreeHost(sl.rot_pinned);
         if (sl.compute_done) {
             for (cudaEvent_t ev : sl.h2d_done) cudaEventDestroy(ev);
@@ -1127,7 +1202,8 @@ int occb200_engine_forward_video_angle(occb200_engine* e, const float* const* fe
 int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_host, int64_t* occ_cls_i64_host,
                                 float* flow_host, void* stream)
 {
-    OCC_CHECK(e && feats_host && occ_cls_i64_host && flow_host, "null pointer");
+    // with a ray request armed the caller may decline either volume (NULL): that 5.12 MB copy is then skipped
+    OCC_CHECK(e && feats_host && ((occ_cls_i64_host && flow_host) || e->ray_req.armed), "null pointer");
     OCC_CHECK(e->finalized && e->cameras_set, "engine not finalized / cameras not set");
     if (e->feats_bf16 == 3) OCC_CHECK(e->bb != nullptr && feats_host[0] != nullptr, "input dtype 3 needs an attached backbone and a frame buffer");
     const occb200_config& c = e->cfg;
@@ -1141,13 +1217,17 @@ int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_hos
         OCC_CUDA(cudaMemcpyAsync(e->feats_dev[l].p, feats_host[l], n, cudaMemcpyHostToDevice, st));
         dev_feats[l] = e->feats_dev[l].as<float>();
     }
-    if (e->occ_i64_dev.bytes != nvox * 8 && e->occ_i64_dev.alloc(nvox * 8)) return 2;
-    if (e->flow_dev.bytes != nvox * 8 && e->flow_dev.alloc(nvox * 8)) return 2;
-    int rc = occb200_engine_forward(e, dev_feats, nullptr, nullptr, nullptr, e->flow_dev.as<float>(), nullptr,
-                                    e->occ_i64_dev.as<int64_t>(), stream);
+    if (occ_cls_i64_host && ensure(e->occ_i64_dev, nvox * 8)) return 2;
+    if (ensure(e->flow_dev, nvox * 8)) return 2;
+    if (check_frame(e, dev_feats)) return 1;
+    occb200_engine::RayRequest rays_host;                          // an armed request: records through the engine's staging
+    if (stage_ray_request(e, e->ray_stage, &rays_host)) return 2;
+    int rc = run_frame(e, dev_feats, nullptr, nullptr, nullptr, e->flow_dev.as<float>(), nullptr,
+                       occ_cls_i64_host ? e->occ_i64_dev.as<int64_t>() : nullptr, st);
     if (rc) return rc;
-    OCC_CUDA(cudaMemcpyAsync(occ_cls_i64_host, e->occ_i64_dev.p, nvox * 8, cudaMemcpyDeviceToHost, st));
-    OCC_CUDA(cudaMemcpyAsync(flow_host, e->flow_dev.p, nvox * 8, cudaMemcpyDeviceToHost, st));
+    if (occ_cls_i64_host) OCC_CUDA(cudaMemcpyAsync(occ_cls_i64_host, e->occ_i64_dev.p, nvox * 8, cudaMemcpyDeviceToHost, st));
+    if (flow_host) OCC_CUDA(cudaMemcpyAsync(flow_host, e->flow_dev.p, nvox * 8, cudaMemcpyDeviceToHost, st));
+    if (copy_ray_records(e, e->ray_stage, rays_host, st)) return 2;
     OCC_CUDA(cudaStreamSynchronize(st));
     return 0;
 }
@@ -1157,7 +1237,7 @@ int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_hos
 static int submit_frame(occb200_engine* e, int slot, const float* const* feats_host, int64_t* occ_cls_i64_host, float* flow_host,
                         void* stream, bool video, const int32_t* rot_map_host, const RotGrid* grid, int scene_start)
 {
-    OCC_CHECK(e && feats_host && occ_cls_i64_host && flow_host, "null pointer");
+    OCC_CHECK(e && feats_host && ((occ_cls_i64_host && flow_host) || e->ray_req.armed), "null pointer");
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
     OCC_CHECK(e->finalized && e->cameras_set, "engine not finalized / cameras not set");
     if (e->feats_bf16 == 3) OCC_CHECK(e->bb != nullptr && feats_host[0] != nullptr, "input dtype 3 needs an attached backbone and a frame buffer");
@@ -1216,17 +1296,22 @@ static int submit_frame(occb200_engine* e, int slot, const float* const* feats_h
         OCC_CUDA(cudaEventRecord(s.h2d_done[i], e->h2d_stream[i]));
         OCC_CUDA(cudaStreamWaitEvent(st, s.h2d_done[i], 0));
     }
-    if (s.occ.bytes != nvox * 8 && s.occ.alloc(nvox * 8)) return 2;
-    if (s.flow.bytes != nvox * 8 && s.flow.alloc(nvox * 8)) return 2;
+    if (occ_cls_i64_host && ensure(s.occ, nvox * 8)) return 2;
+    if (ensure(s.flow, nvox * 8)) return 2;
+    int64_t* occ_dev = occ_cls_i64_host ? s.occ.as<int64_t>() : nullptr;
+    if (!video && check_frame(e, dev_feats)) return 1;
+    occb200_engine::RayRequest rays_host;                          // an armed request: records through the slot's staging
+    if (stage_ray_request(e, s.ray_stage, &rays_host)) return 2;
     int rc = video ? run_video_frame(e, dev_feats, rot_map_host ? s.rot.as<int32_t>() : nullptr, grid, scene_start, nullptr,
-                                     nullptr, s.flow.as<float>(), nullptr, s.occ.as<int64_t>(), st)
-                   : occb200_engine_forward(e, dev_feats, nullptr, nullptr, nullptr, s.flow.as<float>(), nullptr,
-                                            s.occ.as<int64_t>(), stream);
+                                     nullptr, s.flow.as<float>(), nullptr, occ_dev, st, &s.ray_stage)
+                   : run_frame(e, dev_feats, nullptr, nullptr, nullptr, s.flow.as<float>(), nullptr, occ_dev, st, nullptr,
+                               &s.ray_stage);
     if (rc) return rc;
     OCC_CUDA(cudaEventRecord(s.compute_done, st));
     OCC_CUDA(cudaStreamWaitEvent(e->d2h_stream, s.compute_done, 0));
-    OCC_CUDA(cudaMemcpyAsync(occ_cls_i64_host, s.occ.p, nvox * 8, cudaMemcpyDeviceToHost, e->d2h_stream));
-    OCC_CUDA(cudaMemcpyAsync(flow_host, s.flow.p, nvox * 8, cudaMemcpyDeviceToHost, e->d2h_stream));
+    if (occ_cls_i64_host) OCC_CUDA(cudaMemcpyAsync(occ_cls_i64_host, s.occ.p, nvox * 8, cudaMemcpyDeviceToHost, e->d2h_stream));
+    if (flow_host) OCC_CUDA(cudaMemcpyAsync(flow_host, s.flow.p, nvox * 8, cudaMemcpyDeviceToHost, e->d2h_stream));
+    if (copy_ray_records(e, s.ray_stage, rays_host, e->d2h_stream)) return 2;
     OCC_CUDA(cudaEventRecord(s.d2h_done, e->d2h_stream));
     s.busy = true;
     return 0;
@@ -1242,7 +1327,7 @@ int occb200_engine_submit_host_video(occb200_engine* e, int slot, const float* c
                                      int scene_start, int64_t* occ_cls_i64_host, float* flow_host, void* stream)
 {
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
-    OCC_CHECK(feats_host && occ_cls_i64_host && flow_host, "null pointer");
+    OCC_CHECK(feats_host && ((occ_cls_i64_host && flow_host) || (e && e->ray_req.armed)), "null pointer");
     OCC_CHECK(e, "null engine");
     return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, true, rot_map_host, nullptr, scene_start);
 }
@@ -1252,7 +1337,7 @@ int occb200_engine_submit_host_video_angle(occb200_engine* e, int slot, const fl
 {
     OCC_CHECK(std::isfinite(angle_deg), "rotation angle must be finite");
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
-    OCC_CHECK(feats_host && occ_cls_i64_host && flow_host, "null pointer");
+    OCC_CHECK(feats_host && ((occ_cls_i64_host && flow_host) || (e && e->ray_req.armed)), "null pointer");
     OCC_CHECK(e, "null engine");
     const RotGrid g = rotation_grid(e, angle_deg);
     return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, true, nullptr, &g, scene_start);
@@ -1265,6 +1350,59 @@ int occb200_engine_wait_host(occb200_engine* e, int slot)
     if (!s.busy) return 0;
     OCC_CUDA(cudaEventSynchronize(s.d2h_done));
     s.busy = false;
+    return 0;
+}
+
+// origins_host [T,3] (f32, or f64 if is_f64) -> the kernel argument; error 1 for a non-finite coordinate
+static int fill_origins(RayOrigins& r, const void* origins_host, int is_f64, int T)
+{
+    r.T = T;
+    r.is_f64 = is_f64 ? 1 : 0;
+    for (int i = 0; i < T * 3; ++i) {
+        const double v = is_f64 ? static_cast<const double*>(origins_host)[i] : (double)static_cast<const float*>(origins_host)[i];
+        OCC_CHECK(std::isfinite(v), "ray origins must be finite");
+        r.o[i / 3][i % 3] = v;
+    }
+    return 0;
+}
+
+int occb200_ray_records(const uint8_t* sem_u8, const float* flow, const void* origins_host, int origin_is_f64, int T,
+                        const float* rays_dev, int M, int8_t* cls_i8, void* dist_f16, void* flow_f16, void* stream)
+{
+    OCC_CHECK(T >= 1 && T <= 8, "T (lidar origins) must be in 1..8");
+    OCC_CHECK(M >= 1, "M (rays) must be positive");
+    OCC_CHECK(sem_u8 && flow && origins_host && rays_dev && cls_i8 && dist_f16 && flow_f16, "null pointer");
+    RayOrigins org;
+    if (fill_origins(org, origins_host, origin_is_f64, T)) return 1;
+    return launch_ray_records(sem_u8, flow, org, rays_dev, M, cls_i8, dist_f16, flow_f16, (cudaStream_t)stream);
+}
+
+int occb200_engine_set_rays(occb200_engine* e, const float* rays_host, int M)
+{
+    OCC_CHECK(e, "null engine");
+    OCC_CHECK(rays_host && M >= 1, "set_rays: null ray bundle or M < 1");
+    e->ray_req.armed = false;
+    if (upload(e->rays, rays_host, (size_t)M * 3)) return 2;
+    e->rays_M = M;
+    return 0;
+}
+
+int occb200_engine_request_rays(occb200_engine* e, const void* origins_host, int origin_is_f64, int T, int8_t* cls_i8,
+                                void* dist_f16, void* flow_f16)
+{
+    if (e) e->ray_req.armed = false;                               // every rejection below leaves the request disarmed
+    OCC_CHECK(T >= 0 && T <= 8, "T (lidar origins) must be in 0..8");
+    OCC_CHECK(e, "null engine");
+    if (T == 0 || origins_host == nullptr) return 0;
+    OCC_CHECK(cls_i8 && dist_f16 && flow_f16, "null pointer");
+    OCC_CHECK(e->rays.p != nullptr, "request_rays: occb200_engine_set_rays() has not been called");
+    OCC_CHECK(e->cfg.bev_w == 200 && e->cfg.bev_h == 200 && e->cfg.pillar_h == 16,
+              "request_rays: the ray caster works on the 200 x 200 x 16 grid only");
+    occb200_engine::RayRequest rq;
+    if (fill_origins(rq.org, origins_host, origin_is_f64, T)) return 1;
+    rq.armed = true;
+    rq.cls = cls_i8; rq.dist = dist_f16; rq.flow = flow_f16;
+    e->ray_req = rq;
     return 0;
 }
 

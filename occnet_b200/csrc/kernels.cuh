@@ -126,5 +126,15 @@ int launch_render_forward(const float* sigma, const float* origin, const float* 
 int launch_ray_metric(const uint8_t* sem_pred, const float* flow_pred, const uint8_t* sem_gt, const float* flow_gt,
                       const void* origins, int origin_is_f64, int T, const float* rays, int M, double* counters,
                       float* pcd_pred, float* pcd_gt, cudaStream_t stream);
+// The lidar origins of one frame (ego frame, metres), passed by value to ray_records_kernel: fp32 origins are stored as their
+// exact double values, is_f64 selects the arithmetic (torch's type promotion in process_one_sample)
+struct RayOrigins {
+    double o[8][3];
+    int T, is_f64;
+};
+// T x M rays through one predicted volume (sem u8 [200,200,16], flow f32 [200,200,16,2]) -> the challenge file's records in
+// process_one_sample's row order: pcd_cls i8 [T*M], pcd_dist f16 [T*M], pcd_flow f16 [T*M,2]
+int launch_ray_records(const uint8_t* sem, const float* flow, const RayOrigins& org, const float* rays, int M, int8_t* pcd_cls,
+                       void* pcd_dist, void* pcd_flow, cudaStream_t stream);
 
 }  // namespace occ

@@ -6,6 +6,8 @@
 // memory per thread) and scans it afterwards; here the first sigma > 0.5 voxel is latched during
 // the walk, which needs no path storage.  The fused kernel casts all T origins x M rays through
 // the predicted and the ground-truth volume in one launch and reduces the 187 counters on device.
+//   ray_records_kernel    <- datasets/nuscenes_occ.py format_results :230-255: the same rays through the predicted volume only,
+//                            written as the challenge file's records (int8 class, fp16 distance, fp16 flow)
 #include <float.h>
 
 #include "common.cuh"
@@ -96,6 +98,28 @@ __global__ void render_forward_kernel(const float* __restrict__ sigma, const flo
 constexpr int NCLS = 17, FREE = 16, NFLOW = 8, NCNT = 11 * NCLS;
 constexpr int GX = 200, GY = 200, GZ = 16;
 
+// Voxel-unit origin og / end point en of one metric ray, exactly as ray_metrics.py:102-112.  torch type promotion: with the
+// dataset's float64 origins (ego_pose_extractor.py:108-119) the arithmetic is double and rounded once by `.float()`; with
+// float32 origins (o holds their exact values) every step is fp32.
+__device__ __forceinline__ void voxel_ray(const double (&o)[3], int origin_is_f64, const float* __restrict__ ray,
+                                          float (&og)[3], float (&en)[3])
+{
+    const float off[3] = {-40.f, -40.f, -1.f};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        if (origin_is_f64) {
+            const double e = (double)ray[k] + o[k];
+            og[k] = (float)((o[k] - (double)off[k]) / (double)0.4f);
+            en[k] = (float)((e - (double)off[k]) / (double)0.4f);
+        } else {
+            const float of = (float)o[k];
+            const float e = __fadd_rn(ray[k], of);
+            og[k] = __fdiv_rn(__fsub_rn(of, off[k]), 0.4f);
+            en[k] = __fdiv_rn(__fsub_rn(e, off[k]), 0.4f);
+        }
+    }
+}
+
 // one thread = one (origin t, ray m); casts through pred and gt, updates the counters
 __global__ void __launch_bounds__(128)
 ray_metric_kernel(const uint8_t* __restrict__ sem_pred, const float* __restrict__ flow_pred,
@@ -109,25 +133,12 @@ ray_metric_kernel(const uint8_t* __restrict__ sem_pred, const float* __restrict_
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx < (int64_t)T * M) {
         const int t = (int)(idx / M), m = (int)(idx % M);
-        // voxel-unit origin / end point exactly as ray_metrics.py:102-112.  torch type promotion: with the
-        // dataset's float64 origins (ego_pose_extractor.py:108-119) the arithmetic is double and rounded
-        // once by `.float()`; with float32 origins every step is fp32.
-        const float off[3] = {-40.f, -40.f, -1.f};
+        const double* od = reinterpret_cast<const double*>(origins) + t * 3;
+        const float* of = reinterpret_cast<const float*>(origins) + t * 3;
+        const double o[3] = {origin_is_f64 ? od[0] : (double)of[0], origin_is_f64 ? od[1] : (double)of[1],
+                             origin_is_f64 ? od[2] : (double)of[2]};
         float og[3], en[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            if (origin_is_f64) {
-                const double o = reinterpret_cast<const double*>(origins)[t * 3 + k];
-                const double e = (double)rays[m * 3 + k] + o;
-                og[k] = (float)((o - (double)off[k]) / (double)0.4f);
-                en[k] = (float)((e - (double)off[k]) / (double)0.4f);
-            } else {
-                const float o = reinterpret_cast<const float*>(origins)[t * 3 + k];
-                const float e = __fadd_rn(rays[m * 3 + k], o);
-                og[k] = __fdiv_rn(__fsub_rn(o, off[k]), 0.4f);
-                en[k] = __fdiv_rn(__fsub_rn(e, off[k]), 0.4f);
-            }
-        }
+        voxel_ray(o, origin_is_f64, rays + m * 3, og, en);
         float row[2][4];
 #pragma unroll
         for (int v = 0; v < 2; ++v) {
@@ -169,6 +180,42 @@ ray_metric_kernel(const uint8_t* __restrict__ sem_pred, const float* __restrict_
         if (s_cnt[i] != 0.0) atomicAdd(&counters[i], s_cnt[i]);
 }
 
+// numpy's astype(np.float16) of a float32: round to nearest even, overflow to inf; a NaN keeps its sign and the top ten
+// payload bits (cvt.rn.f16.f32 would give the canonical NaN 0x7fff instead, and the file would differ in those bytes)
+__device__ __forceinline__ uint16_t half_bits(float v)
+{
+    if (v != v) {
+        const uint32_t u = __float_as_uint(v);
+        uint16_t h = (uint16_t)(0x7c00u | ((u & 0x007fffffu) >> 13));
+        if (h == 0x7c00u) h = 0x7c01u;                                  // the payload was all in the dropped bits
+        return (uint16_t)(h | ((u >> 16) & 0x8000u));
+    }
+    return __half_as_ushort(__float2half_rn(v));
+}
+
+// one thread = one (origin t, ray m): one walk through the predicted volume, one record
+__global__ void __launch_bounds__(128)
+ray_records_kernel(const uint8_t* __restrict__ sem, const float* __restrict__ flow, const RayOrigins org,
+                   const float* __restrict__ rays, int M, int8_t* __restrict__ pcd_cls, uint16_t* __restrict__ pcd_dist,
+                   uint16_t* __restrict__ pcd_flow)
+{
+    const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (int64_t)org.T * M) return;
+    const int t = (int)(idx / M), m = (int)(idx % M);
+    const double o[3] = {org.o[t][0], org.o[t][1], org.o[t][2]};
+    float og[3], en[3];
+    voxel_ray(o, org.is_f64, rays + m * 3, og, en);
+    double gt_d;
+    const Hit h = dda_first_hit(og[0], og[1], og[2], en[0], en[1], en[2], GX, GY, GZ, gt_d,
+                                [&](int x, int y, int z) { return sem[((int64_t)x * GY + y) * GZ + z] != FREE; });
+    const float dist = (h.any ? (float)h.dist : -1.f) * 0.4f;
+    const int64_t vi = ((int64_t)h.x * GY + h.y) * GZ + h.z;           // voxel (0,0,0) for a ray that never enters
+    pcd_cls[idx] = (int8_t)sem[vi];
+    pcd_dist[idx] = half_bits(dist);
+    pcd_flow[idx * 2] = half_bits(flow[vi * 2]);
+    pcd_flow[idx * 2 + 1] = half_bits(flow[vi * 2 + 1]);
+}
+
 }  // namespace
 
 int launch_render_forward(const float* sigma, const float* origin, const float* points, const float* tindex,
@@ -191,6 +238,16 @@ int launch_ray_metric(const uint8_t* sem_pred, const float* flow_pred, const uin
     ray_metric_kernel<<<ceil_div((int64_t)T * M, 128), 128, 0, stream>>>(sem_pred, flow_pred, sem_gt, flow_gt, origins,
                                                                         origin_is_f64, T, rays, M, counters, pcd_pred,
                                                                         pcd_gt);
+    OCC_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int launch_ray_records(const uint8_t* sem, const float* flow, const RayOrigins& org, const float* rays, int M, int8_t* pcd_cls,
+                       void* pcd_dist, void* pcd_flow, cudaStream_t stream)
+{
+    if (org.T == 0 || M == 0) return 0;
+    ray_records_kernel<<<ceil_div((int64_t)org.T * M, 128), 128, 0, stream>>>(
+        sem, flow, org, rays, M, pcd_cls, reinterpret_cast<uint16_t*>(pcd_dist), reinterpret_cast<uint16_t*>(pcd_flow));
     OCC_CUDA(cudaGetLastError());
     return 0;
 }

@@ -5,13 +5,16 @@ This is the host-side counterpart of `BEVFormerOccHead.forward` + `get_occ`
 their reference state_dict keys, camera geometry comes from `img_metas` exactly as
 `BEVFormerEncoder.point_sampling` reads it (encoder.py:94-101, 133-134).
 """
+import contextlib
 import ctypes
+import itertools
 import numbers
 
 import numpy as np
 import torch
 
 from . import _lib
+from .ops import ray_origins_host
 
 PRECISIONS = {'fp32': 0, 'bf16': 1}
 
@@ -91,6 +94,7 @@ class OccEngine:
         self.feat_dtype, self.feat_channels_last = torch.float32, False
         self.backbone = None
         self.history = False                                          # set_history(True) has allocated the BEV history
+        self.num_rays = 0                                             # set_rays() has uploaded the ray bundle
 
     def set_input_dtype(self, dtype, channels_last=False):
         """Feature levels are handed over as `dtype` from now on (torch.float32, the reference's, or torch.bfloat16);
@@ -134,6 +138,50 @@ class OccEngine:
         assert m.shape == (self.Nq,)
         _lib.check(self.lib.occb200_engine_set_prev_rotation(self._h, _lib.ptr(m)))
 
+    # ------------------------------------------------------------------------------------------------------ ray records
+    def set_rays(self, rays=None):
+        """Upload the constant ray bundle, (M,3) float32 (default: `generate_lidar_rays()`), for `ray_origins=`; called on
+        first use."""
+        if rays is None:
+            from .metric import generate_lidar_rays
+            rays = generate_lidar_rays()
+        rays = np.ascontiguousarray(rays, np.float32).reshape(-1, 3)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.occb200_engine_set_rays(self._h, _lib.ptr(rays), rays.shape[0]))
+        self.num_rays = rays.shape[0]
+
+    def ray_buffers(self, T=8, host=False):
+        """{'ray_cls' int8 (T*M,), 'ray_dist' fp16 (T*M,), 'ray_flow' fp16 (T*M,2)}: CUDA tensors, or pinned CPU tensors"""
+        if not self.num_rays:
+            self.set_rays()
+        n = T * self.num_rays
+        kw = dict(pin_memory=True) if host else dict(device=self.device)
+        return {'ray_cls': torch.empty(n, dtype=torch.int8, **kw), 'ray_dist': torch.empty(n, dtype=torch.float16, **kw),
+                'ray_flow': torch.empty((n, 2), dtype=torch.float16, **kw)}
+
+    @contextlib.contextmanager
+    def _ray_request(self, origins, bufs=None, host=False):
+        """Arm the frame call made inside the block with `origins` ((T,3) or (1,T,3), float32 / float64, T <= 8; None: no
+        request).  Yields the record tensors, the first T*M rows of `bufs` (allocated when None).  A frame call that raises
+        leaves nothing armed."""
+        if origins is None:
+            yield {}
+            return
+        o, is64 = ray_origins_host(origins)
+        if not self.num_rays:
+            self.set_rays()
+        if bufs is None:
+            bufs = self.ray_buffers(o.shape[0], host=host)
+        n = o.shape[0] * self.num_rays
+        rec = {k: v[:n] for k, v in bufs.items()}
+        _lib.check(self.lib.occb200_engine_request_rays(self._h, _lib.ptr(o), int(is64), o.shape[0], _lib.ptr(rec['ray_cls']),
+                                                        _lib.ptr(rec['ray_dist']), _lib.ptr(rec['ray_flow'])))
+        try:
+            yield rec
+        except BaseException:
+            self.lib.occb200_engine_request_rays(self._h, None, 0, 0, None, None, None)
+            raise
+
     def _check_feats(self, feats, cuda):
         """A mismatched tensor would be an out-of-bounds device read in the pack kernel: fail on the host instead."""
         if self.feat_dtype == torch.uint8:
@@ -175,9 +223,11 @@ class OccEngine:
             out['occ_cls_i64'] = torch.empty((X, Y, Z), dtype=torch.int64, device=dev)
         return out
 
-    def forward(self, feats, prev_bev=None, want=('bev_embed', 'occ', 'flow', 'occ_cls')):
+    def forward(self, feats, prev_bev=None, want=('bev_embed', 'occ', 'flow', 'occ_cls'), ray_origins=None):
         """feats: 4 CUDA fp32 tensors (num_cams, C, h, w) of one frame, or with `set_input_dtype(torch.uint8)` one CUDA
-        uint8 tensor of camera frames (num_cams, src_h, src_w, 3).  Returns a dict of CUDA tensors."""
+        uint8 tensor of camera frames (num_cams, src_h, src_w, 3).  Returns a dict of CUDA tensors.  `ray_origins` ((T,3) or
+        (1,T,3), T <= 8): the frame also ray-casts its prediction and adds 'ray_cls' int8 (T*M,), 'ray_dist' fp16 (T*M,) and
+        'ray_flow' fp16 (T*M,2), the challenge file's records (`ops.ray_records` of this frame's volumes)."""
         C = self.cfg['embed_dims']
         dev = self.device
         if not self.feat_channels_last and self.feat_dtype != torch.uint8:
@@ -186,64 +236,88 @@ class OccEngine:
         out = self._outputs(want)
         if prev_bev is not None:
             prev_bev = prev_bev.to(device=dev, dtype=torch.float32).reshape(self.Nq, C).contiguous()
-        with torch.cuda.device(dev):
+        with torch.cuda.device(dev), self._ray_request(ray_origins) as rec:
             _lib.check(self.lib.occb200_engine_forward(
                 self._h, self._feat_ptrs(feats), _lib.ptr(prev_bev), _lib.ptr(out.get('bev_embed')),
                 _lib.ptr(out.get('occ')), _lib.ptr(out.get('flow')), _lib.ptr(out.get('occ_cls')),
                 _lib.ptr(out.get('occ_cls_i64')), _lib.stream_ptr()))
+        out.update(rec)
         return out
 
-    def forward_host(self, feats_host, occ_out=None, flow_out=None):
+    def forward_host(self, feats_host, occ_out=None, flow_out=None, ray_origins=None, volumes=True):
         """feats_host: 4 pinned CPU fp32 tensors (num_cams, C, h, w), or one pinned uint8 tensor of camera frames with
         `set_input_dtype(torch.uint8)` (25.9 MB per 6 x 900 x 1600 frame).  H2D + frame + D2H + sync inside.
-        Returns (occ_cls int64 (X,Y,Z) CPU, flow fp32 (X,Y,Z,2) CPU)."""
+        Returns (occ_cls int64 (X,Y,Z) CPU, flow fp32 (X,Y,Z,2) CPU); with `ray_origins` a third element, the frame's ray
+        records as pinned CPU tensors (see `forward`), and with `volumes=False` the two volumes are None and not copied."""
         X, Y, Z = self.vox_shape
-        if occ_out is None or flow_out is None:
+        if not volumes:
+            if ray_origins is None:
+                raise ValueError('volumes=False needs ray_origins')
+            occ_out = flow_out = None
+        elif occ_out is None or flow_out is None:
             if self._pinned is None:
                 self._pinned = (torch.empty((X, Y, Z), dtype=torch.int64).pin_memory(),
                                 torch.empty((X, Y, Z, 2), dtype=torch.float32).pin_memory())
             occ_out, flow_out = self._pinned
         self._check_feats(feats_host, cuda=False)
         arr = self._feat_ptrs(feats_host)
-        with torch.cuda.device(self.device):
+        with torch.cuda.device(self.device), self._ray_request(ray_origins, host=True) as rec:
             _lib.check(self.lib.occb200_engine_forward_host(self._h, arr, _lib.ptr(occ_out), _lib.ptr(flow_out),
                                                             _lib.stream_ptr()))
-        return occ_out, flow_out
+        return (occ_out, flow_out) if ray_origins is None else (occ_out, flow_out, rec)
 
-    def submit_host(self, slot, feats_host, occ_out, flow_out):
-        """Pipelined host-buffer call (slot 0/1): returns immediately; `wait_host(slot)` completes it."""
+    def submit_host(self, slot, feats_host, occ_out, flow_out, ray_origins=None, ray_out=None):
+        """Pipelined host-buffer call (slot 0/1): returns immediately; `wait_host(slot)` completes it.  With `ray_origins` the
+        frame's ray records go to the pinned CPU tensors `ray_out` (`ray_buffers(host=True)`), whose first T*M rows are
+        returned as a dict, and `occ_out` / `flow_out` may be None: that volume is then not copied."""
         self._check_feats(feats_host, cuda=False)
         arr = self._feat_ptrs(feats_host)
-        with torch.cuda.device(self.device):
+        with torch.cuda.device(self.device), self._ray_request(ray_origins, ray_out, host=True) as rec:
             _lib.check(self.lib.occb200_engine_submit_host(self._h, slot, arr, _lib.ptr(occ_out), _lib.ptr(flow_out),
                                                            _lib.stream_ptr()))
+        return rec
 
     def wait_host(self, slot):
         _lib.check(self.lib.occb200_engine_wait_host(self._h, slot))
 
-    def stream_host(self, frames_host):
+    def stream_host(self, frames_host, ray_origins=None, volumes=True):
         """Generator over an iterable of host frames with two frames in flight; yields (occ int64 CPU, flow CPU)
-        views of the slot's pinned output buffers (valid until the slot is reused two frames later)."""
-        return self._stream(frames_host, lambda slot, fr, outs: self.submit_host(slot, fr, *outs))
+        views of the slot's pinned output buffers (valid until the slot is reused two frames later).  `ray_origins`: one
+        origin set per frame ((T,3) or (1,T,3), T <= 8, T may differ between frames); every frame then yields (occ, flow,
+        records) with the frame's ray records {'ray_cls', 'ray_dist', 'ray_flow'} as views of the slot's pinned record
+        buffers (see `forward`).  `volumes=False` (with `ray_origins`): occ and flow are None and never leave the device,
+        786 KB per frame cross the bus at T = 8 instead of 10.24 MB."""
+        if ray_origins is None:
+            if not volumes:
+                raise ValueError('volumes=False needs ray_origins')
+            return self._stream(frames_host, lambda slot, fr, outs, rays: self.submit_host(slot, fr, *outs))
+        return self._stream(zip(frames_host, ray_origins), lambda slot, it, outs, rays: self.submit_host(
+            slot, it[0], *outs, ray_origins=it[1], ray_out=rays), volumes=volumes, rays=True)
 
-    def _stream(self, items, submit):
+    def _stream(self, items, submit, volumes=True, rays=False):
+        """submit(slot, item, (occ, flow) pinned or (None, None), the slot's pinned record buffers or None) -> the frame's
+        records or None"""
         X, Y, Z = self.vox_shape
-        if getattr(self, '_stream_outs', None) is None:              # pinned once: cudaHostAlloc costs milliseconds
+        if volumes and getattr(self, '_stream_outs', None) is None:  # pinned once: cudaHostAlloc costs milliseconds
             self._stream_outs = [(torch.empty((X, Y, Z), dtype=torch.int64).pin_memory(),
                                   torch.empty((X, Y, Z, 2)).pin_memory()) for _ in range(2)]
-        outs = self._stream_outs
+        if rays and getattr(self, '_stream_rays', None) is None:
+            self._stream_rays = [self.ray_buffers(8, host=True) for _ in range(2)]
+        outs = self._stream_outs if volumes else [(None, None)] * 2
         pending = []
+
+        def finish(slot, rec):
+            self.wait_host(slot)
+            return outs[slot] + (rec,) if rays else outs[slot]
+
         for i, item in enumerate(items):
             slot = i & 1
             if len(pending) == 2:
-                s = pending.pop(0)
-                self.wait_host(s)
-                yield outs[s]
-            submit(slot, item, outs[slot])
-            pending.append(slot)
-        for s in pending:
-            self.wait_host(s)
-            yield outs[s]
+                yield finish(*pending.pop(0))
+            rec = submit(slot, item, outs[slot], self._stream_rays[slot] if rays else None)
+            pending.append((slot, rec))
+        for p in pending:
+            yield finish(*p)
 
     # ---------------------------------------------------------------------------------------- video (temporal) inference
     def set_history(self, enabled=True):
@@ -287,12 +361,14 @@ class OccEngine:
             raise ValueError(f'rotation map entry out of range: must be in [-1, {self.Nq})')
         return torch.from_numpy(m).pin_memory().to(self.device, non_blocking=True)
 
-    def forward_video(self, feats, rotation=None, scene_start=False, want=('bev_embed', 'occ', 'flow', 'occ_cls')):
+    def forward_video(self, feats, rotation=None, scene_start=False, want=('bev_embed', 'occ', 'flow', 'occ_cls'),
+                      ray_origins=None):
         """One frame of a video (needs `set_history()`): `feats` as for `forward`; the previous BEV is the engine's history,
         rotated by `rotation` (None, an angle in degrees or an index map), unless `scene_start` or this is the first frame
         since `set_history()` (self mode).  Equals `forward(feats, prev_bev=<previous frame's bev_embed>)` with the same
         rotation, bit for bit; the frame's BEV stays in the history whether or not 'bev_embed' is in `want`.  An angle
-        costs no host work: the engine computes the cells of `rotation_index_map(angle)` on the device."""
+        costs no host work: the engine computes the cells of `rotation_index_map(angle)` on the device.  `ray_origins`: as
+        for `forward`."""
         if not self.feat_channels_last and self.feat_dtype != torch.uint8:
             feats = [f.contiguous() for f in feats]
         self._check_feats(feats, cuda=True)
@@ -300,36 +376,50 @@ class OccEngine:
         outs = (_lib.ptr(out.get('bev_embed')), _lib.ptr(out.get('occ')), _lib.ptr(out.get('flow')),
                 _lib.ptr(out.get('occ_cls')), _lib.ptr(out.get('occ_cls_i64')))
         with torch.cuda.device(self.device):
-            if isinstance(rotation, numbers.Real):
-                _lib.check(self.lib.occb200_engine_forward_video_angle(
-                    self._h, self._feat_ptrs(feats), float(rotation), int(bool(scene_start)), *outs, _lib.stream_ptr()))
-            else:
-                rot = self._rotation_dev(rotation)
-                _lib.check(self.lib.occb200_engine_forward_video(
-                    self._h, self._feat_ptrs(feats), _lib.ptr(rot), int(bool(scene_start)), *outs, _lib.stream_ptr()))
+            rot = None if isinstance(rotation, numbers.Real) else self._rotation_dev(rotation)
+            with self._ray_request(ray_origins) as rec:
+                if isinstance(rotation, numbers.Real):
+                    _lib.check(self.lib.occb200_engine_forward_video_angle(
+                        self._h, self._feat_ptrs(feats), float(rotation), int(bool(scene_start)), *outs, _lib.stream_ptr()))
+                else:
+                    _lib.check(self.lib.occb200_engine_forward_video(
+                        self._h, self._feat_ptrs(feats), _lib.ptr(rot), int(bool(scene_start)), *outs, _lib.stream_ptr()))
+        out.update(rec)
         return out
 
-    def submit_host_video(self, slot, feats_host, occ_out, flow_out, rotation=None, scene_start=False):
+    def submit_host_video(self, slot, feats_host, occ_out, flow_out, rotation=None, scene_start=False, ray_origins=None,
+                          ray_out=None):
         """Pipelined host-buffer video frame (slot 0/1; `submit_host` + the history of `forward_video`): returns
         immediately, `wait_host(slot)` completes it.  An index map is copied before the call returns; an angle needs no
-        map at all."""
+        map at all.  `ray_origins` / `ray_out` and the returned records: as for `submit_host`."""
         self._check_feats(feats_host, cuda=False)
         arr = self._feat_ptrs(feats_host)
-        with torch.cuda.device(self.device):
+        rot = None if isinstance(rotation, numbers.Real) else self._rotation_host(rotation)
+        with torch.cuda.device(self.device), self._ray_request(ray_origins, ray_out, host=True) as rec:
             if isinstance(rotation, numbers.Real):
                 _lib.check(self.lib.occb200_engine_submit_host_video_angle(
                     self._h, slot, arr, float(rotation), int(bool(scene_start)), _lib.ptr(occ_out), _lib.ptr(flow_out),
                     _lib.stream_ptr()))
-                return
-            rot = self._rotation_host(rotation)
-            _lib.check(self.lib.occb200_engine_submit_host_video(self._h, slot, arr, _lib.ptr(rot), int(bool(scene_start)),
-                                                                 _lib.ptr(occ_out), _lib.ptr(flow_out), _lib.stream_ptr()))
+            else:
+                _lib.check(self.lib.occb200_engine_submit_host_video(self._h, slot, arr, _lib.ptr(rot), int(bool(scene_start)),
+                                                                     _lib.ptr(occ_out), _lib.ptr(flow_out), _lib.stream_ptr()))
+        return rec
 
-    def stream_host_video(self, items):
+    def stream_host_video(self, items, volumes=True):
         """`stream_host` for video: items are (feats_host, rotation, scene_start); two frames in flight, yields
-        (occ int64 CPU, flow CPU) views of the slot's pinned output buffers, frame by frame."""
-        return self._stream(items, lambda slot, it, outs: self.submit_host_video(slot, it[0], *outs, rotation=it[1],
-                                                                                  scene_start=it[2]))
+        (occ int64 CPU, flow CPU) views of the slot's pinned output buffers, frame by frame.  Items with a fourth element,
+        the frame's ray origins, make every frame yield (occ, flow, records) as `stream_host(ray_origins=...)` does;
+        `volumes=False` then keeps the volumes on the device."""
+        items = iter(items)
+        first = next(items, None)
+        if first is None:
+            return iter(())
+        rays = len(first) > 3
+        if not volumes and not rays:
+            raise ValueError('volumes=False needs ray origins (a fourth element in every item)')
+        return self._stream(itertools.chain([first], items), lambda slot, it, outs, rb: self.submit_host_video(
+            slot, it[0], *outs, rotation=it[1], scene_start=it[2], ray_origins=it[3] if rays else None, ray_out=rb),
+            volumes=volumes, rays=rays)
 
     def enable_taps(self, on=True):
         _lib.check(self.lib.occb200_engine_enable_taps(self._h, int(on)))

@@ -5,11 +5,13 @@
       reference call site: bevformer/modules/multi_scale_deformable_attn_function.py:118-124
   MultiScaleDeformableAttnFunction_fp32.apply(...)                     :90-128
   dvr.render_forward(sigma, origin, points, tindex, grid, phase)       tools/ray_iou/lib/dvr/dvr.cpp:39-48
+  ray_records(sem_u8, flow, origins): the prediction half of NuSceneOcc.format_results, datasets/nuscenes_occ.py:230-255
 
 Same argument meaning and error behaviour (RuntimeError on non-CUDA / non-contiguous input or a batch
 that does not divide im2col_step).  torch is only the tensor container: the arithmetic happens in
 libocc_b200 through the C ABI.
 """
+import numpy as np
 import torch
 
 from . import _lib
@@ -115,6 +117,51 @@ def render_forward(sigma, origin, points, tindex, grid, phase='test'):
                                               _lib.stream_ptr()))
     torch.cuda.current_stream().synchronize()      # the reference op returns after cudaDeviceSynchronize (dvr.cu:384)
     return [pred, gt, coord]
+
+
+def ray_origins_host(origins):
+    """(T,3) or (1,T,3) lidar origins -> (contiguous numpy (T,3) float32 or float64, is_f64).  float64 origins keep their
+    dtype (process_one_sample's arithmetic then runs in double, torch's type promotion); everything else is cast to float32."""
+    o = origins.detach().cpu().numpy() if isinstance(origins, torch.Tensor) else np.asarray(origins)
+    o = np.ascontiguousarray(o.reshape(-1, 3), np.float64 if o.dtype == np.float64 else np.float32)
+    if not 1 <= o.shape[0] <= 8:
+        raise ValueError(f'ray records take 1..8 lidar origins, got {o.shape[0]}')
+    return o, o.dtype == np.float64
+
+
+_RAYS = {}
+
+
+def lidar_rays(device):
+    """generate_lidar_rays() as a CUDA tensor, uploaded once per device"""
+    from .metric import generate_lidar_rays
+    device = torch.device(device)
+    if device not in _RAYS:
+        _RAYS[device] = torch.from_numpy(generate_lidar_rays()).to(device)
+    return _RAYS[device]
+
+
+def ray_records(sem_u8, flow, origins):
+    """The challenge file's records of one predicted volume: sem_u8 (200,200,16) uint8 and flow (200,200,16,2) fp32 CUDA
+    tensors, origins (T,3) or (1,T,3) float32 / float64 with T <= 8 -> (pcd_cls int8 (T*M,), pcd_dist fp16 (T*M,), pcd_flow
+    fp16 (T*M,2)) CUDA tensors, M = 14040 rays: `process_one_sample`'s rows narrowed as numpy's astype narrows them, from
+    one walk per ray."""
+    _require(sem_u8, 'sem_u8', torch.uint8)
+    _require(flow, 'flow', torch.float32)
+    if tuple(sem_u8.shape) != (200, 200, 16) or tuple(flow.shape) != (200, 200, 16, 2):
+        raise ValueError(f'ray_records needs (200,200,16) classes and (200,200,16,2) flow, got {tuple(sem_u8.shape)} / '
+                         f'{tuple(flow.shape)}')
+    o, is64 = ray_origins_host(origins)
+    rays = lidar_rays(sem_u8.device)
+    n = o.shape[0] * rays.shape[0]
+    cls = torch.empty(n, dtype=torch.int8, device=sem_u8.device)
+    dist = torch.empty(n, dtype=torch.float16, device=sem_u8.device)
+    fl = torch.empty((n, 2), dtype=torch.float16, device=sem_u8.device)
+    lib = _lib.load()
+    with torch.cuda.device(sem_u8.device):
+        _lib.check(lib.occb200_ray_records(_lib.ptr(sem_u8), _lib.ptr(flow), _lib.ptr(o), int(is64), o.shape[0], _lib.ptr(rays),
+                                           rays.shape[0], _lib.ptr(cls), _lib.ptr(dist), _lib.ptr(fl), _lib.stream_ptr()))
+    return cls, dist, fl
 
 
 def _no_autograd(name, *tensors):
