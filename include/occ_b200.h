@@ -230,6 +230,28 @@ int occb200_engine_set_rays(occb200_engine* e, const float* rays_host, int M);
 int occb200_engine_request_rays(occb200_engine* e, const void* origins_host, int origin_is_f64, int T, int8_t* cls_i8,
                                 void* dist_f16, void* flow_f16);
 
+/* Score a frame against its ground truth inside the frame that predicted it: Ray-mIoU / mAVE counters
+ * (datasets/ray_metrics.py:200-257) without the predicted volumes leaving the device.
+ * _request_score arms ONE frame, as _request_rays does: the next frame call of any kind that passes its own checks consumes
+ *   the request and, after its head kernel, launches ray_score_kernel on its stream: one kernel more than
+ *   occb200_engine_launches_per_frame counts for an unarmed frame.  The kernel casts the T x M rays of the _set_rays bundle
+ *   through the ground truth and, for rays whose ground-truth hit is not `free`, through the volumes the frame produced, and
+ *   adds to counters_dev what occb200_ray_metric_accumulate adds for those volumes (the integer counters bit for bit; the
+ *   `ave` sums up to the order of the fp64 additions).
+ *   sem_gt u8 [200,200,16], flow_gt f32 [200,200,16,2]: DEVICE pointers for the device calls, borrowed until the frame has
+ *   run; HOST pointers for the host calls (pinned for asynchronous copies), uploaded on the slot's copy stream into
+ *   slot-owned staging (5.76 MB per slot, allocated on first use; engine-owned staging for _forward_host), reusable after
+ *   _forward_host returns / after _wait_host.  counters_dev: DEVICE f64 [187] (gt_cnt[17] pred_cnt[17] tp[3][17] ave[3][17]
+ *   ave_count[3][17]), caller-owned, accumulated in place, always a device pointer; complete when the frame is (stream
+ *   synchronised / _wait_host).  origins_host: as for _request_rays, copied into the request.
+ *   Host only, no CUDA call.  T = 0 or NULL origins disarms and returns 0.  Rejected with error 1, leaving no request armed:
+ *   NULL engine, T outside 0..8, NULL sem_gt / flow_gt / counters_dev, a non-finite origin, no ray bundle set, a grid other
+ *   than 200 x 200 x 16.  A frame call that is itself rejected leaves the request armed.
+ * A score request lets the host calls decline their volumes (NULL) exactly as a ray request does, and both may be armed for
+ * the same frame, which then launches both kernels.  The caller's own outputs are the same bytes with and without a request. */
+int occb200_engine_request_score(occb200_engine* e, const uint8_t* sem_gt, const float* flow_gt, const void* origins_host,
+                                 int origin_is_f64, int T, double* counters_dev);
+
 /* Intermediate taps for parity tests (dev f32, valid after a forward; NULL if not produced):
  *   which: 0 = layer output [Nq,C] of layer `layer`; 1 = TSA output (pre-norm, with residual); 2 = SCA output
  *   (pre-norm, with residual); 3 = voxel features [X,Y,Z,out_dim] (converted to fp32 into `dst`);
@@ -240,7 +262,8 @@ int occb200_engine_copy_tap(occb200_engine* e, int which, int layer, float* dst_
 /* Row a2 on its own: reference_points_cam dev f32 [num_cams, Nq, D, 2], bev_mask dev u8 [num_cams, Nq, D]. */
 int occb200_engine_project_pillars(occb200_engine* e, float* ref_cam, uint8_t* mask, void* stream);
 /* number of kernels one forward launches (for the benchmark's gpu_launches claim); with input dtype 3 (camera frames) the
- * attached backbone's kernels are included; a frame that consumed a ray request launched one kernel more */
+ * attached backbone's kernels are included; a frame that consumed a ray request or a score request launched one kernel more
+ * for each */
 int occb200_engine_launches_per_frame(const occb200_engine* e);
 /* Per-kernel-category device timing with CUDA events on the launch stream (benchmark roofline).
  * Categories: 0 pack/prepare, 1 dense GEMM, 2 TSA gather, 3 SCA gather, 4 LayerNorm, 5 bev->voxel, 6 conv3d,
@@ -274,6 +297,14 @@ int occb200_ray_metric_accumulate(const uint8_t* sem_pred, const float* flow_pre
  * of range or a non-finite origin returns 1 before any CUDA call. */
 int occb200_ray_records(const uint8_t* sem_u8, const float* flow, const void* origins_host, int origin_is_f64, int T,
                         const float* rays_dev, int M, int8_t* cls_i8, void* dist_f16, void* flow_f16, void* stream);
+
+/* The score kernel on its own (see occb200_engine_request_score), for tests and timing: all volumes dev, origins_host HOST
+ * [T,3] (f32, or f64 if origin_is_f64), T in 1..8, rays_dev dev f32 [M,3], counters_dev dev f64 [187] accumulated in place.
+ * One launch of ray_score_kernel on `stream`.  A NULL pointer, T or M out of range or a non-finite origin returns 1 before
+ * any CUDA call. */
+int occb200_ray_score(const uint8_t* sem_pred, const float* flow_pred, const uint8_t* sem_gt, const float* flow_gt,
+                      const void* origins_host, int origin_is_f64, int T, const float* rays_dev, int M, double* counters_dev,
+                      void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Building blocks exposed for the module-level API mirror and for kernel tests (dev pointers).

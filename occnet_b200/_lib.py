@@ -50,6 +50,8 @@ SIGNATURES = {
     'occb200_engine_submit_host_video_angle': (_i, [_vp, _i, ctypes.POINTER(_vp), _f64, _i, _vp, _vp, _vp]),
     'occb200_engine_set_rays': (_i, [_vp, _vp, _i]),
     'occb200_engine_request_rays': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
+    'occb200_engine_request_score': (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp]),
+    'occb200_ray_score': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp]),
     'occb200_ray_records': (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp]),
     'occb200_engine_enable_taps': (_i, [_vp, _i]),
     'occb200_engine_copy_tap': (_i, [_vp, _i, _i, _vp, _vp]),

@@ -114,12 +114,23 @@ struct occb200_engine {
         int8_t* cls = nullptr;          // device pointers for the device calls, host pointers for the host calls
         void *dist = nullptr, *flow = nullptr;
     } ray_req;
+    // occb200_engine_request_score: the frame scores itself against this ground truth into the caller's 187 device counters
+    struct ScoreRequest {
+        bool armed = false;
+        RayOrigins org;
+        const uint8_t* sem_gt = nullptr;    // device pointers for the device calls, host pointers for the host calls
+        const float* flow_gt = nullptr;
+        double* counters = nullptr;         // always a device pointer
+    } score_req;
     // what an armed frame needs beyond the caller's outputs: the u8 class volume / the flow when the caller asked for neither,
-    // and for the host calls the device staging of the three record arrays.  One set for the device calls and _forward_host,
-    // one per _submit_host slot (a slot's device->host copy overlaps the next frame's kernels).
+    // and for the host calls the device staging of the three record arrays and of the ground truth.  One set for the device
+    // calls and _forward_host, one per _submit_host slot (a slot's copies overlap the other slot's kernels).
     struct RayStage {
-        DevBuf sem, flow, cls, dist, rflow;
-        void release() { sem.release(); flow.release(); cls.release(); dist.release(); rflow.release(); }
+        DevBuf sem, flow, cls, dist, rflow, gt_sem, gt_flow;
+        void release()
+        {
+            sem.release(); flow.release(); cls.release(); dist.release(); rflow.release(); gt_sem.release(); gt_flow.release();
+        }
     } ray_stage;
     // host-buffer variant
     DevBuf feats_dev[4], occ_i64_dev, flow_dev;
@@ -708,19 +719,38 @@ int copy_ray_records(const occb200_engine* e, const occb200_engine::RayStage& rs
     return 0;
 }
 
+// The host calls upload an armed score request's ground truth into device staging on `copy`, a stream the frame is ordered
+// after, and point the request at the staging.
+int stage_score_request(occb200_engine* e, occb200_engine::RayStage& rs, cudaStream_t copy)
+{
+    occb200_engine::ScoreRequest& sq = e->score_req;
+    if (!sq.armed) return 0;
+    const size_t nvox = (size_t)e->cfg.bev_w * e->cfg.bev_h * e->cfg.pillar_h;
+    if (ensure(rs.gt_sem, nvox) || ensure(rs.gt_flow, nvox * 8)) { sq.armed = false; return 2; }
+    OCC_CUDA(cudaMemcpyAsync(rs.gt_sem.p, sq.sem_gt, nvox, cudaMemcpyHostToDevice, copy));
+    OCC_CUDA(cudaMemcpyAsync(rs.gt_flow.p, sq.flow_gt, nvox * 8, cudaMemcpyHostToDevice, copy));
+    sq.sem_gt = rs.gt_sem.as<uint8_t>(); sq.flow_gt = rs.gt_flow.as<float>();
+    return 0;
+}
+
+// a frame with a request armed may decline its volumes
+bool request_armed(const occb200_engine* e) { return e && (e->ray_req.armed || e->score_req.armed); }
+
 int run_frame_volumes(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed, float* occ_logits,
                       float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video);
 
-// Every frame call ends up here.  An armed ray request (occb200_engine_request_rays) is consumed by this frame: the head also
-// writes the u8 classes and the flow (into `rs` when the caller did not ask for them) and ray_records_kernel follows it on
-// the frame's stream.
+// Every frame call ends up here.  An armed ray request (occb200_engine_request_rays) and an armed score request
+// (occb200_engine_request_score) are consumed by this frame: the head also writes the u8 classes and the flow (into `rs` when
+// the caller did not ask for them) and ray_records_kernel / ray_score_kernel follow it on the frame's stream.
 int run_frame(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed, float* occ_logits,
               float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video = nullptr,
               occb200_engine::RayStage* rs = nullptr)
 {
     const occb200_engine::RayRequest rq = e->ray_req;
     e->ray_req.armed = false;
-    if (rq.armed) {
+    const occb200_engine::ScoreRequest sq = e->score_req;
+    e->score_req.armed = false;
+    if (rq.armed || sq.armed) {
         if (rs == nullptr) rs = &e->ray_stage;
         const size_t nvox = (size_t)e->cfg.bev_w * e->cfg.bev_h * e->cfg.pillar_h;
         if (cls_u8 == nullptr) {
@@ -733,9 +763,17 @@ int run_frame(occb200_engine* e, const float* const* feats, const float* prev_be
         }
     }
     const int rc = run_frame_volumes(e, feats, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, video);
-    if (rc || !rq.armed) return rc;
-    e->launches++;
-    return launch_ray_records(cls_u8, flow, rq.org, e->rays.as<float>(), e->rays_M, rq.cls, rq.dist, rq.flow, st);
+    if (rc) return rc;
+    if (rq.armed) {
+        e->launches++;
+        if (launch_ray_records(cls_u8, flow, rq.org, e->rays.as<float>(), e->rays_M, rq.cls, rq.dist, rq.flow, st)) return 2;
+    }
+    if (sq.armed) {
+        e->launches++;
+        if (launch_ray_score(cls_u8, flow, sq.sem_gt, sq.flow_gt, sq.org, e->rays.as<float>(), e->rays_M, sq.counters, st))
+            return 2;
+    }
+    return 0;
 }
 
 int run_frame_volumes(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed, float* occ_logits,
@@ -1202,8 +1240,8 @@ int occb200_engine_forward_video_angle(occb200_engine* e, const float* const* fe
 int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_host, int64_t* occ_cls_i64_host,
                                 float* flow_host, void* stream)
 {
-    // with a ray request armed the caller may decline either volume (NULL): that 5.12 MB copy is then skipped
-    OCC_CHECK(e && feats_host && ((occ_cls_i64_host && flow_host) || e->ray_req.armed), "null pointer");
+    // with a ray or score request armed the caller may decline either volume (NULL): that 5.12 MB copy is then skipped
+    OCC_CHECK(e && feats_host && ((occ_cls_i64_host && flow_host) || request_armed(e)), "null pointer");
     OCC_CHECK(e->finalized && e->cameras_set, "engine not finalized / cameras not set");
     if (e->feats_bf16 == 3) OCC_CHECK(e->bb != nullptr && feats_host[0] != nullptr, "input dtype 3 needs an attached backbone and a frame buffer");
     const occb200_config& c = e->cfg;
@@ -1222,6 +1260,7 @@ int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_hos
     if (check_frame(e, dev_feats)) return 1;
     occb200_engine::RayRequest rays_host;                          // an armed request: records through the engine's staging
     if (stage_ray_request(e, e->ray_stage, &rays_host)) return 2;
+    if (stage_score_request(e, e->ray_stage, st)) return 2;
     int rc = run_frame(e, dev_feats, nullptr, nullptr, nullptr, e->flow_dev.as<float>(), nullptr,
                        occ_cls_i64_host ? e->occ_i64_dev.as<int64_t>() : nullptr, st);
     if (rc) return rc;
@@ -1237,7 +1276,7 @@ int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_hos
 static int submit_frame(occb200_engine* e, int slot, const float* const* feats_host, int64_t* occ_cls_i64_host, float* flow_host,
                         void* stream, bool video, const int32_t* rot_map_host, const RotGrid* grid, int scene_start)
 {
-    OCC_CHECK(e && feats_host && ((occ_cls_i64_host && flow_host) || e->ray_req.armed), "null pointer");
+    OCC_CHECK(e && feats_host && ((occ_cls_i64_host && flow_host) || request_armed(e)), "null pointer");
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
     OCC_CHECK(e->finalized && e->cameras_set, "engine not finalized / cameras not set");
     if (e->feats_bf16 == 3) OCC_CHECK(e->bb != nullptr && feats_host[0] != nullptr, "input dtype 3 needs an attached backbone and a frame buffer");
@@ -1292,6 +1331,7 @@ static int submit_frame(occb200_engine* e, int slot, const float* const* feats_h
         }
         dev_feats[l] = s.feats[l].as<float>();
     }
+    if (stage_score_request(e, s.ray_stage, e->h2d_stream[0])) return 2;   // ground truth of a score request: h2d_done[0] covers it
     for (int i = 0; i < nsplit; ++i) {                              // compute waits for this frame's features only
         OCC_CUDA(cudaEventRecord(s.h2d_done[i], e->h2d_stream[i]));
         OCC_CUDA(cudaStreamWaitEvent(st, s.h2d_done[i], 0));
@@ -1327,7 +1367,7 @@ int occb200_engine_submit_host_video(occb200_engine* e, int slot, const float* c
                                      int scene_start, int64_t* occ_cls_i64_host, float* flow_host, void* stream)
 {
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
-    OCC_CHECK(feats_host && ((occ_cls_i64_host && flow_host) || (e && e->ray_req.armed)), "null pointer");
+    OCC_CHECK(feats_host && ((occ_cls_i64_host && flow_host) || request_armed(e)), "null pointer");
     OCC_CHECK(e, "null engine");
     return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, true, rot_map_host, nullptr, scene_start);
 }
@@ -1337,7 +1377,7 @@ int occb200_engine_submit_host_video_angle(occb200_engine* e, int slot, const fl
 {
     OCC_CHECK(std::isfinite(angle_deg), "rotation angle must be finite");
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
-    OCC_CHECK(feats_host && ((occ_cls_i64_host && flow_host) || (e && e->ray_req.armed)), "null pointer");
+    OCC_CHECK(feats_host && ((occ_cls_i64_host && flow_host) || request_armed(e)), "null pointer");
     OCC_CHECK(e, "null engine");
     const RotGrid g = rotation_grid(e, angle_deg);
     return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, true, nullptr, &g, scene_start);
@@ -1377,11 +1417,24 @@ int occb200_ray_records(const uint8_t* sem_u8, const float* flow, const void* or
     return launch_ray_records(sem_u8, flow, org, rays_dev, M, cls_i8, dist_f16, flow_f16, (cudaStream_t)stream);
 }
 
+int occb200_ray_score(const uint8_t* sem_pred, const float* flow_pred, const uint8_t* sem_gt, const float* flow_gt,
+                      const void* origins_host, int origin_is_f64, int T, const float* rays_dev, int M, double* counters_dev,
+                      void* stream)
+{
+    OCC_CHECK(T >= 1 && T <= 8, "T (lidar origins) must be in 1..8");
+    OCC_CHECK(M >= 1, "M (rays) must be positive");
+    OCC_CHECK(sem_pred && flow_pred && sem_gt && flow_gt && origins_host && rays_dev && counters_dev, "null pointer");
+    RayOrigins org;
+    if (fill_origins(org, origins_host, origin_is_f64, T)) return 1;
+    return launch_ray_score(sem_pred, flow_pred, sem_gt, flow_gt, org, rays_dev, M, counters_dev, (cudaStream_t)stream);
+}
+
 int occb200_engine_set_rays(occb200_engine* e, const float* rays_host, int M)
 {
     OCC_CHECK(e, "null engine");
     OCC_CHECK(rays_host && M >= 1, "set_rays: null ray bundle or M < 1");
     e->ray_req.armed = false;
+    e->score_req.armed = false;
     if (upload(e->rays, rays_host, (size_t)M * 3)) return 2;
     e->rays_M = M;
     return 0;
@@ -1403,6 +1456,25 @@ int occb200_engine_request_rays(occb200_engine* e, const void* origins_host, int
     rq.armed = true;
     rq.cls = cls_i8; rq.dist = dist_f16; rq.flow = flow_f16;
     e->ray_req = rq;
+    return 0;
+}
+
+int occb200_engine_request_score(occb200_engine* e, const uint8_t* sem_gt, const float* flow_gt, const void* origins_host,
+                                 int origin_is_f64, int T, double* counters_dev)
+{
+    if (e) e->score_req.armed = false;                             // every rejection below leaves the request disarmed
+    OCC_CHECK(T >= 0 && T <= 8, "T (lidar origins) must be in 0..8");
+    OCC_CHECK(e, "null engine");
+    if (T == 0 || origins_host == nullptr) return 0;
+    OCC_CHECK(sem_gt && flow_gt && counters_dev, "null pointer");
+    OCC_CHECK(e->rays.p != nullptr, "request_score: occb200_engine_set_rays() has not been called");
+    OCC_CHECK(e->cfg.bev_w == 200 && e->cfg.bev_h == 200 && e->cfg.pillar_h == 16,
+              "request_score: the ray caster works on the 200 x 200 x 16 grid only");
+    occb200_engine::ScoreRequest sq;
+    if (fill_origins(sq.org, origins_host, origin_is_f64, T)) return 1;
+    sq.armed = true;
+    sq.sem_gt = sem_gt; sq.flow_gt = flow_gt; sq.counters = counters_dev;
+    e->score_req = sq;
     return 0;
 }
 

@@ -126,7 +126,7 @@ int launch_render_forward(const float* sigma, const float* origin, const float* 
 int launch_ray_metric(const uint8_t* sem_pred, const float* flow_pred, const uint8_t* sem_gt, const float* flow_gt,
                       const void* origins, int origin_is_f64, int T, const float* rays, int M, double* counters,
                       float* pcd_pred, float* pcd_gt, cudaStream_t stream);
-// The lidar origins of one frame (ego frame, metres), passed by value to ray_records_kernel: fp32 origins are stored as their
+// The lidar origins of one frame (ego frame, metres), passed by value to ray_records_kernel and ray_score_kernel: fp32 origins are stored as their
 // exact double values, is_f64 selects the arithmetic (torch's type promotion in process_one_sample)
 struct RayOrigins {
     double o[8][3];
@@ -136,5 +136,9 @@ struct RayOrigins {
 // process_one_sample's row order: pcd_cls i8 [T*M], pcd_dist f16 [T*M], pcd_flow f16 [T*M,2]
 int launch_ray_records(const uint8_t* sem, const float* flow, const RayOrigins& org, const float* rays, int M, int8_t* pcd_cls,
                        void* pcd_dist, void* pcd_flow, cudaStream_t stream);
+// launch_ray_metric's counters with the origins by value and no row outputs; the prediction is walked only for rays whose
+// ground-truth hit is not `free`
+int launch_ray_score(const uint8_t* sem_pred, const float* flow_pred, const uint8_t* sem_gt, const float* flow_gt,
+                     const RayOrigins& org, const float* rays, int M, double* counters, cudaStream_t stream);
 
 }  // namespace occ

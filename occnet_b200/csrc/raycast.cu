@@ -8,6 +8,8 @@
 // the predicted and the ground-truth volume in one launch and reduces the 187 counters on device.
 //   ray_records_kernel    <- datasets/nuscenes_occ.py format_results :230-255: the same rays through the predicted volume only,
 //                            written as the challenge file's records (int8 class, fp16 distance, fp16 flow)
+//   ray_score_kernel      <- ray_metric_kernel for a frame the engine has just predicted: origins by value, the ground truth
+//                            walked first and the prediction only for rays that count
 #include <float.h>
 
 #include "common.cuh"
@@ -120,6 +122,45 @@ __device__ __forceinline__ void voxel_ray(const double (&o)[3], int origin_is_f6
     }
 }
 
+// process_one_sample's row of one ray through one volume: {class, distance in metres, flow x, flow y} of the first occupied
+// voxel; the exit voxel for a ray that hits nothing, voxel (0,0,0) and -0.4 m for a ray that never enters the grid
+__device__ __forceinline__ void ray_row(const uint8_t* __restrict__ sem, const float* __restrict__ flow, const float (&og)[3],
+                                        const float (&en)[3], float (&row)[4])
+{
+    double gt_d;
+    const Hit h = dda_first_hit(og[0], og[1], og[2], en[0], en[1], en[2], GX, GY, GZ, gt_d,
+                                [&](int x, int y, int z) { return sem[((int64_t)x * GY + y) * GZ + z] != FREE; });
+    const int64_t vi = ((int64_t)h.x * GY + h.y) * GZ + h.z;
+    row[0] = (float)sem[vi]; row[1] = (h.any ? (float)h.dist : -1.f) * 0.4f; row[2] = flow[vi * 2]; row[3] = flow[vi * 2 + 1];
+}
+
+// calc_metrics' update for one ray (ray_metrics.py:146-189, 218-220) from its predicted and ground-truth rows, into the CTA's
+// shared counters
+__device__ __forceinline__ void score_ray(double* s_cnt, const float (&pred)[4], const float (&gt)[4])
+{
+    const int cp = (int)pred[0], cg = (int)gt[0];
+    if (cg != FREE) {                                                  // ray_metrics.py:218-220
+        if (cg < NCLS) atomicAdd(&s_cnt[cg], 1.0);
+        if (cp < NCLS) atomicAdd(&s_cnt[NCLS + cp], 1.0);
+        if (cg == cp && cg < NCLS) {
+            const float l1 = fabsf(pred[1] - gt[1]);
+            const float fx = gt[2] - pred[2], fy = gt[3] - pred[3];
+            const float err = sqrtf(fx * fx + fy * fy);
+            const float thr[3] = {1.f, 2.f, 4.f};
+#pragma unroll
+            for (int j = 0; j < 3; ++j) {
+                if (l1 < thr[j]) {
+                    atomicAdd(&s_cnt[2 * NCLS + j * NCLS + cg], 1.0);
+                    if (cg < NFLOW) {
+                        atomicAdd(&s_cnt[5 * NCLS + j * NCLS + cg], (double)err);
+                        atomicAdd(&s_cnt[8 * NCLS + j * NCLS + cg], 1.0);
+                    }
+                }
+            }
+        }
+    }
+}
+
 // one thread = one (origin t, ray m); casts through pred and gt, updates the counters
 __global__ void __launch_bounds__(128)
 ray_metric_kernel(const uint8_t* __restrict__ sem_pred, const float* __restrict__ flow_pred,
@@ -140,39 +181,39 @@ ray_metric_kernel(const uint8_t* __restrict__ sem_pred, const float* __restrict_
         float og[3], en[3];
         voxel_ray(o, origin_is_f64, rays + m * 3, og, en);
         float row[2][4];
-#pragma unroll
-        for (int v = 0; v < 2; ++v) {
-            const uint8_t* sem = v ? sem_gt : sem_pred;
-            const float* flow = v ? flow_gt : flow_pred;
-            double gt_d;
-            const Hit h = dda_first_hit(og[0], og[1], og[2], en[0], en[1], en[2], GX, GY, GZ, gt_d,
-                                        [&](int x, int y, int z) { return sem[((int64_t)x * GY + y) * GZ + z] != FREE; });
-            const float dist = (h.any ? (float)h.dist : -1.f) * 0.4f;
-            const int64_t vi = ((int64_t)h.x * GY + h.y) * GZ + h.z;
-            row[v][0] = (float)sem[vi]; row[v][1] = dist; row[v][2] = flow[vi * 2]; row[v][3] = flow[vi * 2 + 1];
-        }
+        ray_row(sem_pred, flow_pred, og, en, row[0]);
+        ray_row(sem_gt, flow_gt, og, en, row[1]);
         if (pcd_pred) *reinterpret_cast<float4*>(pcd_pred + idx * 4) = make_float4(row[0][0], row[0][1], row[0][2], row[0][3]);
         if (pcd_gt) *reinterpret_cast<float4*>(pcd_gt + idx * 4) = make_float4(row[1][0], row[1][1], row[1][2], row[1][3]);
-        const int cp = (int)row[0][0], cg = (int)row[1][0];
-        if (cg != FREE) {                                              // ray_metrics.py:218-220
-            if (cg < NCLS) atomicAdd(&s_cnt[cg], 1.0);
-            if (cp < NCLS) atomicAdd(&s_cnt[NCLS + cp], 1.0);
-            if (cg == cp && cg < NCLS) {
-                const float l1 = fabsf(row[0][1] - row[1][1]);
-                const float fx = row[1][2] - row[0][2], fy = row[1][3] - row[0][3];
-                const float err = sqrtf(fx * fx + fy * fy);
-                const float thr[3] = {1.f, 2.f, 4.f};
-#pragma unroll
-                for (int j = 0; j < 3; ++j) {
-                    if (l1 < thr[j]) {
-                        atomicAdd(&s_cnt[2 * NCLS + j * NCLS + cg], 1.0);
-                        if (cg < NFLOW) {
-                            atomicAdd(&s_cnt[5 * NCLS + j * NCLS + cg], (double)err);
-                            atomicAdd(&s_cnt[8 * NCLS + j * NCLS + cg], 1.0);
-                        }
-                    }
-                }
-            }
+        score_ray(s_cnt, row[0], row[1]);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < NCNT; i += blockDim.x)
+        if (s_cnt[i] != 0.0) atomicAdd(&counters[i], s_cnt[i]);
+}
+
+// ray_metric_kernel's counters for the volumes a frame has just predicted.  The origins arrive by value, so a frame uploads
+// none.  The ground truth is walked first: a ray whose ground-truth row is `free` adds to no counter (ray_metrics.py:218-220),
+// so its walk through the prediction is skipped -- the metric's upward rays, a large share of a real scene.
+__global__ void __launch_bounds__(128)
+ray_score_kernel(const uint8_t* __restrict__ sem_pred, const float* __restrict__ flow_pred,
+                 const uint8_t* __restrict__ sem_gt, const float* __restrict__ flow_gt, const RayOrigins org,
+                 const float* __restrict__ rays, int M, double* __restrict__ counters)
+{
+    __shared__ double s_cnt[NCNT];
+    for (int i = threadIdx.x; i < NCNT; i += blockDim.x) s_cnt[i] = 0.0;
+    __syncthreads();
+    const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx < (int64_t)org.T * M) {
+        const int t = (int)(idx / M), m = (int)(idx % M);
+        const double o[3] = {org.o[t][0], org.o[t][1], org.o[t][2]};
+        float og[3], en[3], gt[4];
+        voxel_ray(o, org.is_f64, rays + m * 3, og, en);
+        ray_row(sem_gt, flow_gt, og, en, gt);
+        if ((int)gt[0] != FREE) {
+            float pred[4];
+            ray_row(sem_pred, flow_pred, og, en, pred);
+            score_ray(s_cnt, pred, gt);
         }
     }
     __syncthreads();
@@ -238,6 +279,16 @@ int launch_ray_metric(const uint8_t* sem_pred, const float* flow_pred, const uin
     ray_metric_kernel<<<ceil_div((int64_t)T * M, 128), 128, 0, stream>>>(sem_pred, flow_pred, sem_gt, flow_gt, origins,
                                                                         origin_is_f64, T, rays, M, counters, pcd_pred,
                                                                         pcd_gt);
+    OCC_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int launch_ray_score(const uint8_t* sem_pred, const float* flow_pred, const uint8_t* sem_gt, const float* flow_gt,
+                     const RayOrigins& org, const float* rays, int M, double* counters, cudaStream_t stream)
+{
+    if (org.T == 0 || M == 0) return 0;
+    ray_score_kernel<<<ceil_div((int64_t)org.T * M, 128), 128, 0, stream>>>(sem_pred, flow_pred, sem_gt, flow_gt, org, rays, M,
+                                                                           counters);
     OCC_CUDA(cudaGetLastError());
     return 0;
 }

@@ -70,6 +70,25 @@ def rotation_index_map(bev_h, bev_w, angle_deg, center):
     return _ROT_CACHE[key]
 
 
+def score_args(score, metric, device, host):
+    """The checks of a frame call's `score=(sem_gt, flow_gt, origins)` / `metric=` -> (sem_gt uint8 (200,200,16), flow_gt
+    fp32 (200,200,16,2), origins numpy (T,3), is_f64).  The ground truth comes back on `device` for the device calls and on
+    the CPU (`host`) for the host calls, converted only when it is not already a contiguous tensor of that kind."""
+    if metric is None:
+        raise ValueError('score= needs metric=, the RayMetric whose counters receive the frame')
+    if metric.counters.device != device:
+        raise ValueError(f'metric lives on {metric.counters.device}, the engine on {device}: its counters must be on the '
+                         f"engine's device")
+    sem_gt, flow_gt, origins = score
+    where = torch.device('cpu') if host else device
+    sem_gt = torch.as_tensor(sem_gt).to(where, torch.uint8).contiguous()
+    flow_gt = torch.as_tensor(flow_gt).to(where, torch.float32).contiguous()
+    if tuple(sem_gt.shape) != (200, 200, 16) or tuple(flow_gt.shape) != (200, 200, 16, 2):
+        raise ValueError(f'score: ground truth {tuple(sem_gt.shape)} / {tuple(flow_gt.shape)}, need (200, 200, 16) / '
+                         f'(200, 200, 16, 2)')
+    return (sem_gt, flow_gt) + ray_origins_host(origins)
+
+
 class OccEngine:
     def __init__(self, cfg, params, precision='fp32', use_tensor_cores=False, device='cuda:0'):
         if not torch.cuda.is_available():
@@ -95,6 +114,7 @@ class OccEngine:
         self.backbone = None
         self.history = False                                          # set_history(True) has allocated the BEV history
         self.num_rays = 0                                             # set_rays() has uploaded the ray bundle
+        self._slot_gt = [None, None]                                  # a submitted frame's ground truth, alive while in flight
 
     def set_input_dtype(self, dtype, channels_last=False):
         """Feature levels are handed over as `dtype` from now on (torch.float32, the reference's, or torch.bfloat16);
@@ -182,6 +202,28 @@ class OccEngine:
             self.lib.occb200_engine_request_rays(self._h, None, 0, 0, None, None, None)
             raise
 
+    @contextlib.contextmanager
+    def _score_request(self, score, metric, slot=None, host=False):
+        """Arm the frame call made inside the block to score itself: `score` = (sem_gt (200,200,16) uint8, flow_gt
+        (200,200,16,2) fp32, origins as for `_ray_request`), CUDA tensors for the device calls and (pinned) CPU tensors for
+        the host calls; the frame's 187 counters are added to `metric.counters` (a `RayMetric` on this device).  None: no
+        request.  A frame call that raises leaves nothing armed."""
+        if score is None:
+            yield
+            return
+        sem_gt, flow_gt, o, is64 = score_args(score, metric, self.device, host)
+        if not self.num_rays:
+            self.set_rays()
+        if slot is not None:
+            self._slot_gt[slot] = (sem_gt, flow_gt)                   # the slot's upload reads them after the call returns
+        _lib.check(self.lib.occb200_engine_request_score(self._h, _lib.ptr(sem_gt), _lib.ptr(flow_gt), _lib.ptr(o), int(is64),
+                                                         o.shape[0], _lib.ptr(metric.counters)))
+        try:
+            yield
+        except BaseException:
+            self.lib.occb200_engine_request_score(self._h, None, None, None, 0, 0, None)
+            raise
+
     def _check_feats(self, feats, cuda):
         """A mismatched tensor would be an out-of-bounds device read in the pack kernel: fail on the host instead."""
         if self.feat_dtype == torch.uint8:
@@ -223,11 +265,15 @@ class OccEngine:
             out['occ_cls_i64'] = torch.empty((X, Y, Z), dtype=torch.int64, device=dev)
         return out
 
-    def forward(self, feats, prev_bev=None, want=('bev_embed', 'occ', 'flow', 'occ_cls'), ray_origins=None):
+    def forward(self, feats, prev_bev=None, want=('bev_embed', 'occ', 'flow', 'occ_cls'), ray_origins=None, score=None,
+                metric=None):
         """feats: 4 CUDA fp32 tensors (num_cams, C, h, w) of one frame, or with `set_input_dtype(torch.uint8)` one CUDA
         uint8 tensor of camera frames (num_cams, src_h, src_w, 3).  Returns a dict of CUDA tensors.  `ray_origins` ((T,3) or
         (1,T,3), T <= 8): the frame also ray-casts its prediction and adds 'ray_cls' int8 (T*M,), 'ray_dist' fp16 (T*M,) and
-        'ray_flow' fp16 (T*M,2), the challenge file's records (`ops.ray_records` of this frame's volumes)."""
+        'ray_flow' fp16 (T*M,2), the challenge file's records (`ops.ray_records` of this frame's volumes).  `score` = (sem_gt
+        (200,200,16) uint8 CUDA, flow_gt (200,200,16,2) fp32 CUDA, origins) with `metric`, a `RayMetric` on this device: the
+        frame also scores itself, adding to `metric.counters` what `metric.add_frame` adds for this frame's 'occ_cls' and
+        'flow'; the counters are complete when the frame is (stream order)."""
         C = self.cfg['embed_dims']
         dev = self.device
         if not self.feat_channels_last and self.feat_dtype != torch.uint8:
@@ -236,7 +282,7 @@ class OccEngine:
         out = self._outputs(want)
         if prev_bev is not None:
             prev_bev = prev_bev.to(device=dev, dtype=torch.float32).reshape(self.Nq, C).contiguous()
-        with torch.cuda.device(dev), self._ray_request(ray_origins) as rec:
+        with torch.cuda.device(dev), self._ray_request(ray_origins) as rec, self._score_request(score, metric):
             _lib.check(self.lib.occb200_engine_forward(
                 self._h, self._feat_ptrs(feats), _lib.ptr(prev_bev), _lib.ptr(out.get('bev_embed')),
                 _lib.ptr(out.get('occ')), _lib.ptr(out.get('flow')), _lib.ptr(out.get('occ_cls')),
@@ -244,15 +290,17 @@ class OccEngine:
         out.update(rec)
         return out
 
-    def forward_host(self, feats_host, occ_out=None, flow_out=None, ray_origins=None, volumes=True):
+    def forward_host(self, feats_host, occ_out=None, flow_out=None, ray_origins=None, volumes=True, score=None, metric=None):
         """feats_host: 4 pinned CPU fp32 tensors (num_cams, C, h, w), or one pinned uint8 tensor of camera frames with
         `set_input_dtype(torch.uint8)` (25.9 MB per 6 x 900 x 1600 frame).  H2D + frame + D2H + sync inside.
         Returns (occ_cls int64 (X,Y,Z) CPU, flow fp32 (X,Y,Z,2) CPU); with `ray_origins` a third element, the frame's ray
-        records as pinned CPU tensors (see `forward`), and with `volumes=False` the two volumes are None and not copied."""
+        records as pinned CPU tensors (see `forward`).  `score` / `metric`: as for `forward`, with the ground truth as CPU
+        tensors; the counters stay on the device.  With `volumes=False` (needs `ray_origins` or `score`) the two volumes are
+        None and not copied."""
         X, Y, Z = self.vox_shape
         if not volumes:
-            if ray_origins is None:
-                raise ValueError('volumes=False needs ray_origins')
+            if ray_origins is None and score is None:
+                raise ValueError('volumes=False needs ray_origins or score')
             occ_out = flow_out = None
         elif occ_out is None or flow_out is None:
             if self._pinned is None:
@@ -261,18 +309,21 @@ class OccEngine:
             occ_out, flow_out = self._pinned
         self._check_feats(feats_host, cuda=False)
         arr = self._feat_ptrs(feats_host)
-        with torch.cuda.device(self.device), self._ray_request(ray_origins, host=True) as rec:
+        with torch.cuda.device(self.device), self._ray_request(ray_origins, host=True) as rec, \
+                self._score_request(score, metric, host=True):
             _lib.check(self.lib.occb200_engine_forward_host(self._h, arr, _lib.ptr(occ_out), _lib.ptr(flow_out),
                                                             _lib.stream_ptr()))
         return (occ_out, flow_out) if ray_origins is None else (occ_out, flow_out, rec)
 
-    def submit_host(self, slot, feats_host, occ_out, flow_out, ray_origins=None, ray_out=None):
+    def submit_host(self, slot, feats_host, occ_out, flow_out, ray_origins=None, ray_out=None, score=None, metric=None):
         """Pipelined host-buffer call (slot 0/1): returns immediately; `wait_host(slot)` completes it.  With `ray_origins` the
         frame's ray records go to the pinned CPU tensors `ray_out` (`ray_buffers(host=True)`), whose first T*M rows are
-        returned as a dict, and `occ_out` / `flow_out` may be None: that volume is then not copied."""
+        returned as a dict.  `score` / `metric`: as for `forward_host`; the counters are complete at `wait_host(slot)`.  With
+        either request `occ_out` / `flow_out` may be None: that volume is then not copied."""
         self._check_feats(feats_host, cuda=False)
         arr = self._feat_ptrs(feats_host)
-        with torch.cuda.device(self.device), self._ray_request(ray_origins, ray_out, host=True) as rec:
+        with torch.cuda.device(self.device), self._ray_request(ray_origins, ray_out, host=True) as rec, \
+                self._score_request(score, metric, slot, host=True):
             _lib.check(self.lib.occb200_engine_submit_host(self._h, slot, arr, _lib.ptr(occ_out), _lib.ptr(flow_out),
                                                            _lib.stream_ptr()))
         return rec
@@ -280,19 +331,22 @@ class OccEngine:
     def wait_host(self, slot):
         _lib.check(self.lib.occb200_engine_wait_host(self._h, slot))
 
-    def stream_host(self, frames_host, ray_origins=None, volumes=True):
+    def stream_host(self, frames_host, ray_origins=None, volumes=True, score=None, metric=None):
         """Generator over an iterable of host frames with two frames in flight; yields (occ int64 CPU, flow CPU)
         views of the slot's pinned output buffers (valid until the slot is reused two frames later).  `ray_origins`: one
         origin set per frame ((T,3) or (1,T,3), T <= 8, T may differ between frames); every frame then yields (occ, flow,
         records) with the frame's ray records {'ray_cls', 'ray_dist', 'ray_flow'} as views of the slot's pinned record
-        buffers (see `forward`).  `volumes=False` (with `ray_origins`): occ and flow are None and never leave the device,
-        786 KB per frame cross the bus at T = 8 instead of 10.24 MB."""
-        if ray_origins is None:
-            if not volumes:
-                raise ValueError('volumes=False needs ray_origins')
-            return self._stream(frames_host, lambda slot, fr, outs, rays: self.submit_host(slot, fr, *outs))
-        return self._stream(zip(frames_host, ray_origins), lambda slot, it, outs, rays: self.submit_host(
-            slot, it[0], *outs, ray_origins=it[1], ray_out=rays), volumes=volumes, rays=True)
+        buffers (see `forward`).  `score`: one (sem_gt, flow_gt, origins) of CPU tensors per frame (None: that frame is not
+        scored); every scored frame adds its counters to `metric` (see `forward_host`), complete when the frame is yielded.
+        `volumes=False` (with `ray_origins` or `score`): occ and flow are None and never leave the device; 786 KB per frame
+        cross the bus at T = 8 with ray records, 5.76 MB of ground truth go up with a score, instead of 10.24 MB."""
+        if not volumes and ray_origins is None and score is None:
+            raise ValueError('volumes=False needs ray_origins or score')
+        rays = ray_origins is not None
+        items = zip(frames_host, ray_origins if rays else itertools.repeat(None),
+                    itertools.repeat(None) if score is None else score)
+        return self._stream(items, lambda slot, it, outs, rb: self.submit_host(
+            slot, it[0], *outs, ray_origins=it[1], ray_out=rb, score=it[2], metric=metric), volumes=volumes, rays=rays)
 
     def _stream(self, items, submit, volumes=True, rays=False):
         """submit(slot, item, (occ, flow) pinned or (None, None), the slot's pinned record buffers or None) -> the frame's
@@ -362,13 +416,13 @@ class OccEngine:
         return torch.from_numpy(m).pin_memory().to(self.device, non_blocking=True)
 
     def forward_video(self, feats, rotation=None, scene_start=False, want=('bev_embed', 'occ', 'flow', 'occ_cls'),
-                      ray_origins=None):
+                      ray_origins=None, score=None, metric=None):
         """One frame of a video (needs `set_history()`): `feats` as for `forward`; the previous BEV is the engine's history,
         rotated by `rotation` (None, an angle in degrees or an index map), unless `scene_start` or this is the first frame
         since `set_history()` (self mode).  Equals `forward(feats, prev_bev=<previous frame's bev_embed>)` with the same
         rotation, bit for bit; the frame's BEV stays in the history whether or not 'bev_embed' is in `want`.  An angle
-        costs no host work: the engine computes the cells of `rotation_index_map(angle)` on the device.  `ray_origins`: as
-        for `forward`."""
+        costs no host work: the engine computes the cells of `rotation_index_map(angle)` on the device.  `ray_origins`,
+        `score` and `metric`: as for `forward`."""
         if not self.feat_channels_last and self.feat_dtype != torch.uint8:
             feats = [f.contiguous() for f in feats]
         self._check_feats(feats, cuda=True)
@@ -377,7 +431,7 @@ class OccEngine:
                 _lib.ptr(out.get('occ_cls')), _lib.ptr(out.get('occ_cls_i64')))
         with torch.cuda.device(self.device):
             rot = None if isinstance(rotation, numbers.Real) else self._rotation_dev(rotation)
-            with self._ray_request(ray_origins) as rec:
+            with self._ray_request(ray_origins) as rec, self._score_request(score, metric):
                 if isinstance(rotation, numbers.Real):
                     _lib.check(self.lib.occb200_engine_forward_video_angle(
                         self._h, self._feat_ptrs(feats), float(rotation), int(bool(scene_start)), *outs, _lib.stream_ptr()))
@@ -388,14 +442,15 @@ class OccEngine:
         return out
 
     def submit_host_video(self, slot, feats_host, occ_out, flow_out, rotation=None, scene_start=False, ray_origins=None,
-                          ray_out=None):
+                          ray_out=None, score=None, metric=None):
         """Pipelined host-buffer video frame (slot 0/1; `submit_host` + the history of `forward_video`): returns
         immediately, `wait_host(slot)` completes it.  An index map is copied before the call returns; an angle needs no
-        map at all.  `ray_origins` / `ray_out` and the returned records: as for `submit_host`."""
+        map at all.  `ray_origins` / `ray_out`, the returned records, `score` and `metric`: as for `submit_host`."""
         self._check_feats(feats_host, cuda=False)
         arr = self._feat_ptrs(feats_host)
         rot = None if isinstance(rotation, numbers.Real) else self._rotation_host(rotation)
-        with torch.cuda.device(self.device), self._ray_request(ray_origins, ray_out, host=True) as rec:
+        with torch.cuda.device(self.device), self._ray_request(ray_origins, ray_out, host=True) as rec, \
+                self._score_request(score, metric, slot, host=True):
             if isinstance(rotation, numbers.Real):
                 _lib.check(self.lib.occb200_engine_submit_host_video_angle(
                     self._h, slot, arr, float(rotation), int(bool(scene_start)), _lib.ptr(occ_out), _lib.ptr(flow_out),
@@ -405,21 +460,23 @@ class OccEngine:
                                                                      _lib.ptr(occ_out), _lib.ptr(flow_out), _lib.stream_ptr()))
         return rec
 
-    def stream_host_video(self, items, volumes=True):
+    def stream_host_video(self, items, volumes=True, score=None, metric=None):
         """`stream_host` for video: items are (feats_host, rotation, scene_start); two frames in flight, yields
         (occ int64 CPU, flow CPU) views of the slot's pinned output buffers, frame by frame.  Items with a fourth element,
         the frame's ray origins, make every frame yield (occ, flow, records) as `stream_host(ray_origins=...)` does;
-        `volumes=False` then keeps the volumes on the device."""
+        `score` (one ground truth per item) and `metric`: as for `stream_host`.  `volumes=False` (with ray origins or
+        `score`) keeps the volumes on the device."""
         items = iter(items)
         first = next(items, None)
         if first is None:
             return iter(())
         rays = len(first) > 3
-        if not volumes and not rays:
-            raise ValueError('volumes=False needs ray origins (a fourth element in every item)')
-        return self._stream(itertools.chain([first], items), lambda slot, it, outs, rb: self.submit_host_video(
-            slot, it[0], *outs, rotation=it[1], scene_start=it[2], ray_origins=it[3] if rays else None, ray_out=rb),
-            volumes=volumes, rays=rays)
+        if not volumes and not rays and score is None:
+            raise ValueError('volumes=False needs ray origins (a fourth element in every item) or score')
+        scored = zip(itertools.chain([first], items), itertools.repeat(None) if score is None else score)
+        return self._stream(scored, lambda slot, p, outs, rb: self.submit_host_video(
+            slot, p[0][0], *outs, rotation=p[0][1], scene_start=p[0][2], ray_origins=p[0][3] if rays else None, ray_out=rb,
+            score=p[1], metric=metric), volumes=volumes, rays=rays)
 
     def enable_taps(self, on=True):
         _lib.check(self.lib.occb200_engine_enable_taps(self._h, int(on)))

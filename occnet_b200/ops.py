@@ -164,6 +164,26 @@ def ray_records(sem_u8, flow, origins):
     return cls, dist, fl
 
 
+def ray_score(sem_pred, flow_pred, sem_gt, flow_gt, origins, counters):
+    """ray_score_kernel on its own: adds to `counters` (187 float64, CUDA) what `RayMetric.add_frame` adds for the same
+    (200,200,16) uint8 / (200,200,16,2) fp32 CUDA volumes and origins ((T,3) or (1,T,3), T <= 8); rays whose ground-truth
+    hit is free skip their walk through the prediction.  The frame engine launches the same kernel for `score=`."""
+    for t, name, dt, shape in ((sem_pred, 'sem_pred', torch.uint8, (200, 200, 16)), (sem_gt, 'sem_gt', torch.uint8, (200, 200, 16)),
+                               (flow_pred, 'flow_pred', torch.float32, (200, 200, 16, 2)),
+                               (flow_gt, 'flow_gt', torch.float32, (200, 200, 16, 2)), (counters, 'counters', torch.float64, (187,))):
+        _require(t, name, dt)
+        if tuple(t.shape) != shape:
+            raise ValueError(f'ray_score: {name} has shape {tuple(t.shape)}, need {shape}')
+    o, is64 = ray_origins_host(origins)
+    rays = lidar_rays(sem_pred.device)
+    lib = _lib.load()
+    with torch.cuda.device(sem_pred.device):
+        _lib.check(lib.occb200_ray_score(_lib.ptr(sem_pred), _lib.ptr(flow_pred), _lib.ptr(sem_gt), _lib.ptr(flow_gt), _lib.ptr(o),
+                                         int(is64), o.shape[0], _lib.ptr(rays), rays.shape[0], _lib.ptr(counters),
+                                         _lib.stream_ptr()))
+    return counters
+
+
 def _no_autograd(name, *tensors):
     """The module-level mirror is an INFERENCE path: these two building blocks have no backward.  Silently cutting the
     graph would leave projection / FFN / norm weights without gradients, so a training-mode call fails loudly instead

@@ -488,16 +488,18 @@ class BEVFormerOccHead(BaseModule):
             self._engine_key = key
         return self._engine
 
-    def forward(self, mlvl_feats, img_metas, prev_bev=None, only_bev=False, test=False, ray_origins=None):
+    def forward(self, mlvl_feats, img_metas, prev_bev=None, only_bev=False, test=False, ray_origins=None, score=None,
+                metric=None):
         """mlvl_feats: 4 x (B, num_cams, C, h, w) CUDA fp32 -> {'bev_embed','occ','flow'} in the reference layouts.
         Frames of a batch are processed independently (== the reference at samples_per_gpu=1, its only shipped mode;
         the reference's batch>1 cross-item quirks, SURVEY a2/a5/a6, are not reproduced).
         `ray_origins` ((1,T,3) or (T,3) lidar origins, batch 1): the frame's engine call also ray-casts the prediction and
-        the result carries 'ray_cls' / 'ray_dist' / 'ray_flow' (`OccEngine.forward`)."""
+        the result carries 'ray_cls' / 'ray_dist' / 'ray_flow' (`OccEngine.forward`).  `score` = (sem_gt, flow_gt, origins)
+        with `metric` (batch 1): the frame's engine call also scores the prediction into `metric.counters`."""
         _need_cuda(mlvl_feats[0], 'BEVFormerOccHead')
         bs = mlvl_feats[0].shape[0]
-        if ray_origins is not None and (bs != 1 or only_bev):
-            raise ValueError('ray_origins takes one frame (batch 1) that runs the heads')
+        if (ray_origins is not None or score is not None) and (bs != 1 or only_bev):
+            raise ValueError('ray_origins / score take one frame (batch 1) that runs the heads')
         eng = self._get_engine(mlvl_feats[0].device, [tuple(f.shape[-2:]) for f in mlvl_feats])
         rot_maps = None
         if prev_bev is not None:
@@ -518,7 +520,7 @@ class BEVFormerOccHead(BaseModule):
             eng.set_prev_rotation(None if rot_maps is None else rot_maps[b])
             fb = self._engine_feats(eng, [f[b] for f in mlvl_feats])
             out = eng.forward(fb, prev_bev=None if prev_bev is None else prev_bev[b],
-                              want=('bev_embed',) if only_bev else want, ray_origins=ray_origins)
+                              want=('bev_embed',) if only_bev else want, ray_origins=ray_origins, score=score, metric=metric)
             rays = {k: v for k, v in out.items() if k.startswith('ray_')}
             bevs.append(out['bev_embed'])
             if not only_bev:
@@ -546,12 +548,12 @@ class BEVFormerOccHead(BaseModule):
             fb = [f.float() for f in fb]
         return fb
 
-    def forward_video(self, mlvl_feats, img_metas, scene_start, ray_origins=None):
+    def forward_video(self, mlvl_feats, img_metas, scene_start, ray_origins=None, score=None, metric=None):
         """One video frame of batch 1 with the BEV history kept inside the engine (`OccEngine.forward_video`): the previous
         frame's BEV never leaves the engine, and the rotation by can_bus[-1] degrees (none when the transformer's
         rotate_prev_bev is False) is computed on the device.  `scene_start` (or the first frame after the engine is built)
         runs without a previous BEV.  Bit-identical to `forward(mlvl_feats, img_metas, prev_bev=<previous frame's
-        bev_embed>, test=True)`; the result's 'bev_embed' is None.  `ray_origins`: as for `forward`."""
+        bev_embed>, test=True)`; the result's 'bev_embed' is None.  `ray_origins`, `score` and `metric`: as for `forward`."""
         _need_cuda(mlvl_feats[0], 'BEVFormerOccHead')
         if mlvl_feats[0].shape[0] != 1:
             raise ValueError(f'forward_video takes batch 1, got {mlvl_feats[0].shape[0]}')
@@ -562,7 +564,7 @@ class BEVFormerOccHead(BaseModule):
         rotation = float(img_metas[0]['can_bus'][-1]) if self.transformer.rotate_prev_bev else None
         want = ('occ', 'flow', 'occ_cls_i64') if self.test_logits else ('flow', 'occ_cls_i64')
         out = eng.forward_video(self._engine_feats(eng, [f[0] for f in mlvl_feats]), rotation=rotation,
-                                scene_start=scene_start, want=want, ray_origins=ray_origins)
+                                scene_start=scene_start, want=want, ray_origins=ray_origins, score=score, metric=metric)
         return dict({'bev_embed': None, 'occ': out['occ'][None] if 'occ' in out else None, 'flow': out['flow'][None],
                      'occ_cls': out['occ_cls_i64'][None]}, **{k: v for k, v in out.items() if k.startswith('ray_')})
 
@@ -648,7 +650,7 @@ class BEVFormerOcc(BaseModule):
 
     def __init__(self, pts_bbox_head=None, img_backbone=None, img_neck=None, use_grid_mask=False, video_test_mode=False,
                  train_cfg=None, test_cfg=None, pretrained=None, feature_extractor=None, native_backbone=True,
-                 backbone_precision=None, temporal_test=False, engine_history=False, ray_only=False,
+                 backbone_precision=None, temporal_test=False, engine_history=False, ray_only=False, score_only=False,
                  frame_norm_cfg=dict(mean=[103.530, 116.280, 123.675], std=[1.0, 1.0, 1.0], to_rgb=False),
                  frame_pad=dict(size_divisor=32), **kwargs):
         super().__init__()
@@ -690,6 +692,9 @@ class BEVFormerOcc(BaseModule):
         # ray_only=True: `forward_test(lidar_origins=...)` returns the frame's ray records only; 'occ_results' and
         # 'flow_results' are None and the 10.24 MB of volumes stay on the device
         self.ray_only = ray_only
+        # score_only=True: `forward_test(gt_semantics=..., gt_flow=..., lidar_origins=..., ray_metric=...)` only scores the
+        # frame into `ray_metric`; 'occ_results' and 'flow_results' are None and nothing is copied to the host
+        self.score_only = score_only
         self.prev_frame_info = {'prev_bev': None, 'scene_token': None, 'prev_pos': 0, 'prev_angle': 0}
 
     def _get_backbone_engine(self, device, shape):
@@ -802,24 +807,28 @@ class BEVFormerOcc(BaseModule):
         """the head's ray records (CUDA) under the challenge file's names"""
         return {'pcd_cls': outs['ray_cls'], 'pcd_dist': outs['ray_dist'], 'pcd_flow': outs['ray_flow']}
 
-    def simple_test_pts(self, x, img_metas, prev_bev=None, rescale=False, ray_origins=None):
-        """-> (bev_embed, occ, flow), and with `ray_origins` a fourth element: the frame's ray records (CUDA tensors)"""
-        outs = self.pts_bbox_head(x, img_metas, prev_bev=prev_bev, test=True, ray_origins=ray_origins)
+    def simple_test_pts(self, x, img_metas, prev_bev=None, rescale=False, ray_origins=None, score=None, metric=None):
+        """-> (bev_embed, occ, flow), and with `ray_origins` a fourth element: the frame's ray records (CUDA tensors);
+        `score` / `metric`: the frame scores itself (`BEVFormerOccHead.forward`)"""
+        outs = self.pts_bbox_head(x, img_metas, prev_bev=prev_bev, test=True, ray_origins=ray_origins, score=score,
+                                  metric=metric)
         occ, flow = self.pts_bbox_head.get_occ(outs, img_metas, rescale=rescale)
         if ray_origins is not None:
             return outs['bev_embed'], occ, flow, self._ray_results(outs)
         return outs['bev_embed'], occ, flow
 
-    def simple_test(self, img_metas, img=None, img_feats=None, prev_bev=None, rescale=False, ray_origins=None, **kwargs):
+    def simple_test(self, img_metas, img=None, img_feats=None, prev_bev=None, rescale=False, ray_origins=None, score=None,
+                    metric=None, **kwargs):
         if img_feats is None and isinstance(img, torch.Tensor) and img.dtype == torch.uint8:
             img_metas = self.frame_metas(img_metas, img)                       # before any launch: shape errors are free
             return self.simple_test_pts(self.extract_frame_feat(img), img_metas, prev_bev, rescale=rescale,
-                                        ray_origins=ray_origins)
+                                        ray_origins=ray_origins, score=score, metric=metric)
         feats = img_feats if img_feats is not None else self.extract_feat(img, img_metas)
-        return self.simple_test_pts(feats, img_metas, prev_bev, rescale=rescale, ray_origins=ray_origins)
+        return self.simple_test_pts(feats, img_metas, prev_bev, rescale=rescale, ray_origins=ray_origins, score=score,
+                                    metric=metric)
 
     def simple_test_video(self, img_metas, img=None, img_feats=None, scene_start=False, rescale=False, ray_origins=None,
-                          **kwargs):
+                          score=None, metric=None, **kwargs):
         """`simple_test` of one batch-1 video frame on the head engine's BEV history (`BEVFormerOccHead.forward_video`)
         -> (occ, flow), and with `ray_origins` a third element: the frame's ray records (CUDA tensors)"""
         if img_feats is None and isinstance(img, torch.Tensor) and img.dtype == torch.uint8:
@@ -827,7 +836,8 @@ class BEVFormerOcc(BaseModule):
             feats = self.extract_frame_feat(img)
         else:
             feats = img_feats if img_feats is not None else self.extract_feat(img, img_metas)
-        outs = self.pts_bbox_head.forward_video(feats, img_metas, scene_start, ray_origins=ray_origins)
+        outs = self.pts_bbox_head.forward_video(feats, img_metas, scene_start, ray_origins=ray_origins, score=score,
+                                                metric=metric)
         occ, flow = self.pts_bbox_head.get_occ(outs, img_metas, rescale=rescale)
         return (occ, flow) if ray_origins is None else (occ, flow, self._ray_results(outs))
 
@@ -838,23 +848,38 @@ class BEVFormerOcc(BaseModule):
         return 1 if img is None or img.dim() == 4 else img.shape[0]
 
     def _results(self, occ, flow, rays):
-        """the result dict of `forward_test`: CPU tensors; `rays` (None without lidar_origins) adds 'ray_results'"""
-        if rays is None:
-            return {'occ_results': occ.cpu(), 'flow_results': flow.cpu()}
-        res = {'occ_results': None, 'flow_results': None} if self.ray_only else \
+        """the result dict of `forward_test`: CPU tensors, no volumes for a `ray_only` / `score_only` detector; `rays` (None when the frame
+        made no ray records) adds 'ray_results'"""
+        res = {'occ_results': None, 'flow_results': None} if self.score_only or self.ray_only else \
             {'occ_results': occ.cpu(), 'flow_results': flow.cpu()}
-        res['ray_results'] = {k: v.cpu() for k, v in rays.items()}
+        if rays is not None:
+            res['ray_results'] = {k: v.cpu() for k, v in rays.items()}
         return res
 
-    def forward_test(self, img_metas, img=None, img_feats=None, lidar_origins=None, **kwargs):
+    def forward_test(self, img_metas, img=None, img_feats=None, lidar_origins=None, gt_semantics=None, gt_flow=None,
+                     ray_metric=None, **kwargs):
         """`lidar_origins` ((1,T,3) or (T,3), T <= 8, batch 1): the frame's engine call also ray-casts its prediction and
         the result carries 'ray_results' {'pcd_cls' int8, 'pcd_dist' fp16, 'pcd_flow' fp16}, the records
-        `datasets.submission.format_results` writes as they are.  Without it the result is {'occ_results', 'flow_results'}."""
+        `datasets.submission.format_results` writes as they are.  Without it the result is {'occ_results', 'flow_results'}.
+        `gt_semantics` ((200,200,16) or (1,200,200,16)), `gt_flow` (.., 2) and `ray_metric` (a `RayMetric` on the frame's
+        device) together with `lidar_origins` (batch 1): the frame's engine call scores its prediction against that ground
+        truth into `ray_metric.counters` instead, what `evaluate_miou` + `ray_based_miou` do with the volumes on the host;
+        the result carries ray records only if the detector is `ray_only`."""
         metas = img_metas[0] if isinstance(img_metas[0], (list, tuple)) else img_metas
         if isinstance(img, (list, tuple)):
             img = img[0]
         if self.ray_only and lidar_origins is None:
             raise ValueError('ray_only=True needs lidar_origins for every frame')
+        score = None
+        if gt_semantics is not None or gt_flow is not None or ray_metric is not None:
+            if gt_semantics is None or gt_flow is None or ray_metric is None or lidar_origins is None:
+                raise ValueError('scoring a frame needs gt_semantics, gt_flow, lidar_origins and ray_metric together')
+            score = (torch.as_tensor(gt_semantics).reshape(200, 200, 16), torch.as_tensor(gt_flow).reshape(200, 200, 16, 2),
+                     lidar_origins)
+            if not self.ray_only:
+                lidar_origins = None
+        elif self.score_only:
+            raise ValueError('score_only=True needs gt_semantics, gt_flow, lidar_origins and ray_metric for every frame')
         prev_bev = None                                                                             # reference: prev_bev=None
         video = self.temporal_test and self.video_test_mode
         if video:
@@ -867,11 +892,12 @@ class BEVFormerOcc(BaseModule):
             prev_bev = info['prev_bev']
             if self.engine_history and self._batch_size(img, img_feats) == 1:
                 occ, flow, *rays = self.simple_test_video(metas, img, img_feats=img_feats, ray_origins=lidar_origins,
+                                                          score=score, metric=ray_metric,
                                                           scene_start=new_scene or not self._engine_history_valid, **kwargs)
                 self._engine_history_valid = True
                 return self._results(occ, flow, rays[0] if rays else None)
         new_prev_bev, occ, flow, *rays = self.simple_test(metas, img, img_feats=img_feats, prev_bev=prev_bev,
-                                                          ray_origins=lidar_origins, **kwargs)
+                                                          ray_origins=lidar_origins, score=score, metric=ray_metric, **kwargs)
         if video:
             self.prev_frame_info['prev_bev'] = new_prev_bev                                         # (B, C, H, W), stays on the device
             self._engine_history_valid = False
