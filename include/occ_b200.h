@@ -348,6 +348,23 @@ int occb200_gemm_tc_split3(const void* S, int Ks, const void* W3, const float* b
                            int act, void* stream);
 int occb200_split_bf16(const float* a, int Ka, const float* b, int Kb, int64_t rows, void* S, void* stream);
 
+/* The fused deformable-attention gathers of the frame engine, for operator tests: one launch of the kernel the engine launches
+ * for the same types.  value_bf16 / qproj_f16 select the storage of the values / outputs (fp32 or bf16) and of the sampling
+ * projection (fp32 or fp16); accepted: fp32 / fp32, bf16 / fp32, bf16 / fp16.  All arrays are dense row-major device arrays
+ * unless marked HOST.  A NULL required pointer, an unsupported type combination or size returns 1 before any CUDA call.
+ *   tsa_gather: v_prev, v_cur [Nq,256] (queue 0 / 1), qproj [Nq,192] = [offsets (head, queue, point, xy) | logits (head,
+ *     queue, point)], out [Nq,256] = the mean over the two queues; Nq = bev_h * bev_w, bev_h, bev_w >= 2.
+ *   sca_gather: value [num_cams, Nv, 256] (levels in order, Nv = sum h_l * w_l), qproj [Nq,768] = [offsets (head, level, point,
+ *     xy) | logits (head, level * point)], out [Nq,256] = the sum over the cameras that see the pillar / max(1, their count),
+ *     hits [Nq] (may be NULL) = that count.  cam_mat_host [num_cams,16], zs_host [D], pc_range, the padded image size and the
+ *     BEV grid as for occb200_engine_set_cameras; level_hw_host = h0 w0 .. h3 w3.  num_cams in 1..8, D in {1,2,4,8}, every
+ *     level at least 2x2, positive image and BEV sizes. */
+int occb200_tsa_gather(const void* v_prev, const void* v_cur, int value_bf16, const void* qproj, int qproj_f16, int bev_h,
+                       int bev_w, void* out, void* stream);
+int occb200_sca_gather(const void* value, int value_bf16, const void* qproj, int qproj_f16, const float* cam_mat_host,
+                       const float* zs_host, int num_cams, int D, const float pc_range[6], int img_h, int img_w, int bev_h,
+                       int bev_w, const int level_hw_host[8], void* out, uint8_t* hits, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Image backbone + neck (SURVEY 8f rank 1, the step immediately BEFORE the hot path); parity vs its oracle:
  * tests/test_backbone_gpu.py (fp32 1e-3 relative to the feature magnitude, bf16 bars stated there).

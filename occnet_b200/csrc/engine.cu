@@ -199,6 +199,40 @@ const std::vector<float>* find(const occb200_engine* e, const std::string& k, si
     return &it->second;
 }
 
+// ---- geometry of the fused spatial cross-attention gather: built here for the engine (creation, set_cameras) and for the
+// occb200_sca_gather test entry alike, so that the operator tests launch the kernels on exactly what the engine builds
+// the four value-map levels of every camera, rows [start, start + h*w) of the [Nv, 256] map; *Nv = the total
+LevelGeom make_level_geom(const int* level_h, const int* level_w, int* Nv)
+{
+    LevelGeom lg{};
+    lg.num_levels = 4;
+    int start = 0;
+    for (int l = 0; l < 4; ++l) {
+        lg.h[l] = level_h[l]; lg.w[l] = level_w[l]; lg.start[l] = start;
+        start += level_h[l] * level_w[l];
+    }
+    *Nv = start;
+    return lg;
+}
+
+// cam_mat [num_cams,16] = lidar2img[c] @ ego2lidar, zs [D] normalised pillar heights, pc_range, padded image size, BEV grid
+ScaParams make_sca_params(const float* cam_mat, const float* zs, int num_cams, int D, const float* pc_range, int img_h,
+                          int img_w, int bev_h, int bev_w)
+{
+    ScaParams sp;
+    memset(&sp, 0, sizeof(sp));
+    for (int i = 0; i < num_cams; ++i)
+        for (int k = 0; k < 16; ++k) sp.cam_mat[i][k] = cam_mat[i * 16 + k];
+    for (int i = 0; i < D; ++i) sp.zs[i] = zs[i];
+    for (int i = 0; i < 3; ++i) {
+        sp.pc_scale[i] = (float)((double)pc_range[3 + i] - (double)pc_range[i]);
+        sp.pc_min[i] = pc_range[i];
+    }
+    sp.img_w = (float)img_w; sp.img_h = (float)img_h;
+    sp.num_cams = num_cams; sp.D = D; sp.bev_h = bev_h; sp.bev_w = bev_w;
+    return sp;
+}
+
 #define GETP(var, key, n)                            \
     const std::vector<float>* var = find(e, key, n); \
     if (!var) return 3;
@@ -866,13 +900,7 @@ int occb200_engine_create(const occb200_config* cfg, occb200_engine** out)
     auto* e = new occb200_engine();
     e->cfg = *cfg;
     e->Nq = cfg->bev_h * cfg->bev_w;
-    e->lg.num_levels = 4;
-    int start = 0;
-    for (int l = 0; l < 4; ++l) {
-        e->lg.h[l] = cfg->level_h[l]; e->lg.w[l] = cfg->level_w[l]; e->lg.start[l] = start;
-        start += cfg->level_h[l] * cfg->level_w[l];
-    }
-    e->Nv = start;
+    e->lg = make_level_geom(cfg->level_h, cfg->level_w, &e->Nv);
     e->layers.resize(cfg->num_layers);
     *out = e;
     return 0;
@@ -1173,16 +1201,7 @@ int occb200_engine_set_cameras(occb200_engine* e, const float* cam_mat, const fl
 {
     OCC_CHECK(e && cam_mat && zs, "null pointer");
     const occb200_config& c = e->cfg;
-    memset(&e->sp, 0, sizeof(e->sp));
-    for (int i = 0; i < c.num_cams; ++i)
-        for (int k = 0; k < 16; ++k) e->sp.cam_mat[i][k] = cam_mat[i * 16 + k];
-    for (int i = 0; i < c.num_points_in_pillar; ++i) e->sp.zs[i] = zs[i];
-    for (int i = 0; i < 3; ++i) {
-        e->sp.pc_scale[i] = (float)((double)c.pc_range[3 + i] - (double)c.pc_range[i]);
-        e->sp.pc_min[i] = c.pc_range[i];
-    }
-    e->sp.img_w = (float)img_w; e->sp.img_h = (float)img_h;
-    e->sp.num_cams = c.num_cams; e->sp.D = c.num_points_in_pillar; e->sp.bev_h = c.bev_h; e->sp.bev_w = c.bev_w;
+    e->sp = make_sca_params(cam_mat, zs, c.num_cams, c.num_points_in_pillar, c.pc_range, img_h, img_w, c.bev_h, c.bev_w);
     e->cameras_set = true;
     return 0;
 }
@@ -1718,5 +1737,52 @@ int occb200_split_bf16(const float* a, int Ka, const float* b, int Kb, int64_t r
     OCC_CHECK(rows >= 0 && Ka > 0 && Kb >= 0 && Ka % 8 == 0 && Kb % 8 == 0, "Ka, Kb must be multiples of 8");
     return launch_split_bf16(a, Ka, b, Kb, rows, reinterpret_cast<bf16*>(S), (cudaStream_t)stream);
 }
+
+// ---- the fused attention gathers for kernel tests: argument checks only, every rejection before the first CUDA call, then the
+// launcher the frame engine calls.  Value / projection types: the three combinations the engine launches.
+#define OCC_CHECK_GATHER_TYPES(value_bf16, qproj_f16)                                                                   \
+    OCC_CHECK((value_bf16 == 0 || value_bf16 == 1) && (qproj_f16 == 0 || qproj_f16 == 1) && (value_bf16 || !qproj_f16), \
+              "value / projection types must be fp32 / fp32, bf16 / fp32 or bf16 / fp16")
+
+int occb200_tsa_gather(const void* v_prev, const void* v_cur, int value_bf16, const void* qproj, int qproj_f16, int bev_h,
+                       int bev_w, void* out, void* stream)
+{
+    OCC_CHECK(v_prev && v_cur && qproj && out, "null pointer");
+    OCC_CHECK_GATHER_TYPES(value_bf16, qproj_f16);
+    OCC_CHECK(bev_h >= 2 && bev_w >= 2, "the BEV grid must be at least 2x2");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (value_bf16)
+        return launch_tsa_fused<bf16>(reinterpret_cast<const bf16*>(v_prev), reinterpret_cast<const bf16*>(v_cur), qproj,
+                                      qproj_f16 != 0, bev_h, bev_w, reinterpret_cast<bf16*>(out), st);
+    return launch_tsa_fused<float>(reinterpret_cast<const float*>(v_prev), reinterpret_cast<const float*>(v_cur), qproj, false,
+                                   bev_h, bev_w, reinterpret_cast<float*>(out), st);
+}
+
+int occb200_sca_gather(const void* value, int value_bf16, const void* qproj, int qproj_f16, const float* cam_mat_host,
+                       const float* zs_host, int num_cams, int D, const float pc_range[6], int img_h, int img_w, int bev_h,
+                       int bev_w, const int level_hw_host[8], void* out, uint8_t* hits, void* stream)
+{
+    OCC_CHECK(value && qproj && cam_mat_host && zs_host && pc_range && level_hw_host && out, "null pointer");
+    OCC_CHECK_GATHER_TYPES(value_bf16, qproj_f16);
+    OCC_CHECK(num_cams >= 1 && num_cams <= 8, "num_cams must be in [1,8]");
+    OCC_CHECK(D == 1 || D == 2 || D == 4 || D == 8, "D (num_points_in_pillar) must be 1, 2, 4 or 8");
+    OCC_CHECK(img_h > 0 && img_w > 0, "the image size must be positive");
+    OCC_CHECK(bev_h > 0 && bev_w > 0, "the BEV size must be positive");
+    int level_h[4], level_w[4];
+    for (int l = 0; l < 4; ++l) {
+        level_h[l] = level_hw_host[2 * l]; level_w[l] = level_hw_host[2 * l + 1];
+        OCC_CHECK(level_h[l] >= 2 && level_w[l] >= 2, "every level must be at least 2x2");
+    }
+    int Nv = 0;
+    const LevelGeom lg = make_level_geom(level_h, level_w, &Nv);
+    const ScaParams sp = make_sca_params(cam_mat_host, zs_host, num_cams, D, pc_range, img_h, img_w, bev_h, bev_w);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (value_bf16)
+        return launch_sca_fused<bf16>(reinterpret_cast<const bf16*>(value), qproj, qproj_f16 != 0, sp, lg, Nv,
+                                      reinterpret_cast<bf16*>(out), hits, st);
+    return launch_sca_fused<float>(reinterpret_cast<const float*>(value), qproj, false, sp, lg, Nv, reinterpret_cast<float*>(out),
+                                   hits, st);
+}
+#undef OCC_CHECK_GATHER_TYPES
 
 }  // extern "C"
