@@ -78,7 +78,8 @@ typedef struct occb200_config {
     int use_cams_embeds;           /* TransformerOcc(use_cams_embeds=...), transformer_occ.py:214-215; 0 = the
                                       camera embedding is NOT added to the packed features                    */
     int rotate_center[2];          /* TransformerOcc(rotate_center=[100,100]), transformer_occ.py:200: centre
-                                      (x, y) of the prev_bev rotation done by occb200_engine_forward_prev      */
+                                      (x, y) of the prev_bev rotation by angle (_set_prev_rotation_angle, the
+                                      video _angle calls)                                                     */
 } occb200_config;
 
 int occb200_engine_create(const occb200_config* cfg, occb200_engine** out);
@@ -154,7 +155,7 @@ int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_hos
                                 float* flow_host, void* stream);
 
 /* Pipelined form of the same call for streams of frames: _submit_host enqueues the host->device copy of the
- * frame's features (copy streams; levels above 32 MB are split over OCC_H2D_SPLIT = 1..4 of them, default 2), the
+ * frame's features (copy streams; levels above 32 MB are split over two of them), the
  * frame (caller's stream, after those copies) and the device->host copy of the
  * results (second copy stream) for `slot` in {0,1} and returns; _wait_host blocks until the slot's results are in
  * the host buffers.  With two slots in flight the copies of frame i+1 / i-1 overlap the compute of frame i.

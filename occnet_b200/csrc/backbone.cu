@@ -26,22 +26,8 @@ using namespace occ;
 
 namespace {
 
-struct Buf {
-    void* p = nullptr;
-    size_t bytes = 0;
-    int alloc(size_t n) {
-        release();
-        if (n == 0) return 0;
-        OCC_CUDA(cudaMalloc(&p, n));
-        bytes = n;
-        return 0;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
-    template <typename U> U* as() const { return reinterpret_cast<U*>(p); }
-};
-
 struct ConvW {                       // BN-folded, tap-major weights: w[co][(ky*KW + kx)*Cin + c], K zero-padded to kpad
-    Buf w, wh, b;
+    DevBuf w, wh, b;
     int cout = 0, cin = 0, kh = 1, kw = 1, stride = 1, pad = 0, kpad = 0;
 };
 
@@ -63,7 +49,7 @@ struct occb200_backbone {
     FrameNorm fn{};
     int launches = 0;                // kernels the last forward launched
     // workspace
-    Buf img_nhwc, col, ping[2], t1, t2, t3, idn, stage_out[3], lat[3], fo[4];
+    DevBuf img_nhwc, col, ping[2], t1, t2, t3, idn, stage_out[3], lat[3], fo[4];
     size_t elt() const { return precision ? 2 : 4; }
 };
 
@@ -287,20 +273,7 @@ occb200_backbone* occb200_backbone_create(int num_images, int img_h, int img_w, 
     return e;
 }
 
-void occb200_backbone_destroy(occb200_backbone* e)
-{
-    if (!e) return;
-    auto rel = [](ConvW& c) { c.w.release(); c.wh.release(); c.b.release(); };
-    rel(e->stem);
-    for (auto& st : e->blocks) for (auto& b : st) { rel(b.c1); rel(b.c2); rel(b.c3); rel(b.down); }
-    for (auto& c : e->lateral) rel(c);
-    for (auto& c : e->fpnc) rel(c);
-    Buf* all[] = {&e->img_nhwc, &e->col, &e->ping[0], &e->ping[1], &e->t1, &e->t2, &e->t3, &e->idn, &e->stage_out[0],
-                  &e->stage_out[1], &e->stage_out[2], &e->lat[0], &e->lat[1], &e->lat[2], &e->fo[0], &e->fo[1], &e->fo[2],
-                  &e->fo[3]};
-    for (Buf* b : all) b->release();
-    delete e;
-}
+void occb200_backbone_destroy(occb200_backbone* e) { delete e; }
 
 int occb200_backbone_load_param(occb200_backbone* e, const char* key, const float* data, int64_t numel)
 {

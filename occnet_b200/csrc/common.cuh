@@ -29,6 +29,35 @@ void set_last_error(const std::string& msg);
         }                                                                                 \
     } while (0)
 
+// ---- one device allocation, freed by its destructor (movable, not copyable)
+struct DevBuf {
+    void* p = nullptr;
+    size_t bytes = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept
+    {
+        if (this != &o) { release(); p = o.p; bytes = o.bytes; o.p = nullptr; o.bytes = 0; }
+        return *this;
+    }
+    ~DevBuf() { release(); }
+    int alloc(size_t n)
+    {
+        release();
+        if (n == 0) return 0;
+        OCC_CUDA(cudaMalloc(&p, n));
+        bytes = n;
+        return 0;
+    }
+    void release() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
+    template <typename U> U* as() const { return reinterpret_cast<U*>(p); }
+};
+
+// allocate `b` to exactly n bytes unless it already has that size (contents are kept then)
+inline int ensure(DevBuf& b, size_t n) { return b.bytes != n && b.alloc(n) ? 2 : 0; }
+
 typedef __nv_bfloat16 bf16;
 
 // ---- storage-type helpers: T in {float, bf16}; arithmetic is always fp32

@@ -28,20 +28,6 @@ void set_last_error(const std::string& msg) { g_last_error = msg; }
 
 namespace {
 
-struct DevBuf {
-    void* p = nullptr;
-    size_t bytes = 0;
-    int alloc(size_t n) {
-        release();
-        if (n == 0) return 0;
-        OCC_CUDA(cudaMalloc(&p, n));
-        bytes = n;
-        return 0;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
-    template <typename U> U* as() const { return reinterpret_cast<U*>(p); }
-};
-
 struct LayerW {
     DevBuf tsa_v_w, tsa_v_b, tsa_q_w, tsa_q_b, tsa_o_w, tsa_o_b;
     DevBuf sca_q_w, sca_q_b, sca_v_w, sca_v_b, sca_o_w, sca_o_b;
@@ -52,6 +38,58 @@ struct LayerW {
     // self mode (prev_bev = None): W1 q + W2 (q + pos) + b == (W1 + W2) q + [W2 pos + b]; the bracket depends on parameters
     // only -> an fp32 [Nq,192] constant per layer, added by the GEMM epilogue (K = 256, weight block resident, A read once)
     DevBuf tsa_q_wh_fold, tsa_q_const, tsa_q_const_t32;   // (_t32: the constant in the T32 block layout, read by the GEMM epilogue)
+};
+
+// An armed ray request (occb200_engine_request_rays) and score request (occb200_engine_request_score)
+struct RayRequest {
+    bool armed = false;
+    RayOrigins org;
+    int8_t* cls = nullptr;              // device pointers for the device calls, host pointers for the host calls
+    void *dist = nullptr, *flow = nullptr;
+};
+struct ScoreRequest {
+    bool armed = false;
+    RayOrigins org;
+    const uint8_t* sem_gt = nullptr;    // device pointers for the device calls, host pointers for the host calls
+    const float* flow_gt = nullptr;
+    double* counters = nullptr;         // always a device pointer
+};
+// what one frame consumes
+struct Requests {
+    RayRequest rays;
+    ScoreRequest score;
+};
+
+// The device buffers of a frame: for the host calls the uploaded inputs (four feature levels, or the camera frames in
+// feats[0]) and the i64 classes and flow the copies back read; for an armed frame the u8 classes and the flow when the caller
+// asked for neither, and for the host calls the staging of a ray request's records and of a score request's ground truth.
+// One set for the device calls and _forward_host, one per _submit_host slot (a slot's copies overlap the other slot's kernels).
+struct FrameBufs {
+    DevBuf feats[4], occ, flow, sem, rec_cls, rec_dist, rec_flow, gt_sem, gt_flow;
+};
+
+// _submit_host uploads an input buffer above 32 MB in two pieces on two copy streams: when the split was tuned, one
+// cudaMemcpyAsync stream reached 46 GB/s of the PCIe link and two reached 50 GB/s.
+constexpr int kH2DSplit = 2;
+
+// A frame's outputs on the device (any may be NULL)
+struct FrameOut {
+    float* bev_embed = nullptr;
+    float* occ_logits = nullptr;
+    float* flow = nullptr;
+    uint8_t* cls_u8 = nullptr;
+    int64_t* cls_i64 = nullptr;
+};
+
+// Where a frame's previous BEV comes from: none (self mode, prev_bev = None), a caller's fp32 prev_bev [Nq, 256], or the engine
+// history (a video frame after the first of its scene).  The rotation applied to it is a device map of source cells (NULL = no
+// rotation) or, when `grid` is set, the source cells computed from grid coefficients.  A video frame also writes the history.
+struct PrevBev {
+    enum Source { NONE, CALLER, HISTORY } src = NONE;
+    const float* bev = nullptr;         // CALLER
+    const int32_t* map = nullptr;
+    const RotGrid* grid = nullptr;
+    bool writes_history = false;
 };
 
 }  // namespace
@@ -65,10 +103,11 @@ struct occb200_engine {
     LevelGeom lg;
     ScaParams sp;
     bool cameras_set = false, finalized = false, taps = false;
-    DevBuf rot_map;                     // occb200_engine_set_prev_rotation: source row of every BEV cell (int32, -1 = outside)
-    bool rot_set = false;
-    RotGrid rot_grid;                   // occb200_engine_set_prev_rotation_angle: the same rotation as grid coefficients
-    bool rot_grid_set = false;          // (at most one of rot_set / rot_grid_set: the last call wins)
+    // the rotation of occb200_engine_forward's prev_bev, set by the last of occb200_engine_set_prev_rotation (ROT_MAP: source
+    // row of every BEV cell, int32, -1 = outside; NULL clears it) and occb200_engine_set_prev_rotation_angle (ROT_GRID)
+    enum { ROT_NONE, ROT_MAP, ROT_GRID } rot = ROT_NONE;
+    DevBuf rot_map;
+    RotGrid rot_grid;
     // occb200_engine_set_history: the last video frame's final BEV [Nq, 256] in the storage type (the bf16 / fp32 copy the last
     // LayerNorm writes), read and written only by the video calls; hist_done is recorded after every video frame
     DevBuf hist;
@@ -108,42 +147,18 @@ struct occb200_engine {
     // The origins travel inside the request and then as a kernel argument, so nothing is uploaded per frame.
     DevBuf rays;
     int rays_M = 0;
-    struct RayRequest {
-        bool armed = false;
-        RayOrigins org;
-        int8_t* cls = nullptr;          // device pointers for the device calls, host pointers for the host calls
-        void *dist = nullptr, *flow = nullptr;
-    } ray_req;
-    // occb200_engine_request_score: the frame scores itself against this ground truth into the caller's 187 device counters
-    struct ScoreRequest {
-        bool armed = false;
-        RayOrigins org;
-        const uint8_t* sem_gt = nullptr;    // device pointers for the device calls, host pointers for the host calls
-        const float* flow_gt = nullptr;
-        double* counters = nullptr;         // always a device pointer
-    } score_req;
-    // what an armed frame needs beyond the caller's outputs: the u8 class volume / the flow when the caller asked for neither,
-    // and for the host calls the device staging of the three record arrays and of the ground truth.  One set for the device
-    // calls and _forward_host, one per _submit_host slot (a slot's copies overlap the other slot's kernels).
-    struct RayStage {
-        DevBuf sem, flow, cls, dist, rflow, gt_sem, gt_flow;
-        void release()
-        {
-            sem.release(); flow.release(); cls.release(); dist.release(); rflow.release(); gt_sem.release(); gt_flow.release();
-        }
-    } ray_stage;
-    // host-buffer variant
-    DevBuf feats_dev[4], occ_i64_dev, flow_dev;
+    RayRequest ray_req;
+    ScoreRequest score_req;             // the frame scores itself against this ground truth into the caller's 187 device counters
+    FrameBufs bufs;                     // the device calls' and _forward_host's buffer set
     // pipelined host-buffer variant: 2 slots, copies on their own streams, compute on the caller's stream
     struct Slot {
-        DevBuf feats[4], occ, flow;
-        RayStage ray_stage;
+        FrameBufs bufs;
         DevBuf rot;                     // _submit_host_video: the frame's rotation map, uploaded from rot_pinned on h2d_stream[0]
         int32_t* rot_pinned = nullptr;
-        cudaEvent_t h2d_done[4] = {nullptr, nullptr, nullptr, nullptr}, compute_done = nullptr, d2h_done = nullptr;
+        cudaEvent_t h2d_done[kH2DSplit] = {}, compute_done = nullptr, d2h_done = nullptr;
         bool busy = false;
     } slots[2];
-    cudaStream_t h2d_stream[4] = {nullptr, nullptr, nullptr, nullptr}, d2h_stream = nullptr;
+    cudaStream_t h2d_stream[kH2DSplit] = {}, d2h_stream = nullptr;
     int launches = 0;
     // optional per-kernel-category timing (CUDA events on the launch stream)
     bool profiling = false;
@@ -319,7 +334,6 @@ int build_tsa_query_values(occb200_engine* e)
                        e->tsa_v_query.as<T>() + (size_t)l * Nq * C, Nq, C, C, ACT_NONE, 0)) return 2;
     }
     OCC_CUDA(cudaDeviceSynchronize());
-    q0.release();
     return 0;
 }
 
@@ -356,20 +370,11 @@ RotGrid rotation_grid(const occb200_engine* e, double angle_deg)
     return g;
 }
 
-// A video frame (occb200_engine_forward_video / _submit_host_video and their _angle forms): with `prev`, the previous BEV is
-// the engine history gathered through `map` (NULL = no rotation), or through the source cells computed from `grid` when it is
-// set, instead of a caller's fp32 prev_bev; either way the frame's last LayerNorm writes its storage-type copy of the final
-// BEV into the history.
-struct VideoArgs {
-    bool prev = false;
-    const int32_t* map = nullptr;
-    const RotGrid* grid = nullptr;
-};
-
+// One frame from device feature levels in `layout` (input dtype 0, 1 or 2; see occb200_engine_set_input_dtype).  A frame
+// that writes the history has its last LayerNorm write its storage-type copy of the final BEV there.
 template <typename T>
-int forward_impl(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed,
-                 float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, int mode = MODE_FRAME,
-                 const VideoArgs* video = nullptr)
+int forward_impl(occb200_engine* e, const float* const* feats, int layout, const PrevBev& prev, const FrameOut& out,
+                 cudaStream_t st, int mode = MODE_FRAME)
 {
     const occb200_config& c = e->cfg;
     const int Nq = e->Nq, Nv = e->Nv, C = 256, ncam = c.num_cams;
@@ -377,10 +382,10 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
     T* tokens = e->tokens.as<T>();
     if (mode == MODE_FRAME) {
         ProfScope ps(e, st, CAT_PACK);
-        if (e->feats_bf16 == 2) {
+        if (layout == 2) {
             if (launch_pack_levels_nhwc<T>(reinterpret_cast<const void* const*>(feats), e->lg, e->cams_embeds.as<float>(),
                                            e->level_embeds.as<float>(), ncam, C, Nv, tokens, st)) return 2;
-        } else if (launch_pack_levels<T>(reinterpret_cast<const void* const*>(feats), e->feats_bf16, e->lg, e->cams_embeds.as<float>(),
+        } else if (launch_pack_levels<T>(reinterpret_cast<const void* const*>(feats), layout, e->lg, e->cams_embeds.as<float>(),
                                          e->level_embeds.as<float>(), ncam, C, Nv, tokens, st)) return 2;
         e->launches++;
     }
@@ -421,19 +426,17 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
         q_f32 = x_f32;
         x_f32 = (old == cbuf) ? spare_f32 : old;
     };
-    const bool from_hist = video != nullptr && video->prev;
-    const bool has_prev = prev_bev != nullptr || from_hist;
+    const bool has_prev = prev.src != PrevBev::NONE;
     if (has_prev) {
         // encoder.py:204-209: value = stack([prev_bev, bev_query]) built ONCE before the layer loop, so
         // queue 1 keeps seeing the layer-0 query in every layer.
         // (transformer_occ.py:195-205) the rotation of prev_bev about rotate_center is a nearest-neighbour row permutation:
-        // applied here, fused with the operand cast, from the index map set by occb200_engine_set_prev_rotation (or the
-        // source cells each thread computes from the angle of occb200_engine_set_prev_rotation_angle / the _angle calls).  The
-        // history already holds the operand rounding of the previous bev_embed, so gathering it gives the same operand.
-        if (from_hist) {
-            if (launch_gather_rows_stored<T>(e->hist.as<T>(), video->map, video->grid, Nq, C, e->prev_t.as<T>(), st)) return 2;
-        } else if (launch_gather_rows<T>(prev_bev, e->rot_set ? e->rot_map.as<int32_t>() : nullptr,
-                                         e->rot_grid_set ? &e->rot_grid : nullptr, Nq, C, e->prev_t.as<T>(), nullptr, st))
+        // applied here, fused with the operand cast, from the frame's index map (or the source cells each thread computes
+        // from its grid coefficients).  The history already holds the operand rounding of the previous bev_embed, so
+        // gathering it gives the same operand.
+        if (prev.src == PrevBev::HISTORY) {
+            if (launch_gather_rows_stored<T>(e->hist.as<T>(), prev.map, prev.grid, Nq, C, e->prev_t.as<T>(), st)) return 2;
+        } else if (launch_gather_rows<T>(prev.bev, prev.map, prev.grid, Nq, C, e->prev_t.as<T>(), nullptr, st))
             return 2;
         e->launches++;
     }
@@ -571,7 +574,7 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
         if (gemm<T, T>(e, q_t, nullptr, 0, w.ffn1_w.as<float>(), w.ffn1_wh.p, w.ffn1_b.as<float>(), nullptr,
                        e->ffn_h.as<T>(), Nq, c.ffn_dim, C, ACT_RELU, st)) return 2;
         // a video frame's last LayerNorm writes its storage-type copy straight into the history (q_t is not read afterwards)
-        T* y_t = video != nullptr && l == c.num_layers - 1 ? e->hist.as<T>() : q_t;
+        T* y_t = prev.writes_history && l == c.num_layers - 1 ? e->hist.as<T>() : q_t;
         if (fuse_ln) {
             const bool need_qpos = !fold_pos;                // only the unfolded TSA query projection reads q + pos
             if (gemm_ln_fused(e, e->ffn_h.as<bf16>(), w.ffn2_wh.p, w.ffn2_b.as<float>(), q_f32, w.ln_g[2].as<float>(),
@@ -595,16 +598,16 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
     }
     const int X = c.bev_w, Y = c.bev_h, Z = c.pillar_h, mid = C / Z;
     // the voxel lift reads the T32 residual stream directly when bev_embed itself is not an output (one kernel instead of two)
-    const bool lift_from_t32 = fuse_ln && sizeof(T) == 2 && bev_embed == nullptr && Z == 16 && mid == 16;
+    const bool lift_from_t32 = fuse_ln && sizeof(T) == 2 && out.bev_embed == nullptr && Z == 16 && mid == 16;
     if (fuse_ln && !lift_from_t32) {                               // back to row-major for the outputs / voxel decoder
         ProfScope ps(e, st, CAT_PACK);
         if (launch_t32_convert(q_f32, x_f32, Nq, 1, st)) return 2;
         advance();
         e->launches++;
     }
-    if (bev_embed)
-        OCC_CUDA(cudaMemcpyAsync(bev_embed, q_f32, (size_t)Nq * C * 4, cudaMemcpyDeviceToDevice, st));
-    if (!occ_logits && !flow && !cls_u8 && !cls_i64) return 0;
+    if (out.bev_embed)
+        OCC_CUDA(cudaMemcpyAsync(out.bev_embed, q_f32, (size_t)Nq * C * 4, cudaMemcpyDeviceToDevice, st));
+    if (!out.occ_logits && !out.flow && !out.cls_u8 && !out.cls_i64) return 0;
     // ---- voxel decoder + heads
     {
         ProfScope ps(e, st, CAT_VOX);
@@ -651,8 +654,9 @@ int forward_impl(occb200_engine* e, const float* const* feats, const float* prev
         if (conv_tc && e->head_w1h.p) {
             if (launch_occ_head_tc(e->vox2.as<bf16>(), e->head_w1h.as<bf16>(), e->head_w2h.as<bf16>(),
                                    e->head_b1c.as<float>(), e->head_b2c.as<float>(), c.num_classes, (int64_t)X * Y * Z,
-                                   occ_logits, flow, cls_u8, cls_i64, st)) return 2;
-        } else if (launch_occ_head<T>(e->vox2.as<T>(), hw, (int64_t)X * Y * Z, occ_logits, flow, cls_u8, cls_i64, st))
+                                   out.occ_logits, out.flow, out.cls_u8, out.cls_i64, st)) return 2;
+        } else if (launch_occ_head<T>(e->vox2.as<T>(), hw, (int64_t)X * Y * Z, out.occ_logits, out.flow, out.cls_u8,
+                                      out.cls_i64, st))
             return 2;
     }
     e->launches += 4;
@@ -677,36 +681,35 @@ int check_backbone(const occb200_engine* e, const occb200_backbone* bb)
     return 0;
 }
 
-// uint8 frames [num_cams, src_h, src_w, 3] of the attached backbone
-size_t frame_bytes(const occb200_engine* e)
+// bytes of input buffer l in `layout` (see occb200_engine_set_input_dtype): feature level l of dtype 0 (fp32) or 1 / 2
+// (bf16), or for 3 the uint8 frames [num_cams, src_h, src_w, 3] of the attached backbone (l = 0)
+size_t input_bytes(const occb200_engine* e, int layout, int l)
 {
-    const BackboneInfo bi = backbone_info(e->bb);
-    return (size_t)e->cfg.num_cams * bi.src_h * bi.src_w * 3;
+    if (layout == 3) {
+        const BackboneInfo bi = backbone_info(e->bb);
+        return (size_t)e->cfg.num_cams * bi.src_h * bi.src_w * 3;
+    }
+    return (size_t)e->cfg.num_cams * 256 * e->lg.h[l] * e->lg.w[l] * (layout ? 2 : 4);
 }
 
 template <typename T>
-int forward_frames_impl(occb200_engine* e, const uint8_t* frames, const float* prev_bev, float* bev_embed, float* occ_logits,
-                        float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video)
+int forward_frames_impl(occb200_engine* e, const uint8_t* frames, const PrevBev& prev, const FrameOut& out, cudaStream_t st)
 {
     const BackboneInfo bi = backbone_info(e->bb);
-    const bool cl = e->cfg.precision == 1 && bi.precision == 1;   // bf16 -> bf16: channels-last hand-over (input dtype 2)
+    const int layout = e->cfg.precision == 1 && bi.precision == 1 ? 2 : 0;   // bf16 -> bf16: channels-last hand-over
     void* lv[4];
     for (int l = 0; l < 4; ++l) {
-        const size_t n = (size_t)e->cfg.num_cams * 256 * e->lg.h[l] * e->lg.w[l] * (cl ? 2 : 4);
-        if (e->bb_levels[l].bytes != n && e->bb_levels[l].alloc(n)) return 2;
+        if (ensure(e->bb_levels[l], input_bytes(e, layout, l))) return 2;
         lv[l] = e->bb_levels[l].p;
     }
     if (!e->bb_free) OCC_CUDA(cudaEventCreateWithFlags(&e->bb_free, cudaEventDisableTiming));
     // the backbone workspace and the level buffers are shared by every stream the frames arrive on
     if (e->bb_free_recorded) OCC_CUDA(cudaStreamWaitEvent(st, e->bb_free, 0));
-    int rc = occb200_backbone_forward_frames(e->bb, frames, lv[0], lv[1], lv[2], lv[3], cl ? 1 : 0, st);
+    int rc = occb200_backbone_forward_frames(e->bb, frames, lv[0], lv[1], lv[2], lv[3], layout == 2 ? 1 : 0, st);
     if (rc) return rc;
     const int bb_launches = backbone_info(e->bb).launches;
     const float* feats[4] = {(const float*)lv[0], (const float*)lv[1], (const float*)lv[2], (const float*)lv[3]};
-    const int code = e->feats_bf16;
-    e->feats_bf16 = cl ? 2 : 0;
-    rc = forward_impl<T>(e, feats, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, MODE_FRAME, video);
-    e->feats_bf16 = code;
+    rc = forward_impl<T>(e, feats, layout, prev, out, st);
     if (rc) return rc;
     OCC_CUDA(cudaEventRecord(e->bb_free, st));
     e->bb_free_recorded = true;
@@ -714,7 +717,7 @@ int forward_frames_impl(occb200_engine* e, const uint8_t* frames, const float* p
     return 0;
 }
 
-// Host-side checks of a device-buffer frame: error 1, nothing enqueued.
+// Host-side checks of a frame's input pointers (device or host): error 1, nothing enqueued.
 int check_frame(const occb200_engine* e, const float* const* feats)
 {
     OCC_CHECK(e->finalized, "engine_finalize() has not been called");
@@ -728,118 +731,183 @@ int check_frame(const occb200_engine* e, const float* const* feats)
     return 0;
 }
 
-int ensure(DevBuf& b, size_t n) { return b.bytes != n && b.alloc(n) ? 2 : 0; }
-
-// The host calls hand an armed request device staging for its three record arrays and copy them out after the frame: the
-// request's host pointers are returned in `host`.
-int stage_ray_request(occb200_engine* e, occb200_engine::RayStage& rs, occb200_engine::RayRequest* host)
-{
-    *host = e->ray_req;
-    if (!host->armed) return 0;
-    const size_t n = (size_t)8 * e->rays_M;                        // room for the largest T: no reallocation between frames
-    if (ensure(rs.cls, n) || ensure(rs.dist, n * 2) || ensure(rs.rflow, n * 4)) { e->ray_req.armed = false; return 2; }
-    e->ray_req.cls = rs.cls.as<int8_t>(); e->ray_req.dist = rs.dist.p; e->ray_req.flow = rs.rflow.p;
-    return 0;
-}
-
-int copy_ray_records(const occb200_engine* e, const occb200_engine::RayStage& rs, const occb200_engine::RayRequest& host,
-                     cudaStream_t st)
-{
-    if (!host.armed) return 0;
-    const size_t n = (size_t)host.org.T * e->rays_M;
-    OCC_CUDA(cudaMemcpyAsync(host.cls, rs.cls.p, n, cudaMemcpyDeviceToHost, st));
-    OCC_CUDA(cudaMemcpyAsync(host.dist, rs.dist.p, n * 2, cudaMemcpyDeviceToHost, st));
-    OCC_CUDA(cudaMemcpyAsync(host.flow, rs.rflow.p, n * 4, cudaMemcpyDeviceToHost, st));
-    return 0;
-}
-
-// The host calls upload an armed score request's ground truth into device staging on `copy`, a stream the frame is ordered
-// after, and point the request at the staging.
-int stage_score_request(occb200_engine* e, occb200_engine::RayStage& rs, cudaStream_t copy)
-{
-    occb200_engine::ScoreRequest& sq = e->score_req;
-    if (!sq.armed) return 0;
-    const size_t nvox = (size_t)e->cfg.bev_w * e->cfg.bev_h * e->cfg.pillar_h;
-    if (ensure(rs.gt_sem, nvox) || ensure(rs.gt_flow, nvox * 8)) { sq.armed = false; return 2; }
-    OCC_CUDA(cudaMemcpyAsync(rs.gt_sem.p, sq.sem_gt, nvox, cudaMemcpyHostToDevice, copy));
-    OCC_CUDA(cudaMemcpyAsync(rs.gt_flow.p, sq.flow_gt, nvox * 8, cudaMemcpyHostToDevice, copy));
-    sq.sem_gt = rs.gt_sem.as<uint8_t>(); sq.flow_gt = rs.gt_flow.as<float>();
-    return 0;
-}
-
 // a frame with a request armed may decline its volumes
 bool request_armed(const occb200_engine* e) { return e && (e->ray_req.armed || e->score_req.armed); }
 
-int run_frame_volumes(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed, float* occ_logits,
-                      float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video);
-
-// Every frame call ends up here.  An armed ray request (occb200_engine_request_rays) and an armed score request
-// (occb200_engine_request_score) are consumed by this frame: the head also writes the u8 classes and the flow (into `rs` when
-// the caller did not ask for them) and ray_records_kernel / ray_score_kernel follow it on the frame's stream.
-int run_frame(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed, float* occ_logits,
-              float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video = nullptr,
-              occb200_engine::RayStage* rs = nullptr)
+// The requests the next frame consumes, disarmed in the engine: called once every check of the frame call has passed.
+Requests take_requests(occb200_engine* e)
 {
-    const occb200_engine::RayRequest rq = e->ray_req;
+    const Requests rq{e->ray_req, e->score_req};
     e->ray_req.armed = false;
-    const occb200_engine::ScoreRequest sq = e->score_req;
     e->score_req.armed = false;
-    if (rq.armed || sq.armed) {
-        if (rs == nullptr) rs = &e->ray_stage;
+    return rq;
+}
+
+// A video frame's previous BEV: the history, rotated by `map` (device) or `grid`, unless the scene starts here or no video
+// frame has written it since set_history(e, 1) (self mode); either way the frame writes the history.
+PrevBev video_prev(const occb200_engine* e, int scene_start, const int32_t* map, const RotGrid* grid)
+{
+    PrevBev p;
+    p.src = scene_start == 0 && e->hist_valid ? PrevBev::HISTORY : PrevBev::NONE;
+    p.map = map;
+    p.grid = grid;
+    p.writes_history = true;
+    return p;
+}
+
+// Every frame call ends up here, after all of its checks.  The frame consumes `rq`: the head also writes the u8 classes and
+// the flow (into `b` when the caller did not ask for them) and ray_records_kernel / ray_score_kernel follow it on the frame's
+// stream.  A frame that writes the history waits for the previous one's write (on whatever stream that ran) before it reads
+// it, and records hist_done after its own.
+int run_frame(occb200_engine* e, const float* const* feats, const PrevBev& prev, FrameOut out, const Requests& rq,
+              FrameBufs& b, cudaStream_t st)
+{
+    if (rq.rays.armed || rq.score.armed) {
         const size_t nvox = (size_t)e->cfg.bev_w * e->cfg.bev_h * e->cfg.pillar_h;
-        if (cls_u8 == nullptr) {
-            if (ensure(rs->sem, nvox)) return 2;
-            cls_u8 = rs->sem.as<uint8_t>();
+        if (out.cls_u8 == nullptr) {
+            if (ensure(b.sem, nvox)) return 2;
+            out.cls_u8 = b.sem.as<uint8_t>();
         }
-        if (flow == nullptr) {
-            if (ensure(rs->flow, nvox * 8)) return 2;
-            flow = rs->flow.as<float>();
+        if (out.flow == nullptr) {
+            if (ensure(b.flow, nvox * 8)) return 2;
+            out.flow = b.flow.as<float>();
         }
     }
-    const int rc = run_frame_volumes(e, feats, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, video);
+    if (prev.writes_history && e->hist_recorded) OCC_CUDA(cudaStreamWaitEvent(st, e->hist_done, 0));
+    const bool f32 = e->cfg.precision == 0;
+    int rc;
+    if (e->feats_bf16 == 3) {
+        const uint8_t* frames = reinterpret_cast<const uint8_t*>(feats[0]);
+        rc = f32 ? forward_frames_impl<float>(e, frames, prev, out, st) : forward_frames_impl<bf16>(e, frames, prev, out, st);
+    } else {
+        rc = f32 ? forward_impl<float>(e, feats, e->feats_bf16, prev, out, st)
+                 : forward_impl<bf16>(e, feats, e->feats_bf16, prev, out, st);
+    }
     if (rc) return rc;
-    if (rq.armed) {
+    if (rq.rays.armed) {
+        const RayRequest& r = rq.rays;
         e->launches++;
-        if (launch_ray_records(cls_u8, flow, rq.org, e->rays.as<float>(), e->rays_M, rq.cls, rq.dist, rq.flow, st)) return 2;
+        if (launch_ray_records(out.cls_u8, out.flow, r.org, e->rays.as<float>(), e->rays_M, r.cls, r.dist, r.flow, st)) return 2;
     }
-    if (sq.armed) {
+    if (rq.score.armed) {
+        const ScoreRequest& s = rq.score;
         e->launches++;
-        if (launch_ray_score(cls_u8, flow, sq.sem_gt, sq.flow_gt, sq.org, e->rays.as<float>(), e->rays_M, sq.counters, st))
+        if (launch_ray_score(out.cls_u8, out.flow, s.sem_gt, s.flow_gt, s.org, e->rays.as<float>(), e->rays_M, s.counters, st))
             return 2;
+    }
+    if (prev.writes_history) {
+        OCC_CUDA(cudaEventRecord(e->hist_done, st));
+        e->hist_recorded = true;
+        e->hist_valid = true;
     }
     return 0;
 }
 
-int run_frame_volumes(occb200_engine* e, const float* const* feats, const float* prev_bev, float* bev_embed, float* occ_logits,
-                      float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st, const VideoArgs* video)
+// Every host-buffer frame (_forward_host, _submit_host, _submit_host_video[_angle]) after its entry point's own checks, in
+// this order: the remaining checks (error 1 before any CUDA call, the requests still armed), the uploads of the inputs and of
+// the host rotation map `map_host` (NULL: none), the request staging, the frame, the copies back.  `slot` -1 (_forward_host):
+// every copy on the caller's stream, then a stream synchronise.  Slot 0 / 1: uploads on the copy streams, the frame on the
+// caller's stream after them, the copies back on d2h_stream; the slot stays busy until _wait_host.
+int host_frame(occb200_engine* e, int slot, const float* const* feats_host, PrevBev prev, const int32_t* map_host,
+               int64_t* occ_host, float* flow_host, cudaStream_t st)
 {
-    if (e->feats_bf16 == 3) {
-        const uint8_t* frames = reinterpret_cast<const uint8_t*>(feats[0]);
-        if (e->cfg.precision == 0)
-            return forward_frames_impl<float>(e, frames, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, video);
-        return forward_frames_impl<bf16>(e, frames, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, video);
-    }
-    if (e->cfg.precision == 0)
-        return forward_impl<float>(e, feats, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, MODE_FRAME, video);
-    return forward_impl<bf16>(e, feats, prev_bev, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, MODE_FRAME, video);
-}
+    occb200_engine::Slot* s = slot < 0 ? nullptr : &e->slots[slot];
+    OCC_CHECK(s == nullptr || !s->busy, "slot still in flight: call occb200_engine_wait_host first");
+    if (check_frame(e, feats_host)) return 1;
+    if (map_host)
+        for (int q = 0; q < e->Nq; ++q) OCC_CHECK(map_host[q] >= -1 && map_host[q] < e->Nq, "rotation map entry out of range");
 
-// One video frame on device buffers, after every host-side check has passed.  The frame waits for the previous video
-// frame (on whatever stream that ran) before it reads the history, and records hist_done after it has written it.
-int run_video_frame(occb200_engine* e, const float* const* feats, const int32_t* map_dev, const RotGrid* grid, int scene_start,
-                    float* bev_embed, float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st,
-                    occb200_engine::RayStage* rs = nullptr)
-{
-    VideoArgs v;
-    v.prev = scene_start == 0 && e->hist_valid;
-    v.map = map_dev;
-    v.grid = grid;
-    if (e->hist_recorded) OCC_CUDA(cudaStreamWaitEvent(st, e->hist_done, 0));
-    const int rc = run_frame(e, feats, nullptr, bev_embed, occ_logits, flow, cls_u8, cls_i64, st, &v, rs);
+    FrameBufs& b = s ? s->bufs : e->bufs;
+    if (s && !e->d2h_stream) {
+        for (cudaStream_t& hs : e->h2d_stream) OCC_CUDA(cudaStreamCreateWithFlags(&hs, cudaStreamNonBlocking));
+        OCC_CUDA(cudaStreamCreateWithFlags(&e->d2h_stream, cudaStreamNonBlocking));
+    }
+    if (s && !s->compute_done) {
+        for (cudaEvent_t& ev : s->h2d_done) OCC_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        OCC_CUDA(cudaEventCreateWithFlags(&s->compute_done, cudaEventDisableTiming));
+        OCC_CUDA(cudaEventCreateWithFlags(&s->d2h_done, cudaEventDisableTiming));
+    }
+    if (map_host) {
+        // staged in the slot's pinned buffer so that the caller may reuse its array on return; h2d_done[0] covers the upload
+        const size_t mb = (size_t)e->Nq * 4;
+        if (!s->rot_pinned) OCC_CUDA(cudaMallocHost(&s->rot_pinned, mb));
+        if (ensure(s->rot, mb)) return 2;
+        OCC_CUDA(cudaEventSynchronize(s->h2d_done[0]));            // the slot's previous upload has left the staging buffer
+        memcpy(s->rot_pinned, map_host, mb);
+        OCC_CUDA(cudaMemcpyAsync(s->rot.p, s->rot_pinned, mb, cudaMemcpyHostToDevice, e->h2d_stream[0]));
+        prev.map = s->rot.as<int32_t>();
+    }
+    const int layout = e->feats_bf16;
+    const float* dev_feats[4] = {nullptr, nullptr, nullptr, nullptr};
+    for (int l = 0; l < (layout == 3 ? 1 : 4); ++l) {                     // input dtype 3: one buffer, the uint8 frames
+        const size_t n = input_bytes(e, layout, l);
+        if (ensure(b.feats[l], n)) return 2;
+        if (s) {
+            const int pieces = n >= (32u << 20) ? kH2DSplit : 1;
+            const size_t chunk = ((n / pieces) + 255) & ~(size_t)255;
+            for (int i = 0; i < pieces; ++i) {
+                const size_t o = (size_t)i * chunk, len = o >= n ? 0 : (n - o < chunk ? n - o : chunk);
+                if (len) OCC_CUDA(cudaMemcpyAsync((char*)b.feats[l].p + o, (const char*)feats_host[l] + o, len,
+                                                  cudaMemcpyHostToDevice, e->h2d_stream[i]));
+            }
+        } else {
+            OCC_CUDA(cudaMemcpyAsync(b.feats[l].p, feats_host[l], n, cudaMemcpyHostToDevice, st));
+        }
+        dev_feats[l] = b.feats[l].as<float>();
+    }
+
+    // the requests point the frame at device staging: room for a ray request's records (the largest T, so no reallocation
+    // between frames), and a score request's ground truth, uploaded after the features
+    const Requests host_rq = take_requests(e);
+    Requests rq = host_rq;
+    const size_t nvox = (size_t)e->cfg.bev_w * e->cfg.bev_h * e->cfg.pillar_h;
+    if (rq.rays.armed) {
+        const size_t n = (size_t)8 * e->rays_M;
+        if (ensure(b.rec_cls, n) || ensure(b.rec_dist, n * 2) || ensure(b.rec_flow, n * 4)) return 2;
+        rq.rays.cls = b.rec_cls.as<int8_t>(); rq.rays.dist = b.rec_dist.p; rq.rays.flow = b.rec_flow.p;
+    }
+    if (rq.score.armed) {
+        if (ensure(b.gt_sem, nvox) || ensure(b.gt_flow, nvox * 8)) return 2;
+        cudaStream_t copy = s ? e->h2d_stream[0] : st;
+        OCC_CUDA(cudaMemcpyAsync(b.gt_sem.p, rq.score.sem_gt, nvox, cudaMemcpyHostToDevice, copy));
+        OCC_CUDA(cudaMemcpyAsync(b.gt_flow.p, rq.score.flow_gt, nvox * 8, cudaMemcpyHostToDevice, copy));
+        rq.score.sem_gt = b.gt_sem.as<uint8_t>(); rq.score.flow_gt = b.gt_flow.as<float>();
+    }
+    if (s)
+        for (int i = 0; i < kH2DSplit; ++i) {                       // compute waits for this frame's uploads only
+            OCC_CUDA(cudaEventRecord(s->h2d_done[i], e->h2d_stream[i]));
+            OCC_CUDA(cudaStreamWaitEvent(st, s->h2d_done[i], 0));
+        }
+
+    if (occ_host && ensure(b.occ, nvox * 8)) return 2;
+    if (ensure(b.flow, nvox * 8)) return 2;
+    FrameOut out;
+    out.flow = b.flow.as<float>();
+    out.cls_i64 = occ_host ? b.occ.as<int64_t>() : nullptr;
+    const int rc = run_frame(e, dev_feats, prev, out, rq, b, st);
     if (rc) return rc;
-    OCC_CUDA(cudaEventRecord(e->hist_done, st));
-    e->hist_recorded = true;
-    e->hist_valid = true;
+
+    cudaStream_t d2h = st;
+    if (s) {
+        OCC_CUDA(cudaEventRecord(s->compute_done, st));
+        OCC_CUDA(cudaStreamWaitEvent(e->d2h_stream, s->compute_done, 0));
+        d2h = e->d2h_stream;
+    }
+    if (occ_host) OCC_CUDA(cudaMemcpyAsync(occ_host, b.occ.p, nvox * 8, cudaMemcpyDeviceToHost, d2h));
+    if (flow_host) OCC_CUDA(cudaMemcpyAsync(flow_host, b.flow.p, nvox * 8, cudaMemcpyDeviceToHost, d2h));
+    if (host_rq.rays.armed) {
+        const RayRequest& r = host_rq.rays;
+        const size_t n = (size_t)r.org.T * e->rays_M;
+        OCC_CUDA(cudaMemcpyAsync(r.cls, b.rec_cls.p, n, cudaMemcpyDeviceToHost, d2h));
+        OCC_CUDA(cudaMemcpyAsync(r.dist, b.rec_dist.p, n * 2, cudaMemcpyDeviceToHost, d2h));
+        OCC_CUDA(cudaMemcpyAsync(r.flow, b.rec_flow.p, n * 4, cudaMemcpyDeviceToHost, d2h));
+    }
+    if (!s) {
+        OCC_CUDA(cudaStreamSynchronize(st));
+        return 0;
+    }
+    OCC_CUDA(cudaEventRecord(s->d2h_done, d2h));
+    s->busy = true;
     return 0;
 }
 
@@ -909,30 +977,10 @@ int occb200_engine_create(const occb200_config* cfg, occb200_engine** out)
 void occb200_engine_destroy(occb200_engine* e)
 {
     if (!e) return;
-    // DevBuf members do not own a destructor on purpose (explicit release keeps teardown order obvious)
-    for (auto& w : e->layers) {
-        DevBuf* all[] = {&w.tsa_v_w, &w.tsa_v_b, &w.tsa_q_w, &w.tsa_q_b, &w.tsa_o_w, &w.tsa_o_b, &w.sca_q_w, &w.sca_q_b,
-                         &w.sca_v_w, &w.sca_v_b, &w.sca_o_w, &w.sca_o_b, &w.ffn1_w, &w.ffn1_b, &w.ffn2_w, &w.ffn2_b,
-                         &w.ln_g[0], &w.ln_g[1], &w.ln_g[2], &w.ln_b[0], &w.ln_b[1], &w.ln_b[2], &w.tsa_v_wh,
-                         &w.tsa_q_wh, &w.tsa_o_wh, &w.sca_q_wh, &w.sca_v_wh, &w.sca_o_wh, &w.ffn1_wh, &w.ffn2_wh,
-                         &w.tsa_q_wh_fold, &w.tsa_q_const, &w.tsa_q_const_t32};
-        for (DevBuf* b : all) b->release();
-    }
-    DevBuf* all[] = {&e->rot_map, &e->hist, &e->split_ws, &e->tokens_split, &e->l0_x_f32, &e->l0_q_t, &e->pos_bf, &e->qc_f32, &e->qc_t, &e->qc_pos_t, &e->bev_queries, &e->pos, &e->pos_t32, &e->cams_embeds, &e->level_embeds, &e->conv_w[0], &e->conv_w[1],
-                     &e->conv_b[0], &e->conv_b[1], &e->conv_wh[0], &e->conv_wh[1], &e->conv_wh_hi[0], &e->conv_wh_hi[1], &e->conv_wh_lo[0],
-                     &e->conv_wh_lo[1], &e->vox_split, &e->sca_v_all_wh, &e->sca_v_all_b, &e->sca_value_all, &e->hw1, &e->hb1, &e->hw2, &e->hb2,
-                     &e->fw1, &e->fb1, &e->fw2, &e->fb2, &e->head_w1h, &e->head_w2h, &e->head_b1c, &e->head_b2c, &e->tokens, &e->sca_value, &e->q_f32, &e->q_t,
-                     &e->q_pos_t, &e->prev_t, &e->tsa_value, &e->tsa_v_query, &e->qproj, &e->attn_out,
-                     &e->x_f32, &e->ffn_h, &e->vox0, &e->vox1, &e->vox2, &e->hits, &e->tap_layer, &e->tap_tsa,
-                     &e->tap_sca, &e->feats_dev[0], &e->feats_dev[1], &e->feats_dev[2], &e->feats_dev[3],
-                     &e->occ_i64_dev, &e->flow_dev, &e->rays, &e->bb_levels[0], &e->bb_levels[1], &e->bb_levels[2], &e->bb_levels[3]};
-    for (DevBuf* b : all) b->release();
-    e->ray_stage.release();
+    // the device buffers free themselves; events, streams and pinned staging are released here
     if (e->bb_free) cudaEventDestroy(e->bb_free);
     if (e->hist_done) cudaEventDestroy(e->hist_done);
     for (auto& sl : e->slots) {
-        for (auto& f : sl.feats) f.release();
-        sl.occ.release(); sl.flow.release(); sl.rot.release(); sl.ray_stage.release();
         if (sl.rot_pinned) cudaFreeHost(sl.rot_pinned);
         if (sl.compute_done) {
             for (cudaEvent_t ev : sl.h2d_done) cudaEventDestroy(ev);
@@ -994,7 +1042,6 @@ int occb200_engine_finalize(occb200_engine* e)
                                            e->qc_t.as<bf16>(), e->qc_pos_t.as<bf16>(), 1, 0)) return 2;
         }
         OCC_CUDA(cudaDeviceSynchronize());
-        dre.release(); dce.release();
         GETP(le, "transformer.level_embeds", (size_t)c.num_levels * C);
         GETP(cm, "transformer.cams_embeds", (size_t)c.num_cams * C);
         std::vector<float> cams(*cm);
@@ -1050,7 +1097,6 @@ int occb200_engine_finalize(occb200_engine* e)
                     if (launch_t32_convert(fold_const->as<float>(), w.tsa_q_const_t32.as<float>(), Nq, 0, 0, (int)rows)) return 2;
                 }
                 OCC_CUDA(cudaDeviceSynchronize());
-                w2.release();
             }
             return 0;
         };
@@ -1187,7 +1233,7 @@ int occb200_engine_finalize(occb200_engine* e)
         OCC_CUDA(cudaMemset(e->l0_x_f32.p, 0, rows_pad * C * 4));
         const bool taps = e->taps;
         e->taps = false;
-        const int rc = forward_impl<bf16>(e, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, MODE_L0_TSA_ONLY);
+        const int rc = forward_impl<bf16>(e, nullptr, 0, PrevBev(), FrameOut(), 0, MODE_L0_TSA_ONLY);
         e->taps = taps;
         if (rc) return rc;
         OCC_CUDA(cudaDeviceSynchronize());
@@ -1211,7 +1257,15 @@ int occb200_engine_forward(occb200_engine* e, const float* const* feats, const f
 {
     OCC_CHECK(e && feats, "null pointer");
     if (check_frame(e, feats)) return 1;
-    return run_frame(e, feats, prev_bev, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64, (cudaStream_t)stream);
+    PrevBev prev;
+    if (prev_bev) {
+        prev.src = PrevBev::CALLER;
+        prev.bev = prev_bev;
+        prev.map = e->rot == occb200_engine::ROT_MAP ? e->rot_map.as<int32_t>() : nullptr;
+        prev.grid = e->rot == occb200_engine::ROT_GRID ? &e->rot_grid : nullptr;
+    }
+    return run_frame(e, feats, prev, {bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64}, take_requests(e), e->bufs,
+                     (cudaStream_t)stream);
 }
 
 int occb200_engine_set_history(occb200_engine* e, int enable)
@@ -1225,7 +1279,7 @@ int occb200_engine_set_history(occb200_engine* e, int enable)
         return 0;
     }
     const size_t n = (size_t)e->Nq * 256 * e->elt();
-    if (e->hist.bytes != n && e->hist.alloc(n)) return 2;
+    if (ensure(e->hist, n)) return 2;
     if (!e->hist_done) OCC_CUDA(cudaEventCreateWithFlags(&e->hist_done, cudaEventDisableTiming));
     return 0;
 }
@@ -1238,8 +1292,8 @@ int occb200_engine_forward_video(occb200_engine* e, const float* const* feats, c
     OCC_CHECK(e, "null engine");
     OCC_CHECK(e->hist.p != nullptr, "history not enabled: call occb200_engine_set_history(e, 1) first");
     if (check_frame(e, feats)) return 1;
-    return run_video_frame(e, feats, rot_map_dev, nullptr, scene_start, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64,
-                           (cudaStream_t)stream);
+    return run_frame(e, feats, video_prev(e, scene_start, rot_map_dev, nullptr),
+                     {bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64}, take_requests(e), e->bufs, (cudaStream_t)stream);
 }
 
 int occb200_engine_forward_video_angle(occb200_engine* e, const float* const* feats, double angle_deg, int scene_start,
@@ -1252,8 +1306,8 @@ int occb200_engine_forward_video_angle(occb200_engine* e, const float* const* fe
     OCC_CHECK(e->hist.p != nullptr, "history not enabled: call occb200_engine_set_history(e, 1) first");
     if (check_frame(e, feats)) return 1;
     const RotGrid g = rotation_grid(e, angle_deg);
-    return run_video_frame(e, feats, nullptr, &g, scene_start, bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64,
-                           (cudaStream_t)stream);
+    return run_frame(e, feats, video_prev(e, scene_start, nullptr, &g), {bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64},
+                     take_requests(e), e->bufs, (cudaStream_t)stream);
 }
 
 int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_host, int64_t* occ_cls_i64_host,
@@ -1261,125 +1315,15 @@ int occb200_engine_forward_host(occb200_engine* e, const float* const* feats_hos
 {
     // with a ray or score request armed the caller may decline either volume (NULL): that 5.12 MB copy is then skipped
     OCC_CHECK(e && feats_host && ((occ_cls_i64_host && flow_host) || request_armed(e)), "null pointer");
-    OCC_CHECK(e->finalized && e->cameras_set, "engine not finalized / cameras not set");
-    if (e->feats_bf16 == 3) OCC_CHECK(e->bb != nullptr && feats_host[0] != nullptr, "input dtype 3 needs an attached backbone and a frame buffer");
-    const occb200_config& c = e->cfg;
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t nvox = (size_t)c.bev_w * c.bev_h * c.pillar_h;
-    const float* dev_feats[4] = {nullptr, nullptr, nullptr, nullptr};
-    for (int l = 0; l < (e->feats_bf16 == 3 ? 1 : 4); ++l) {
-        const size_t n = e->feats_bf16 == 3 ? frame_bytes(e)
-                                            : (size_t)c.num_cams * 256 * e->lg.h[l] * e->lg.w[l] * (e->feats_bf16 ? 2 : 4);
-        if (e->feats_dev[l].bytes != n && e->feats_dev[l].alloc(n)) return 2;
-        OCC_CUDA(cudaMemcpyAsync(e->feats_dev[l].p, feats_host[l], n, cudaMemcpyHostToDevice, st));
-        dev_feats[l] = e->feats_dev[l].as<float>();
-    }
-    if (occ_cls_i64_host && ensure(e->occ_i64_dev, nvox * 8)) return 2;
-    if (ensure(e->flow_dev, nvox * 8)) return 2;
-    if (check_frame(e, dev_feats)) return 1;
-    occb200_engine::RayRequest rays_host;                          // an armed request: records through the engine's staging
-    if (stage_ray_request(e, e->ray_stage, &rays_host)) return 2;
-    if (stage_score_request(e, e->ray_stage, st)) return 2;
-    int rc = run_frame(e, dev_feats, nullptr, nullptr, nullptr, e->flow_dev.as<float>(), nullptr,
-                       occ_cls_i64_host ? e->occ_i64_dev.as<int64_t>() : nullptr, st);
-    if (rc) return rc;
-    if (occ_cls_i64_host) OCC_CUDA(cudaMemcpyAsync(occ_cls_i64_host, e->occ_i64_dev.p, nvox * 8, cudaMemcpyDeviceToHost, st));
-    if (flow_host) OCC_CUDA(cudaMemcpyAsync(flow_host, e->flow_dev.p, nvox * 8, cudaMemcpyDeviceToHost, st));
-    if (copy_ray_records(e, e->ray_stage, rays_host, st)) return 2;
-    OCC_CUDA(cudaStreamSynchronize(st));
-    return 0;
-}
-
-// _submit_host and _submit_host_video(_angle): `video` selects the history path, with the frame's host rotation map (or
-// NULL), or its rotation as grid coefficients (`grid`: nothing to stage or upload)
-static int submit_frame(occb200_engine* e, int slot, const float* const* feats_host, int64_t* occ_cls_i64_host, float* flow_host,
-                        void* stream, bool video, const int32_t* rot_map_host, const RotGrid* grid, int scene_start)
-{
-    OCC_CHECK(e && feats_host && ((occ_cls_i64_host && flow_host) || request_armed(e)), "null pointer");
-    OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
-    OCC_CHECK(e->finalized && e->cameras_set, "engine not finalized / cameras not set");
-    if (e->feats_bf16 == 3) OCC_CHECK(e->bb != nullptr && feats_host[0] != nullptr, "input dtype 3 needs an attached backbone and a frame buffer");
-    const occb200_config& c = e->cfg;
-    cudaStream_t st = (cudaStream_t)stream;
-    occb200_engine::Slot& s = e->slots[slot];
-    OCC_CHECK(!s.busy, "slot still in flight: call occb200_engine_wait_host first");
-    if (video) {                                                    // every rejection before the first CUDA call
-        OCC_CHECK(e->hist.p != nullptr, "history not enabled: call occb200_engine_set_history(e, 1) first");
-        if (check_frame(e, feats_host)) return 1;
-        if (rot_map_host)
-            for (int q = 0; q < e->Nq; ++q)
-                OCC_CHECK(rot_map_host[q] >= -1 && rot_map_host[q] < e->Nq, "rotation map entry out of range");
-    }
-    if (!e->d2h_stream) {
-        for (cudaStream_t& hs : e->h2d_stream) OCC_CUDA(cudaStreamCreateWithFlags(&hs, cudaStreamNonBlocking));
-        OCC_CUDA(cudaStreamCreateWithFlags(&e->d2h_stream, cudaStreamNonBlocking));
-    }
-    if (!s.compute_done) {
-        for (cudaEvent_t& ev : s.h2d_done) OCC_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        OCC_CUDA(cudaEventCreateWithFlags(&s.compute_done, cudaEventDisableTiming));
-        OCC_CUDA(cudaEventCreateWithFlags(&s.d2h_done, cudaEventDisableTiming));
-    }
-    if (rot_map_host) {
-        // staged in the slot's pinned buffer so that the caller may reuse its array on return; h2d_done[0] covers the upload
-        const size_t mb = (size_t)e->Nq * 4;
-        if (!s.rot_pinned) OCC_CUDA(cudaMallocHost(&s.rot_pinned, mb));
-        if (s.rot.bytes != mb && s.rot.alloc(mb)) return 2;
-        OCC_CUDA(cudaEventSynchronize(s.h2d_done[0]));             // the slot's previous upload has left the staging buffer
-        memcpy(s.rot_pinned, rot_map_host, mb);
-        OCC_CUDA(cudaMemcpyAsync(s.rot.p, s.rot_pinned, mb, cudaMemcpyHostToDevice, e->h2d_stream[0]));
-    }
-    // Levels larger than 32 MB go up in `nsplit` pieces on separate copy streams: one cudaMemcpyAsync stream reached
-    // 46 GB/s of the PCIe link on the test box, two reach 50 GB/s (OCC_H2D_SPLIT = 1..4, default 2).
-    static const int nsplit = [] {
-        const char* v = getenv("OCC_H2D_SPLIT");
-        const int n = v ? atoi(v) : 2;
-        return n < 1 ? 1 : (n > 4 ? 4 : n);
-    }();
-    const size_t nvox = (size_t)c.bev_w * c.bev_h * c.pillar_h;
-    const float* dev_feats[4] = {nullptr, nullptr, nullptr, nullptr};
-    for (int l = 0; l < (e->feats_bf16 == 3 ? 1 : 4); ++l) {              // input dtype 3: one buffer, the uint8 frames
-        const size_t n = e->feats_bf16 == 3 ? frame_bytes(e)
-                                            : (size_t)c.num_cams * 256 * e->lg.h[l] * e->lg.w[l] * (e->feats_bf16 ? 2 : 4);
-        if (s.feats[l].bytes != n && s.feats[l].alloc(n)) return 2;
-        const int pieces = n >= (32u << 20) ? nsplit : 1;
-        const size_t chunk = ((n / pieces) + 255) & ~(size_t)255;
-        for (int i = 0; i < pieces; ++i) {
-            const size_t o = (size_t)i * chunk, len = o >= n ? 0 : (n - o < chunk ? n - o : chunk);
-            if (len) OCC_CUDA(cudaMemcpyAsync((char*)s.feats[l].p + o, (const char*)feats_host[l] + o, len,
-                                              cudaMemcpyHostToDevice, e->h2d_stream[i]));
-        }
-        dev_feats[l] = s.feats[l].as<float>();
-    }
-    if (stage_score_request(e, s.ray_stage, e->h2d_stream[0])) return 2;   // ground truth of a score request: h2d_done[0] covers it
-    for (int i = 0; i < nsplit; ++i) {                              // compute waits for this frame's features only
-        OCC_CUDA(cudaEventRecord(s.h2d_done[i], e->h2d_stream[i]));
-        OCC_CUDA(cudaStreamWaitEvent(st, s.h2d_done[i], 0));
-    }
-    if (occ_cls_i64_host && ensure(s.occ, nvox * 8)) return 2;
-    if (ensure(s.flow, nvox * 8)) return 2;
-    int64_t* occ_dev = occ_cls_i64_host ? s.occ.as<int64_t>() : nullptr;
-    if (!video && check_frame(e, dev_feats)) return 1;
-    occb200_engine::RayRequest rays_host;                          // an armed request: records through the slot's staging
-    if (stage_ray_request(e, s.ray_stage, &rays_host)) return 2;
-    int rc = video ? run_video_frame(e, dev_feats, rot_map_host ? s.rot.as<int32_t>() : nullptr, grid, scene_start, nullptr,
-                                     nullptr, s.flow.as<float>(), nullptr, occ_dev, st, &s.ray_stage)
-                   : run_frame(e, dev_feats, nullptr, nullptr, nullptr, s.flow.as<float>(), nullptr, occ_dev, st, nullptr,
-                               &s.ray_stage);
-    if (rc) return rc;
-    OCC_CUDA(cudaEventRecord(s.compute_done, st));
-    OCC_CUDA(cudaStreamWaitEvent(e->d2h_stream, s.compute_done, 0));
-    if (occ_cls_i64_host) OCC_CUDA(cudaMemcpyAsync(occ_cls_i64_host, s.occ.p, nvox * 8, cudaMemcpyDeviceToHost, e->d2h_stream));
-    if (flow_host) OCC_CUDA(cudaMemcpyAsync(flow_host, s.flow.p, nvox * 8, cudaMemcpyDeviceToHost, e->d2h_stream));
-    if (copy_ray_records(e, s.ray_stage, rays_host, e->d2h_stream)) return 2;
-    OCC_CUDA(cudaEventRecord(s.d2h_done, e->d2h_stream));
-    s.busy = true;
-    return 0;
+    return host_frame(e, -1, feats_host, PrevBev(), nullptr, occ_cls_i64_host, flow_host, (cudaStream_t)stream);
 }
 
 int occb200_engine_submit_host(occb200_engine* e, int slot, const float* const* feats_host, int64_t* occ_cls_i64_host,
                                float* flow_host, void* stream)
 {
-    return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, false, nullptr, nullptr, 0);
+    OCC_CHECK(e && feats_host && ((occ_cls_i64_host && flow_host) || request_armed(e)), "null pointer");
+    OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
+    return host_frame(e, slot, feats_host, PrevBev(), nullptr, occ_cls_i64_host, flow_host, (cudaStream_t)stream);
 }
 
 int occb200_engine_submit_host_video(occb200_engine* e, int slot, const float* const* feats_host, const int32_t* rot_map_host,
@@ -1388,7 +1332,9 @@ int occb200_engine_submit_host_video(occb200_engine* e, int slot, const float* c
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
     OCC_CHECK(feats_host && ((occ_cls_i64_host && flow_host) || request_armed(e)), "null pointer");
     OCC_CHECK(e, "null engine");
-    return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, true, rot_map_host, nullptr, scene_start);
+    OCC_CHECK(e->hist.p != nullptr, "history not enabled: call occb200_engine_set_history(e, 1) first");
+    return host_frame(e, slot, feats_host, video_prev(e, scene_start, nullptr, nullptr), rot_map_host, occ_cls_i64_host,
+                      flow_host, (cudaStream_t)stream);
 }
 
 int occb200_engine_submit_host_video_angle(occb200_engine* e, int slot, const float* const* feats_host, double angle_deg,
@@ -1398,8 +1344,10 @@ int occb200_engine_submit_host_video_angle(occb200_engine* e, int slot, const fl
     OCC_CHECK(slot == 0 || slot == 1, "slot must be 0 or 1");
     OCC_CHECK(feats_host && ((occ_cls_i64_host && flow_host) || request_armed(e)), "null pointer");
     OCC_CHECK(e, "null engine");
+    OCC_CHECK(e->hist.p != nullptr, "history not enabled: call occb200_engine_set_history(e, 1) first");
     const RotGrid g = rotation_grid(e, angle_deg);
-    return submit_frame(e, slot, feats_host, occ_cls_i64_host, flow_host, stream, true, nullptr, &g, scene_start);
+    return host_frame(e, slot, feats_host, video_prev(e, scene_start, nullptr, &g), nullptr, occ_cls_i64_host, flow_host,
+                      (cudaStream_t)stream);
 }
 
 int occb200_engine_wait_host(occb200_engine* e, int slot)
@@ -1470,7 +1418,7 @@ int occb200_engine_request_rays(occb200_engine* e, const void* origins_host, int
     OCC_CHECK(e->rays.p != nullptr, "request_rays: occb200_engine_set_rays() has not been called");
     OCC_CHECK(e->cfg.bev_w == 200 && e->cfg.bev_h == 200 && e->cfg.pillar_h == 16,
               "request_rays: the ray caster works on the 200 x 200 x 16 grid only");
-    occb200_engine::RayRequest rq;
+    RayRequest rq;
     if (fill_origins(rq.org, origins_host, origin_is_f64, T)) return 1;
     rq.armed = true;
     rq.cls = cls_i8; rq.dist = dist_f16; rq.flow = flow_f16;
@@ -1489,7 +1437,7 @@ int occb200_engine_request_score(occb200_engine* e, const uint8_t* sem_gt, const
     OCC_CHECK(e->rays.p != nullptr, "request_score: occb200_engine_set_rays() has not been called");
     OCC_CHECK(e->cfg.bev_w == 200 && e->cfg.bev_h == 200 && e->cfg.pillar_h == 16,
               "request_score: the ray caster works on the 200 x 200 x 16 grid only");
-    occb200_engine::ScoreRequest sq;
+    ScoreRequest sq;
     if (fill_origins(sq.org, origins_host, origin_is_f64, T)) return 1;
     sq.armed = true;
     sq.sem_gt = sem_gt; sq.flow_gt = flow_gt; sq.counters = counters_dev;
@@ -1500,12 +1448,11 @@ int occb200_engine_request_score(occb200_engine* e, const uint8_t* sem_gt, const
 int occb200_engine_set_prev_rotation(occb200_engine* e, const int32_t* map_host)
 {
     OCC_CHECK(e, "null engine");
-    if (map_host == nullptr) { e->rot_set = false; e->rot_grid_set = false; return 0; }
+    if (map_host == nullptr) { e->rot = occb200_engine::ROT_NONE; return 0; }
     for (int q = 0; q < e->Nq; ++q) OCC_CHECK(map_host[q] >= -1 && map_host[q] < e->Nq, "rotation map entry out of range");
-    if (e->rot_map.bytes != (size_t)e->Nq * 4 && e->rot_map.alloc((size_t)e->Nq * 4)) return 2;
+    if (ensure(e->rot_map, (size_t)e->Nq * 4)) return 2;
     OCC_CUDA(cudaMemcpy(e->rot_map.p, map_host, (size_t)e->Nq * 4, cudaMemcpyHostToDevice));
-    e->rot_set = true;
-    e->rot_grid_set = false;
+    e->rot = occb200_engine::ROT_MAP;
     return 0;
 }
 
@@ -1514,8 +1461,7 @@ int occb200_engine_set_prev_rotation_angle(occb200_engine* e, double angle_deg)
     OCC_CHECK(std::isfinite(angle_deg), "rotation angle must be finite");
     OCC_CHECK(e, "null engine");
     e->rot_grid = rotation_grid(e, angle_deg);
-    e->rot_grid_set = true;
-    e->rot_set = false;
+    e->rot = occb200_engine::ROT_GRID;
     return 0;
 }
 

@@ -1,4 +1,4 @@
-// Launcher declarations shared by the engine (engine.cu) and the C-ABI (capi.cu).
+// Launcher declarations shared by the kernel sources and the host code of the engine and the C ABI (engine.cu, backbone.cu).
 #pragma once
 #include "common.cuh"
 

@@ -319,6 +319,51 @@ def test_rejections_leave_the_counters_alone_and_nothing_armed():
         small.forward(_frames(small.cfg, 1)[0], want=('flow',), score=(sem, flow, o), metric=rm)
 
 
+def test_host_calls_reject_a_null_feature_level_and_keep_the_requests():
+    """_forward_host and _submit_host reject a NULL host feature level with error 1 before any CUDA call (through the C ABI:
+    the Python wrapper never passes one): the slot stays free, and the armed ray and score requests are consumed by the next
+    valid call, which returns what it returns on a fresh engine."""
+    from occnet_b200 import _lib
+    from occnet_b200.metric import RayMetric
+    cfg = grid_cfg()
+    host = [f.cpu().contiguous().pin_memory() for f in _frames(cfg, 1)[0]]
+    _, _, sem_gt, flow_gt = metric_fixture()
+    sem_gt = torch.from_numpy(np.ascontiguousarray(sem_gt, np.uint8)).pin_memory()
+    flow_gt = torch.from_numpy(np.ascontiguousarray(flow_gt, np.float32)).pin_memory()
+    o = np.ascontiguousarray(origins(3)[0])
+    p = _lib.ptr
+
+    def valid_frame(reject_first):
+        eng = _engine(cfg, 'fp32')
+        rm, rec = RayMetric(DEV), eng.ray_buffers(3, host=True)
+        X, Y, Z = eng.vox_shape
+        occ, flow = torch.empty((X, Y, Z), dtype=torch.int64).pin_memory(), torch.empty((X, Y, Z, 2)).pin_memory()
+        st = _lib.stream_ptr()
+        assert eng.lib.occb200_engine_request_rays(eng._h, p(o), 0, 3, p(rec['ray_cls']), p(rec['ray_dist']),
+                                                   p(rec['ray_flow'])) == 0
+        assert eng.lib.occb200_engine_request_score(eng._h, p(sem_gt), p(flow_gt), p(o), 0, 3, p(rm.counters)) == 0
+        if reject_first:
+            for missing in range(4):
+                feats = eng._feat_ptrs(host)
+                feats[missing] = None
+                for rc in (eng.lib.occb200_engine_forward_host(eng._h, feats, p(occ), p(flow), st),
+                           eng.lib.occb200_engine_submit_host(eng._h, 0, feats, p(occ), p(flow), st)):
+                    assert rc == 1 and 'null feature level' in eng.lib.occb200_last_error().decode(), (missing, rc)
+        # slot 0 is free (a busy slot is rejected), and the frame consumes both requests
+        assert eng.lib.occb200_engine_submit_host(eng._h, 0, eng._feat_ptrs(host), p(occ), p(flow), st) == 0
+        eng.wait_host(0)
+        with pytest.raises(_lib.OccB200Error, match='null pointer'):             # nothing is armed any more
+            eng.submit_host(1, host, None, None)
+        return occ, flow, rec, rm.counters.cpu().numpy()
+
+    got, want = valid_frame(True), valid_frame(False)
+    assert torch.equal(got[0], want[0]) and torch.equal(got[1], want[1])
+    for k in KEYS:
+        assert torch.equal(got[2][k].view(torch.uint8), want[2][k].view(torch.uint8)), k
+    assert want[3][:N].sum() > 0                                                   # the frame was scored: gt_cnt
+    assert_counters(got[3], want[3], 'after the rejected calls')
+
+
 # ------------------------------------------------------------------------------------------------------------ 3. detector
 SCENES = [('scene-a', 0.0), ('scene-a', 2.5), ('scene-b', -1.0)]
 
