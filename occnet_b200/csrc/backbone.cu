@@ -133,16 +133,10 @@ int conv_gemm(occb200_backbone* e, const T* A, int64_t M, const ConvW& c, T* out
                            c.cout, c.kpad, act, st);
 }
 
-// Stride-1 3x3 convolutions (and 1x1 + residual) go through the TMA-im2col implicit-GEMM kernel conv2d_tc.cu (the default: it
-// skips the im2col round trip through memory); OCC_BACKBONE_IMPLICIT=0 selects the explicit im2col + gemm_tc path for everything.
-bool implicit_enabled()
-{
-    static const bool on = getenv("OCC_BACKBONE_IMPLICIT") == nullptr || atoi(getenv("OCC_BACKBONE_IMPLICIT")) != 0;
-    return on;
-}
-
-// one convolution on NHWC input [N, H, W, cin] -> out [N, Ho, Wo, cout].  `residual` (same shape as out) is only
-// accepted on the implicit-GEMM path, where the add (+ ReLU) is fused into the epilogue; fused_residual reports it.
+// one convolution on NHWC input [N, H, W, cin] -> out [N, Ho, Wo, cout].  On the tensor cores, stride-1 3x3 convolutions
+// (and 1x1 with a residual) go through the TMA-im2col implicit-GEMM kernel conv2d_tc.cu, which skips the im2col round trip
+// through memory; the others take explicit im2col + the GEMM.  `residual` (same shape as out) is only accepted on the
+// implicit-GEMM path, where the add (+ ReLU) is fused into the epilogue; fused_residual reports it.
 template <typename T>
 int conv(occb200_backbone* e, const T* in, int N, int H, int W, const ConvW& c, T* out, int act, int& Ho, int& Wo,
          cudaStream_t st, const T* residual = nullptr, bool* fused_residual = nullptr)
@@ -152,7 +146,7 @@ int conv(occb200_backbone* e, const T* in, int N, int H, int W, const ConvW& c, 
     const int64_t M = (int64_t)N * Ho * Wo;
     if (fused_residual) *fused_residual = false;
     if constexpr (sizeof(T) == 2) {
-        if (e->use_tc && implicit_enabled() && c.wh.p && c.stride == 1 && c.kpad == c.kh * c.kw * c.cin &&
+        if (e->use_tc && c.wh.p && c.stride == 1 && c.kpad == c.kh * c.kw * c.cin &&
             conv2d_tc_supported(c.cin, c.cout, c.kh, c.kw) && (c.kh == 3 || residual != nullptr)) {
             if (fused_residual) *fused_residual = residual != nullptr;
             e->launches++;
@@ -220,9 +214,7 @@ int forward_impl(occb200_backbone* e, const float* img, const uint8_t* frames, f
             if (last && s >= 1) dst = e->stage_out[s - 1].as<T>();           // C3 / C4 / C5 stay alive for the neck
             // conv3 (1x1): on the implicit-GEMM path the residual add + ReLU ride its epilogue and it writes `dst` directly
             bool fused = false;
-            if (implicit_enabled()) {
-                if (conv<T>(e, e->t2.as<T>(), N, h2, w2, blk.c3, dst, ACT_NONE, h3, w3, st, identity, &fused)) return 2;
-            }
+            if (conv<T>(e, e->t2.as<T>(), N, h2, w2, blk.c3, dst, ACT_NONE, h3, w3, st, identity, &fused)) return 2;
             if (!fused) {
                 if (conv<T>(e, e->t2.as<T>(), N, h2, w2, blk.c3, e->t3.as<T>(), ACT_NONE, h3, w3, st)) return 2;
                 if (launch_add_relu<T>(e->t3.as<T>(), identity, dst, (int64_t)N * h3 * w3 * blk.c3.cout, st)) return 2;

@@ -3,7 +3,6 @@
 //                             (+ residual[n, y, x, co]) ),      NHWC bf16 tensors, fp32 accumulation in registers.
 // Used for the 3x3 convolutions of ResNet-50 / FPN and (KH = KW = 1) for the bottleneck's last 1x1 convolution with the
 // residual add + ReLU fused (reference: mmdet ResNet / FPN as configured in bevformer_base_occ.py:48-66).
-// Default for the stride-1 convolutions of the backbone (OCC_BACKBONE_IMPLICIT=0: explicit im2col + gemm_tc for everything).
 //
 // Same skeleton as gemm_tc.cu (persistent, one CTA per SM, warp-specialised), with im2col done by TMA as in conv3d_tc.cu:
 //   M tile  = 128 output pixels = 8 rows x 16 columns of one image; K loop = taps x (Cin / 64)

@@ -13,6 +13,7 @@
 #include <cstring>
 #include <map>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/occ_b200.h"
@@ -92,6 +93,28 @@ struct PrevBev {
     bool writes_history = false;
 };
 
+// The kernel path of every frame, decided once at finalize from the precision, use_tensor_cores and the shapes
+// (make_frame_plan).  finalize builds exactly the buffers these fields call for and the frame reads only these fields; what
+// varies per frame is the previous BEV, the history write, taps, bev_embed and the input layout.
+struct FramePlan {
+    // bf16 storage + tensor cores: bf16 weight copies, the SCA value maps of every layer in one launch, and (with taps off)
+    // LayerNorm fused into the GEMM epilogues with the fp32 residual stream in the T32 layout and layer 0's operands built once
+    bool tc_bf16 = false;
+    // fp32 storage + tensor cores: GEMMs on bf16 [hi | lo] operand splits and [W_hi | W_hi | W_lo] weights (fp32-grade), the
+    // camera tokens split once per frame
+    bool tc_split = false;
+    // the sampling-offset / attention-logit projections write fp16 (half the bytes between the projection GEMM and the gather
+    // kernel; |offset| is a few pixels, so fp16's 11-bit mantissa keeps locations to < 0.01 px)
+    bool qproj_f16 = false;
+    // self mode on the fused path: layer 0's TSA + LayerNorm see only parameters and are computed once at finalize
+    // (OCC_NO_L0_FOLD=1 at finalize: recomputed every frame instead)
+    bool fold_layer0 = false;
+    // the two 3-D convolutions: CUDA cores, bf16 tensor cores, or three bf16-split tensor-core passes accumulated in fp32
+    enum Conv { CONV_SIMT, CONV_TC, CONV_SPLIT } conv = CONV_SIMT;
+    bool head_tc = false;               // occupancy + flow heads in one tensor-core kernel (concatenated weights)
+    bool lift_t32 = false;              // the shapes let the voxel lift read the T32 residual stream directly
+};
+
 }  // namespace
 }  // namespace occ
 
@@ -99,6 +122,7 @@ using namespace occ;
 
 struct occb200_engine {
     occb200_config cfg;
+    FramePlan plan;
     int Nq = 0, Nv = 0, C = 256;
     LevelGeom lg;
     ScaParams sp;
@@ -124,12 +148,10 @@ struct occb200_engine {
     std::map<std::string, std::vector<float>> host_params;
     std::vector<LayerW> layers;
     DevBuf bev_queries, pos, pos_t32, cams_embeds, level_embeds;
-    DevBuf pos_bf;                      // bev_pos as a bf16 row-major GEMM operand (folded TSA query projection)
     DevBuf qc_f32, qc_t, qc_pos_t;      // parameter-only layer-0 operands (query fp32 T32, bf16 query, bf16 query+pos), built once
     // Self mode (prev_bev = None): layer 0's TemporalSelfAttention + its LayerNorm see only parameters (bev_queries, bev_pos,
     // weights) -- the result is frame-independent and is computed ONCE at finalize by the same kernels (T32 fp32 + bf16 copy)
     DevBuf l0_x_f32, l0_q_t;
-    bool l0_ready = false;
     DevBuf conv_w[2], conv_b[2], conv_wh[2];
     DevBuf conv_wh_hi[2], conv_wh_lo[2], vox_split;      // fp32 storage + tensor cores: bf16 hi / lo split of the folded conv weights, [hi | lo] voxel operand
     DevBuf sca_v_all_wh, sca_v_all_b, sca_value_all;     // value_proj of every layer, concatenated (tensor-core path)
@@ -271,32 +293,46 @@ struct ProfScope {
     }
 };
 
-// ---- GEMM dispatch: tensor-core path for bf16 operands when enabled, CUDA-core path otherwise
+FramePlan make_frame_plan(const occb200_config& c, int Nq)
+{
+    const int C = 256;
+    FramePlan p;
+    p.tc_bf16 = c.precision == 1 && c.use_tensor_cores;
+    p.tc_split = c.precision == 0 && c.use_tensor_cores;
+    p.qproj_f16 = p.tc_bf16 && gemm_tc_supported(Nq, 2 * 8 * c.tsa_points * 3, 2 * C, C) &&
+                  gemm_tc_supported(Nq, 8 * c.num_levels * c.sca_points * 3, C, C);
+    p.fold_layer0 = p.tc_bf16 && getenv("OCC_NO_L0_FOLD") == nullptr;
+    if (p.tc_bf16 && c.pillar_h == 16) p.conv = FramePlan::CONV_TC;
+    if (p.tc_split && c.pillar_h == 16 && c.out_dim == 32) p.conv = FramePlan::CONV_SPLIT;
+    p.head_tc = p.conv == FramePlan::CONV_TC && c.out_dim == 32 && c.num_classes + 2 <= 19;
+    p.lift_t32 = p.tc_bf16 && c.pillar_h == 16;
+    return p;
+}
+
+// ---- GEMM dispatch: the plan's tensor-core path where the shape allows it, the CUDA-core path otherwise
 template <typename TA, typename TC>
 int gemm(occb200_engine* e, const TA* A, const TA* A2, int K1, const float* W, const void* Wh, const float* bias,
-         const float* residual, TC* C, int M, int N, int K, int act, cudaStream_t st)
+         const float* residual, TC* C, int M, int N, int K, int act, cudaStream_t st, const bf16* A_split = nullptr)
 {
     e->launches++;
     ProfScope ps(e, st, CAT_GEMM);
     if constexpr (sizeof(TA) == 2) {
-        if (e->cfg.use_tensor_cores && Wh != nullptr && gemm_tc_supported(M, N, K, A2 != nullptr ? K1 : K)) {
+        if (e->plan.tc_bf16 && gemm_tc_supported(M, N, K, A2 != nullptr ? K1 : K)) {
             return gemm_tc<TC>(reinterpret_cast<const bf16*>(A), reinterpret_cast<const bf16*>(A2), K1,
                                reinterpret_cast<const bf16*>(Wh), bias, residual, C, M, N, K, act, st);
         }
     }
     if constexpr (sizeof(TA) == 4 && std::is_same<TC, float>::value) {
         // fp32 storage + tensor cores: operand split into bf16 hi/lo, weights [W_hi | W_hi | W_lo], three passes in one
-        // wgmma GEMM (relative error ~2^-16: fp32-grade).  The camera tokens are split once per frame.
-        if (e->cfg.use_tensor_cores && e->cfg.precision == 0 && Wh != nullptr && e->split_ws.p != nullptr &&
-            gemm_tc_supported(M, N, 3 * K, 2 * K)) {
-            const bf16* S = e->split_ws.as<bf16>();
-            if ((const void*)A == e->tokens.p && A2 == nullptr && e->tokens_split.p != nullptr) {
-                S = e->tokens_split.as<bf16>();
-            } else {
+        // wgmma GEMM (relative error ~2^-16: fp32-grade).  `A_split`: A already split (the camera tokens, once per frame).
+        if (e->plan.tc_split && gemm_tc_supported(M, N, 3 * K, 2 * K)) {
+            const bf16* S = A_split;
+            if (S == nullptr) {
                 const int Ka = A2 ? K1 : K;
                 if (launch_split_bf16(reinterpret_cast<const float*>(A), Ka, reinterpret_cast<const float*>(A2), K - Ka, M,
                                       e->split_ws.as<bf16>(), st)) return 2;
                 e->launches++;
+                S = e->split_ws.as<bf16>();
             }
             return gemm_tc_split3(S, K, reinterpret_cast<const bf16*>(Wh), bias, residual, C, M, N, act, st);
         }
@@ -337,8 +373,6 @@ int build_tsa_query_values(occb200_engine* e)
     return 0;
 }
 
-enum { MODE_FRAME = 0, MODE_L0_TSA_ONLY = 1 };
-
 // torchvision's rotate(img, angle_deg, center=[cx, cy]) of a bev_h x bev_w image as the six grid coefficients its
 // _gen_affine_grid multiplies the base grid with, computed as torchvision computes them: _get_inverse_affine_matrix(center -
 // size / 2, -angle) in double (zero translation and shear, scale 1: [cos, sin, t0; -sin, cos, t1] about the centre), cast to
@@ -370,17 +404,25 @@ RotGrid rotation_grid(const occb200_engine* e, double angle_deg)
     return g;
 }
 
-// One frame from device feature levels in `layout` (input dtype 0, 1 or 2; see occb200_engine_set_input_dtype).  A frame
-// that writes the history has its last LayerNorm write its storage-type copy of the final BEV there.
+// The fp32 residual stream of a frame (T32 layout on the fused path).  `cur` is the stream; the next fused LayerNorm writes
+// `next`, which advance() makes the stream.  The stream may start on a parameter-only constant (layer 0's query, or its
+// folded TSA output) that is read and never written: `next` and `other` are the two workspace buffers it then alternates
+// between.  The unfused path writes each LayerNorm's output back into `cur` and uses `next` for the pre-LayerNorm sum.
+struct Residual {
+    float* cur;
+    float* next;
+    float* other;
+    void advance() { cur = next; std::swap(next, other); }
+};
+
+// ---- camera tokens (transformer_occ.py:207-227: +cams_embeds, +level_embeds, NCHW -> tokens) and, on the split path, their
+// bf16 [hi | lo] split, which every layer's SCA value GEMM reads
 template <typename T>
-int forward_impl(occb200_engine* e, const float* const* feats, int layout, const PrevBev& prev, const FrameOut& out,
-                 cudaStream_t st, int mode = MODE_FRAME)
+int pack_stage(occb200_engine* e, const float* const* feats, int layout, cudaStream_t st)
 {
-    const occb200_config& c = e->cfg;
-    const int Nq = e->Nq, Nv = e->Nv, C = 256, ncam = c.num_cams;
-    e->launches = 0;
+    const int C = 256, ncam = e->cfg.num_cams, Nv = e->Nv;
     T* tokens = e->tokens.as<T>();
-    if (mode == MODE_FRAME) {
+    {
         ProfScope ps(e, st, CAT_PACK);
         if (layout == 2) {
             if (launch_pack_levels_nhwc<T>(reinterpret_cast<const void* const*>(feats), e->lg, e->cams_embeds.as<float>(),
@@ -389,44 +431,254 @@ int forward_impl(occb200_engine* e, const float* const* feats, int layout, const
                                          e->level_embeds.as<float>(), ncam, C, Nv, tokens, st)) return 2;
         e->launches++;
     }
-    if constexpr (sizeof(T) == 4) {
-        if (mode == MODE_FRAME && c.use_tensor_cores && e->tokens_split.p != nullptr) {
-            ProfScope ps(e, st, CAT_PACK);
-            if (launch_split_bf16(reinterpret_cast<const float*>(tokens), C, nullptr, 0, (int64_t)ncam * Nv,
-                                  e->tokens_split.as<bf16>(), st)) return 2;
+    if (e->plan.tc_split) {
+        ProfScope ps(e, st, CAT_PACK);
+        if (launch_split_bf16(reinterpret_cast<const float*>(tokens), C, nullptr, 0, (int64_t)ncam * Nv,
+                              e->tokens_split.as<bf16>(), st)) return 2;
+        e->launches++;
+    }
+    return 0;
+}
+
+// ---- temporal self-attention of layer l (temporal_self_attention.py:177-272) and its LayerNorm.  q_in / q_pos_in: the
+// storage-type query and query + pos; the LayerNorm output goes to the stream and to y_t.  `fuse_ln`: LayerNorm in the GEMM
+// epilogues (the plan's tc_bf16 with taps off).  finalize runs layer 0 of self mode through here once to fold it.
+template <typename T>
+int tsa_stage(occb200_engine* e, bool fuse_ln, bool has_prev, int l, const T* q_in, const T* q_pos_in, Residual& rs, T* y_t,
+              cudaStream_t st)
+{
+    const int Nq = e->Nq, C = 256, nq_tsa = 2 * 8 * e->cfg.tsa_points * 3;     // offsets (x,y) + logits
+    const bool q_half = e->plan.qproj_f16;
+    LayerW& w = e->layers[l];
+    void* qproj = e->qproj.p;
+    T* attn_out = e->attn_out.as<T>();
+    // one value map per layer and frame: the current query's in self mode (queue 0 = queue 1), prev_bev's with a previous
+    // BEV, whose queue-1 map value_proj_l(bev_queries) was computed once at finalize.  The sampling projection reads the same
+    // operand (and query + pos).
+    const T* a_v = has_prev ? e->prev_t.as<T>() : q_in;
+    T* v_prev = e->tsa_value.as<T>();
+    const T* v_cur = has_prev ? e->tsa_v_query.as<T>() + (size_t)l * Nq * C : v_prev;
+    if (fuse_ln && q_half) {
+        // the value map + the sampling projection are independent GEMMs over [Nq,256] operands: ONE launch on disjoint CTA
+        // ranges.  Self mode: W1 q + W2 (q + pos) + b == (W1 + W2) q + [W2 pos + b], the bracket a parameter-only constant.
+        if constexpr (sizeof(T) == 2) {
+            const bf16* Av[1] = {reinterpret_cast<const bf16*>(a_v)};
+            bf16* Cv[1] = {reinterpret_cast<bf16*>(v_prev)};
+            ProfScope ps(e, st, CAT_GEMM);
+            const int rc = !has_prev
+                ? gemm_tc_tsa_inputs(Av, 1, w.tsa_v_wh.as<bf16>(), w.tsa_v_b.as<float>(), Cv, reinterpret_cast<const bf16*>(q_in),
+                                     nullptr, C, w.tsa_q_wh_fold.as<bf16>(), nullptr, w.tsa_q_const.as<float>(),
+                                     w.tsa_q_const_t32.as<float>(), (__half*)qproj, Nq, nq_tsa, C, st)
+                : gemm_tc_tsa_inputs(Av, 1, w.tsa_v_wh.as<bf16>(), w.tsa_v_b.as<float>(), Cv, reinterpret_cast<const bf16*>(a_v),
+                                     reinterpret_cast<const bf16*>(q_pos_in), C, w.tsa_q_wh.as<bf16>(), w.tsa_q_b.as<float>(),
+                                     nullptr, nullptr, (__half*)qproj, Nq, nq_tsa, 2 * C, st);
+            if (rc) return 2;
             e->launches++;
         }
+    } else {
+        if (gemm<T, T>(e, a_v, nullptr, 0, w.tsa_v_w.as<float>(), w.tsa_v_wh.p, w.tsa_v_b.as<float>(), nullptr, v_prev, Nq, C,
+                       C, ACT_NONE, st)) return 2;
+        const int rc = q_half ? gemm<T, __half>(e, a_v, q_pos_in, C, w.tsa_q_w.as<float>(), w.tsa_q_wh.p, w.tsa_q_b.as<float>(),
+                                                nullptr, (__half*)qproj, Nq, nq_tsa, 2 * C, ACT_NONE, st)
+                              : gemm<T, float>(e, a_v, q_pos_in, C, w.tsa_q_w.as<float>(), w.tsa_q_wh.p, w.tsa_q_b.as<float>(),
+                                               nullptr, (float*)qproj, Nq, nq_tsa, 2 * C, ACT_NONE, st);
+        if (rc) return 2;
     }
-    float* q_f32 = e->q_f32.as<float>();
-    float* x_f32 = e->x_f32.as<float>();
+    {
+        ProfScope ps(e, st, CAT_TSA);
+        if (launch_tsa_fused<T>(v_prev, v_cur, qproj, q_half, e->cfg.bev_h, e->cfg.bev_w, attn_out, st)) return 2;
+        e->launches++;
+    }
+    if (fuse_ln) {
+        if (gemm_ln_fused(e, (const bf16*)attn_out, w.tsa_o_wh.p, w.tsa_o_b.as<float>(), rs.cur, w.ln_g[0].as<float>(),
+                          w.ln_b[0].as<float>(), nullptr, rs.next, (bf16*)y_t, nullptr, Nq, C, st)) return 2;
+        rs.advance();
+        return 0;
+    }
+    if (gemm<T, float>(e, attn_out, nullptr, 0, w.tsa_o_w.as<float>(), w.tsa_o_wh.p, w.tsa_o_b.as<float>(), rs.cur, rs.next,
+                       Nq, C, C, ACT_NONE, st)) return 2;
+    if (e->taps)
+        OCC_CUDA(cudaMemcpyAsync(e->tap_tsa.as<float>() + (size_t)l * Nq * C, rs.next, (size_t)Nq * C * 4,
+                                 cudaMemcpyDeviceToDevice, st));
+    ProfScope ps(e, st, CAT_LN);
+    if (launch_layernorm<T>(rs.next, w.ln_g[0].as<float>(), w.ln_b[0].as<float>(), nullptr, Nq, C, rs.cur, y_t, (T*)nullptr,
+                            st)) return 2;
+    e->launches++;
+    return 0;
+}
+
+// ---- spatial cross-attention of layer l (spatial_cross_attention.py:128-175, :334-393) and its LayerNorm (into the stream
+// and q_t).  q_t_in: the storage-type query the sampling projection reads.
+template <typename T>
+int sca_stage(occb200_engine* e, bool fuse_ln, int l, const T* q_t_in, Residual& rs, cudaStream_t st)
+{
+    const int Nq = e->Nq, Nv = e->Nv, C = 256, ncam = e->cfg.num_cams;
+    const int nq_sca = 8 * e->cfg.num_levels * e->cfg.sca_points * 3;
+    const bool q_half = e->plan.qproj_f16;
+    LayerW& w = e->layers[l];
+    void* qproj = e->qproj.p;
+    T* q_t = e->q_t.as<T>();
+    T* attn_out = e->attn_out.as<T>();
+    const int rc = q_half ? gemm<T, __half>(e, q_t_in, nullptr, 0, w.sca_q_w.as<float>(), w.sca_q_wh.p, w.sca_q_b.as<float>(),
+                                            nullptr, (__half*)qproj, Nq, nq_sca, C, ACT_NONE, st)
+                          : gemm<T, float>(e, q_t_in, nullptr, 0, w.sca_q_w.as<float>(), w.sca_q_wh.p, w.sca_q_b.as<float>(),
+                                           nullptr, (float*)qproj, Nq, nq_sca, C, ACT_NONE, st);
+    if (rc) return 2;
+    const T* sca_val = e->sca_value.as<T>();
+    if (e->plan.tc_bf16) {                  // this layer's slice of the value maps the frame computed for every layer
+        sca_val = reinterpret_cast<const T*>(e->sca_value_all.as<bf16>() + (size_t)l * ncam * Nv * C);
+    } else if (gemm<T, T>(e, e->tokens.as<T>(), nullptr, 0, w.sca_v_w.as<float>(), w.sca_v_wh.p, w.sca_v_b.as<float>(), nullptr,
+                          e->sca_value.as<T>(), ncam * Nv, C, C, ACT_NONE, st,
+                          e->plan.tc_split ? e->tokens_split.as<bf16>() : nullptr)) return 2;
+    {
+        ProfScope ps(e, st, CAT_SCA);
+        if (launch_sca_fused<T>(sca_val, qproj, q_half, e->sp, e->lg, Nv, attn_out, e->hits.as<uint8_t>(), st)) return 2;
+        e->launches++;
+    }
+    if (fuse_ln) {
+        if (gemm_ln_fused(e, (const bf16*)attn_out, w.sca_o_wh.p, w.sca_o_b.as<float>(), rs.cur, w.ln_g[1].as<float>(),
+                          w.ln_b[1].as<float>(), nullptr, rs.next, (bf16*)q_t, nullptr, Nq, C, st)) return 2;
+        rs.advance();
+        return 0;
+    }
+    if (gemm<T, float>(e, attn_out, nullptr, 0, w.sca_o_w.as<float>(), w.sca_o_wh.p, w.sca_o_b.as<float>(), rs.cur, rs.next,
+                       Nq, C, C, ACT_NONE, st)) return 2;
+    if (e->taps)
+        OCC_CUDA(cudaMemcpyAsync(e->tap_sca.as<float>() + (size_t)l * Nq * C, rs.next, (size_t)Nq * C * 4,
+                                 cudaMemcpyDeviceToDevice, st));
+    ProfScope ps(e, st, CAT_LN);
+    if (launch_layernorm<T>(rs.next, w.ln_g[1].as<float>(), w.ln_b[1].as<float>(), nullptr, Nq, C, rs.cur, q_t, (T*)nullptr,
+                            st)) return 2;
+    e->launches++;
+    return 0;
+}
+
+// ---- FFN of layer l (mmcv FFN: x + W2 relu(W1 x)) and its LayerNorm: into the stream, y_t and (for the next layer's
+// unfolded TSA query projection) q_pos_t
+template <typename T>
+int ffn_stage(occb200_engine* e, bool fuse_ln, bool has_prev, int l, Residual& rs, T* y_t, cudaStream_t st)
+{
+    const int Nq = e->Nq, C = 256, F = e->cfg.ffn_dim;
+    LayerW& w = e->layers[l];
     T* q_t = e->q_t.as<T>();
     T* q_pos_t = e->q_pos_t.as<T>();
-    const float* pos = e->pos.as<float>();
-    // tensor-core path: LayerNorm is fused into the GEMM epilogues and the fp32 residual stream lives in the T32 layout
-    const bool fuse_ln = sizeof(T) == 2 && c.use_tensor_cores && !e->taps && e->pos_t32.p != nullptr &&
-                         e->layers[0].tsa_o_wh.p != nullptr;
-    // Layer-0 operands.  On the fused tensor-core path they were built once at finalize (parameters only); the
-    // residual stream then rotates through {constant, q_f32, x_f32} without ever writing the constant buffer.
-    const bool const_q = fuse_ln && e->qc_f32.p != nullptr;
-    const float* cbuf = const_q ? e->qc_f32.as<float>() : nullptr;     // the constant buffer in the rotation (never written)
-    float* spare_f32 = nullptr;
-    const T* q_in = q_t;                    // bf16/fp32 operand copy of the current query
-    const T* q_pos_in = q_pos_t;            // ... of query + pos
-    if (const_q) {
-        q_in = e->qc_t.as<T>(); q_pos_in = e->qc_pos_t.as<T>();
-        spare_f32 = x_f32; x_f32 = q_f32; q_f32 = e->qc_f32.as<float>();     // q_f32 is only READ until advance()
+    if (gemm<T, T>(e, q_t, nullptr, 0, w.ffn1_w.as<float>(), w.ffn1_wh.p, w.ffn1_b.as<float>(), nullptr, e->ffn_h.as<T>(), Nq, F,
+                   C, ACT_RELU, st)) return 2;
+    if (fuse_ln) {
+        // self mode with the merged TSA launch folds pos into a constant: no LayerNorm has to write q + pos
+        const bool need_qpos = has_prev || !e->plan.qproj_f16;
+        if (gemm_ln_fused(e, e->ffn_h.as<bf16>(), w.ffn2_wh.p, w.ffn2_b.as<float>(), rs.cur, w.ln_g[2].as<float>(),
+                          w.ln_b[2].as<float>(), need_qpos ? e->pos_t32.as<float>() : nullptr, rs.next, (bf16*)y_t,
+                          need_qpos ? (bf16*)q_pos_t : nullptr, Nq, F, st)) return 2;
+        rs.advance();
+        return 0;
+    }
+    if (gemm<T, float>(e, e->ffn_h.as<T>(), nullptr, 0, w.ffn2_w.as<float>(), w.ffn2_wh.p, w.ffn2_b.as<float>(), rs.cur, rs.next,
+                       Nq, C, F, ACT_NONE, st)) return 2;
+    ProfScope ps(e, st, CAT_LN);
+    if (launch_layernorm<T>(rs.next, w.ln_g[2].as<float>(), w.ln_b[2].as<float>(), e->pos.as<float>(), Nq, C, rs.cur, y_t,
+                            q_pos_t, st)) return 2;
+    e->launches++;
+    return 0;
+}
+
+// ---- the final BEV to bev_embed, then the voxel decoder and heads (transformer_occ.py:305-319, bevformer_occ_head.py:211-212)
+template <typename T>
+int decode_stage(occb200_engine* e, bool fuse_ln, Residual& rs, const FrameOut& out, cudaStream_t st)
+{
+    const occb200_config& c = e->cfg;
+    const FramePlan& p = e->plan;
+    const int Nq = e->Nq, C = 256, X = c.bev_w, Y = c.bev_h, Z = c.pillar_h, mid = C / Z;
+    const int64_t nvox = (int64_t)X * Y * Z;
+    // the voxel lift reads the T32 residual stream directly when bev_embed itself is not an output (one kernel instead of two)
+    const bool lift_from_t32 = fuse_ln && p.lift_t32 && out.bev_embed == nullptr;
+    if (fuse_ln && !lift_from_t32) {                               // back to row-major for the outputs / voxel decoder
+        ProfScope ps(e, st, CAT_PACK);
+        if (launch_t32_convert(rs.cur, rs.next, Nq, 1, st)) return 2;
+        e->launches++;
+        rs.advance();
+    }
+    if (out.bev_embed)
+        OCC_CUDA(cudaMemcpyAsync(out.bev_embed, rs.cur, (size_t)Nq * C * 4, cudaMemcpyDeviceToDevice, st));
+    if (!out.occ_logits && !out.flow && !out.cls_u8 && !out.cls_i64) return 0;
+    {
+        ProfScope ps(e, st, CAT_VOX);
+        if (lift_from_t32) {
+            if (launch_t32_to_voxel(rs.cur, c.bev_h, c.bev_w, e->vox0.as<bf16>(), st)) return 2;
+        } else if (launch_bev_to_voxel<T>(rs.cur, c.bev_h, c.bev_w, Z, mid, e->vox0.as<T>(), st)) return 2;
+        e->launches++;
+    }
+    if (p.conv == FramePlan::CONV_SPLIT) {
+        ProfScope ps(e, st, CAT_CONV);
+        if (launch_split_bf16(e->vox0.as<float>(), mid, nullptr, 0, nvox, e->vox_split.as<bf16>(), st)) return 2;
+        e->launches++;
+        if (launch_conv3d_tc_split(e->vox_split.as<bf16>(), e->conv_wh_hi[0].as<bf16>(), e->conv_wh_lo[0].as<bf16>(),
+                                   e->conv_b[0].as<float>(), X, Y, Z, mid, e->vox1.as<float>(), st)) return 2;
+        e->launches += 3;                                           // the launcher's three passes
+        if (launch_split_bf16(e->vox1.as<float>(), c.out_dim, nullptr, 0, nvox, e->vox_split.as<bf16>(), st)) return 2;
+        e->launches++;
+        if (launch_conv3d_tc_split(e->vox_split.as<bf16>(), e->conv_wh_hi[1].as<bf16>(), e->conv_wh_lo[1].as<bf16>(),
+                                   e->conv_b[1].as<float>(), X, Y, Z, c.out_dim, e->vox2.as<float>(), st)) return 2;
+        e->launches += 3;
+    } else {
+        const bool tc = p.conv == FramePlan::CONV_TC;
+        {
+            ProfScope ps(e, st, CAT_CONV);
+            if (tc) {
+                if (launch_conv3d_tc(e->vox0.as<bf16>(), e->conv_wh[0].as<bf16>(), e->conv_b[0].as<float>(), X, Y, Z, mid,
+                                     e->vox1.as<bf16>(), st)) return 2;
+            } else if (launch_conv3d_simt<T>(e->vox0.as<T>(), e->conv_w[0].as<float>(), e->conv_b[0].as<float>(), X, Y, Z,
+                                             mid, e->vox1.as<T>(), st)) return 2;
+            e->launches++;
+        }
+        ProfScope ps(e, st, CAT_CONV);
+        if (tc) {
+            if (launch_conv3d_tc(e->vox1.as<bf16>(), e->conv_wh[1].as<bf16>(), e->conv_b[1].as<float>(), X, Y, Z, c.out_dim,
+                                 e->vox2.as<bf16>(), st)) return 2;
+        } else if (launch_conv3d_simt<T>(e->vox1.as<T>(), e->conv_w[1].as<float>(), e->conv_b[1].as<float>(), X, Y, Z,
+                                         c.out_dim, e->vox2.as<T>(), st)) return 2;
+        e->launches++;
+    }
+    ProfScope ps(e, st, CAT_HEAD);
+    if (p.head_tc) {
+        if (launch_occ_head_tc(e->vox2.as<bf16>(), e->head_w1h.as<bf16>(), e->head_w2h.as<bf16>(), e->head_b1c.as<float>(),
+                               e->head_b2c.as<float>(), c.num_classes, nvox, out.occ_logits, out.flow, out.cls_u8,
+                               out.cls_i64, st)) return 2;
+    } else {
+        const HeadWeights hw{e->hw1.as<float>(), e->hb1.as<float>(), e->hw2.as<float>(), e->hb2.as<float>(),
+                             e->fw1.as<float>(), e->fb1.as<float>(), e->fw2.as<float>(), e->fb2.as<float>(), c.num_classes};
+        if (launch_occ_head<T>(e->vox2.as<T>(), hw, nvox, out.occ_logits, out.flow, out.cls_u8, out.cls_i64, st)) return 2;
+    }
+    e->launches++;
+    return 0;
+}
+
+// One frame from device feature levels in `layout` (input dtype 0, 1 or 2; see occb200_engine_set_input_dtype).  A frame
+// that writes the history has its last LayerNorm write its storage-type copy of the final BEV there.
+template <typename T>
+int forward_impl(occb200_engine* e, const float* const* feats, int layout, const PrevBev& prev, const FrameOut& out,
+                 cudaStream_t st)
+{
+    const occb200_config& c = e->cfg;
+    const int Nq = e->Nq, Nv = e->Nv, C = 256;
+    const bool fuse_ln = e->plan.tc_bf16 && !e->taps;
+    const bool has_prev = prev.src != PrevBev::NONE;
+    const bool fold_l0 = fuse_ln && !has_prev && e->plan.fold_layer0;
+    T* q_t = e->q_t.as<T>();
+    T* q_pos_t = e->q_pos_t.as<T>();
+    e->launches = 0;
+    if (pack_stage<T>(e, feats, layout, st)) return 2;
+    // Layer-0 operands.  On the fused path they were built once at finalize (parameters only), and so was layer 0's TSA output
+    // when it is folded: the stream starts on that constant.
+    Residual rs{e->q_f32.as<float>(), e->x_f32.as<float>(), e->q_f32.as<float>()};
+    if (fuse_ln) {
+        rs = {fold_l0 ? e->l0_x_f32.as<float>() : e->qc_f32.as<float>(), e->q_f32.as<float>(), e->x_f32.as<float>()};
     } else {
         ProfScope ps(e, st, CAT_PACK);
-        if (launch_prepare_query<T>(e->bev_queries.as<float>(), pos, (int64_t)Nq * C, q_f32, q_t, q_pos_t, fuse_ln ? 1 : 0,
+        if (launch_prepare_query<T>(e->bev_queries.as<float>(), e->pos.as<float>(), (int64_t)Nq * C, rs.cur, q_t, q_pos_t, 0,
                                     st)) return 2;
         e->launches++;
     }
-    auto advance = [&]() {                  // the LayerNorm output just written to x_f32 becomes the residual stream
-        float* old = q_f32;
-        q_f32 = x_f32;
-        x_f32 = (old == cbuf) ? spare_f32 : old;
-    };
-    const bool has_prev = prev.src != PrevBev::NONE;
     if (has_prev) {
         // encoder.py:204-209: value = stack([prev_bev, bev_query]) built ONCE before the layer loop, so
         // queue 1 keeps seeing the layer-0 query in every layer.
@@ -440,227 +692,29 @@ int forward_impl(occb200_engine* e, const float* const* feats, int layout, const
             return 2;
         e->launches++;
     }
-    // sampling offsets / attention logits: fp16 on the tensor-core path (half the bytes between the projection GEMM and
-    // the gather kernel; |offset| is a few pixels, so fp16's 11-bit mantissa keeps locations to < 0.01 px), fp32 otherwise
-    const int nq_tsa = 2 * 8 * c.tsa_points * 3;   // offsets (x,y) + logits
-    const int nq_sca = 8 * c.num_levels * c.sca_points * 3;
-    const bool q_half = sizeof(T) == 2 && c.use_tensor_cores && e->layers[0].tsa_q_wh.p != nullptr &&
-                        e->layers[0].sca_q_wh.p != nullptr && gemm_tc_supported(Nq, nq_tsa, 2 * C, C) &&
-                        gemm_tc_supported(Nq, nq_sca, C, C);
-    void* qproj = e->qproj.p;
-    T* attn_out = e->attn_out.as<T>();
-    const bool hoist_v = sizeof(T) == 2 && c.use_tensor_cores && e->sca_value_all.p != nullptr;
-    // layer-0 TSA + LayerNorm folded into a constant (self mode only; OCC_NO_L0_FOLD=1 recomputes it every frame)
-    const bool l0_fold = mode == MODE_FRAME && const_q && !has_prev && e->l0_ready;
-    const T* q_t_in = q_t;                  // A operand of the SCA query projection (= the TSA LayerNorm output)
-    if (hoist_v && mode == MODE_FRAME) {
-        e->launches++;
+    if (e->plan.tc_bf16) {
+        // SpatialCrossAttention's value_proj input (the camera tokens) does not depend on the layer
+        // (spatial_cross_attention.py:334): every layer's value map in one launch
         ProfScope ps(e, st, CAT_GEMM);
-        if (gemm_tc_blocked256((const bf16*)tokens, e->sca_v_all_wh.as<bf16>(), e->sca_v_all_b.as<float>(),
-                               e->sca_value_all.as<bf16>(), ncam * Nv, c.num_layers * C, C, st)) return 2;
-    }
-    for (int l = 0; l < c.num_layers; ++l) {
-        LayerW& w = e->layers[l];
-        // self mode (prev_bev = None): W1 q + W2 (q + pos) = (W1 + W2) q + W2 pos -- the second operand is the CONSTANT
-        // bf16 pos, so no layer has to write (and the FFN LayerNorm epilogue has to read pos for) a bf16 copy of q + pos
-        const bool fold_pos = fuse_ln && !has_prev && w.tsa_q_wh_fold.p != nullptr && w.tsa_q_const.p != nullptr && q_half;
-        // ---- temporal self-attention (temporal_self_attention.py:177-272)
-        if (l == 0 && l0_fold) {
-            // precomputed at finalize: residual stream := constant T32 buffer, SCA projection operand := constant bf16 copy
-            q_f32 = e->l0_x_f32.as<float>(); x_f32 = e->q_f32.as<float>(); spare_f32 = e->x_f32.as<float>();
-            cbuf = q_f32;
-            q_t_in = e->l0_q_t.as<T>();
-            q_in = q_t; q_pos_in = q_pos_t;
-        } else {
-            // one value map per layer and frame: the current query's in self mode (queue 0 = queue 1), prev_bev's with a
-            // previous BEV, whose queue-1 map value_proj_l(bev_queries) was computed once at finalize
-            const T* a_v = has_prev ? e->prev_t.as<T>() : q_in;
-            T* v_prev = e->tsa_value.as<T>();
-            const T* v_cur = has_prev ? e->tsa_v_query.as<T>() + (size_t)l * Nq * C : v_prev;
-            // the value map + the sampling projection are independent GEMMs over [Nq,256] operands: ONE launch on disjoint
-            // CTA ranges on the fused tensor-core path, one launch each otherwise
-            const bool tsa_merge = sizeof(T) == 2 && fuse_ln && q_half && w.tsa_v_wh.p != nullptr;
-            if (tsa_merge) {
-                if constexpr (sizeof(T) == 2) {
-                    const bf16* Av[1] = {reinterpret_cast<const bf16*>(a_v)};
-                    bf16* Cv[1] = {reinterpret_cast<bf16*>(v_prev)};
-                    e->launches++;
-                    ProfScope ps(e, st, CAT_GEMM);
-                    const int rc = fold_pos
-                        ? gemm_tc_tsa_inputs(Av, 1, w.tsa_v_wh.as<bf16>(), w.tsa_v_b.as<float>(), Cv, reinterpret_cast<const bf16*>(q_in),
-                                             nullptr, C, w.tsa_q_wh_fold.as<bf16>(), nullptr, w.tsa_q_const.as<float>(),
-                                             w.tsa_q_const_t32.as<float>(), (__half*)qproj, Nq, nq_tsa, C, st)
-                        : gemm_tc_tsa_inputs(Av, 1, w.tsa_v_wh.as<bf16>(), w.tsa_v_b.as<float>(), Cv,
-                                             reinterpret_cast<const bf16*>(has_prev ? e->prev_t.as<T>() : q_in),
-                                             reinterpret_cast<const bf16*>(q_pos_in), C, w.tsa_q_wh.as<bf16>(), w.tsa_q_b.as<float>(),
-                                             nullptr, nullptr, (__half*)qproj, Nq, nq_tsa, 2 * C, st);
-                    if (rc) return 2;
-                }
-            } else {
-                auto value_gemm = [&](const T* a, T* dst) {
-                    return gemm<T, T>(e, a, nullptr, 0, w.tsa_v_w.as<float>(), w.tsa_v_wh.p, w.tsa_v_b.as<float>(), nullptr, dst,
-                                      Nq, C, C, ACT_NONE, st);
-                };
-                if (value_gemm(a_v, v_prev)) return 2;
-                const T* qa = has_prev ? e->prev_t.as<T>() : q_in;
-                const int rc = q_half ? gemm<T, __half>(e, qa, q_pos_in, C, w.tsa_q_w.as<float>(), w.tsa_q_wh.p, w.tsa_q_b.as<float>(),
-                                                        nullptr, (__half*)qproj, Nq, nq_tsa, 2 * C, ACT_NONE, st)
-                                      : gemm<T, float>(e, qa, q_pos_in, C, w.tsa_q_w.as<float>(), w.tsa_q_wh.p, w.tsa_q_b.as<float>(),
-                                                       nullptr, (float*)qproj, Nq, nq_tsa, 2 * C, ACT_NONE, st);
-                if (rc) return 2;
-            }
-            {
-                ProfScope ps(e, st, CAT_TSA);
-                if (launch_tsa_fused<T>(v_prev, v_cur, qproj, q_half, c.bev_h, c.bev_w, attn_out, st)) return 2;
-            }
-            e->launches++;
-            if (fuse_ln) {
-                float* y32 = mode == MODE_L0_TSA_ONLY ? e->l0_x_f32.as<float>() : x_f32;
-                bf16* y16 = mode == MODE_L0_TSA_ONLY ? e->l0_q_t.as<bf16>() : (bf16*)q_t;
-                if (gemm_ln_fused(e, (const bf16*)attn_out, w.tsa_o_wh.p, w.tsa_o_b.as<float>(), q_f32, w.ln_g[0].as<float>(),
-                                  w.ln_b[0].as<float>(), nullptr, y32, y16, nullptr, Nq, C, st)) return 2;
-                if (mode == MODE_L0_TSA_ONLY) return 0;
-                advance();
-                q_in = q_t; q_pos_in = q_pos_t;
-            } else {
-                if (gemm<T, float>(e, attn_out, nullptr, 0, w.tsa_o_w.as<float>(), w.tsa_o_wh.p, w.tsa_o_b.as<float>(),
-                                   q_f32, x_f32, Nq, C, C, ACT_NONE, st)) return 2;
-                if (e->taps)
-                    OCC_CUDA(cudaMemcpyAsync(e->tap_tsa.as<float>() + (size_t)l * Nq * C, x_f32, (size_t)Nq * C * 4,
-                                             cudaMemcpyDeviceToDevice, st));
-                {
-                    ProfScope ps(e, st, CAT_LN);
-                    if (launch_layernorm<T>(x_f32, w.ln_g[0].as<float>(), w.ln_b[0].as<float>(), nullptr, Nq, C, q_f32, q_t,
-                                            (T*)nullptr, st)) return 2;
-                }
-                e->launches++;
-            }
-        }
-        // ---- spatial cross-attention (spatial_cross_attention.py:128-175, :334-393)
-        const int rc = q_half ? gemm<T, __half>(e, q_t_in, nullptr, 0, w.sca_q_w.as<float>(), w.sca_q_wh.p, w.sca_q_b.as<float>(),
-                                                nullptr, (__half*)qproj, Nq, nq_sca, C, ACT_NONE, st)
-                              : gemm<T, float>(e, q_t_in, nullptr, 0, w.sca_q_w.as<float>(), w.sca_q_wh.p, w.sca_q_b.as<float>(),
-                                               nullptr, (float*)qproj, Nq, nq_sca, C, ACT_NONE, st);
-        if (rc) return 2;
-        q_t_in = q_t;
-        const T* sca_val = e->sca_value.as<T>();
-        if (hoist_v) {
-            sca_val = reinterpret_cast<const T*>(e->sca_value_all.as<bf16>() + (size_t)l * ncam * Nv * C);
-        } else if (gemm<T, T>(e, tokens, nullptr, 0, w.sca_v_w.as<float>(), w.sca_v_wh.p, w.sca_v_b.as<float>(), nullptr,
-                              e->sca_value.as<T>(), ncam * Nv, C, C, ACT_NONE, st)) return 2;
-        {
-            ProfScope ps(e, st, CAT_SCA);
-            if (launch_sca_fused<T>(sca_val, qproj, q_half, e->sp, e->lg, Nv, attn_out, e->hits.as<uint8_t>(), st)) return 2;
-        }
+        if (gemm_tc_blocked256(e->tokens.as<bf16>(), e->sca_v_all_wh.as<bf16>(), e->sca_v_all_b.as<float>(),
+                               e->sca_value_all.as<bf16>(), c.num_cams * Nv, c.num_layers * C, C, st)) return 2;
         e->launches++;
-        if (fuse_ln) {
-            if (gemm_ln_fused(e, (const bf16*)attn_out, w.sca_o_wh.p, w.sca_o_b.as<float>(), q_f32, w.ln_g[1].as<float>(),
-                              w.ln_b[1].as<float>(), nullptr, x_f32, (bf16*)q_t, nullptr, Nq, C, st)) return 2;
-            advance();
-        } else {
-            if (gemm<T, float>(e, attn_out, nullptr, 0, w.sca_o_w.as<float>(), w.sca_o_wh.p, w.sca_o_b.as<float>(),
-                               q_f32, x_f32, Nq, C, C, ACT_NONE, st)) return 2;
-            if (e->taps)
-                OCC_CUDA(cudaMemcpyAsync(e->tap_sca.as<float>() + (size_t)l * Nq * C, x_f32, (size_t)Nq * C * 4,
-                                         cudaMemcpyDeviceToDevice, st));
-            {
-                ProfScope ps(e, st, CAT_LN);
-                if (launch_layernorm<T>(x_f32, w.ln_g[1].as<float>(), w.ln_b[1].as<float>(), nullptr, Nq, C, q_f32, q_t,
-                                        (T*)nullptr, st)) return 2;
-            }
-            e->launches++;
-        }
-        // ---- FFN (mmcv FFN: x + W2 relu(W1 x))
-        if (gemm<T, T>(e, q_t, nullptr, 0, w.ffn1_w.as<float>(), w.ffn1_wh.p, w.ffn1_b.as<float>(), nullptr,
-                       e->ffn_h.as<T>(), Nq, c.ffn_dim, C, ACT_RELU, st)) return 2;
+    }
+    // per encoder layer (encoder.py:356-404): self_attn, norm, cross_attn, norm, ffn, norm
+    for (int l = 0; l < c.num_layers; ++l) {
+        const bool l0_const = fuse_ln && l == 0;          // layer 0 reads the operands built at finalize
+        if (!(l == 0 && fold_l0) &&
+            tsa_stage<T>(e, fuse_ln, has_prev, l, l0_const ? e->qc_t.as<T>() : q_t, l0_const ? e->qc_pos_t.as<T>() : q_pos_t,
+                         rs, q_t, st)) return 2;
+        if (sca_stage<T>(e, fuse_ln, l, l == 0 && fold_l0 ? e->l0_q_t.as<T>() : q_t, rs, st)) return 2;
         // a video frame's last LayerNorm writes its storage-type copy straight into the history (q_t is not read afterwards)
         T* y_t = prev.writes_history && l == c.num_layers - 1 ? e->hist.as<T>() : q_t;
-        if (fuse_ln) {
-            const bool need_qpos = !fold_pos;                // only the unfolded TSA query projection reads q + pos
-            if (gemm_ln_fused(e, e->ffn_h.as<bf16>(), w.ffn2_wh.p, w.ffn2_b.as<float>(), q_f32, w.ln_g[2].as<float>(),
-                              w.ln_b[2].as<float>(), need_qpos ? e->pos_t32.as<float>() : nullptr, x_f32, (bf16*)y_t,
-                              need_qpos ? (bf16*)q_pos_t : nullptr, Nq, c.ffn_dim, st))
-                return 2;
-            advance();
-        } else {
-            if (gemm<T, float>(e, e->ffn_h.as<T>(), nullptr, 0, w.ffn2_w.as<float>(), w.ffn2_wh.p, w.ffn2_b.as<float>(),
-                               q_f32, x_f32, Nq, C, c.ffn_dim, ACT_NONE, st)) return 2;
-            {
-                ProfScope ps(e, st, CAT_LN);
-                if (launch_layernorm<T>(x_f32, w.ln_g[2].as<float>(), w.ln_b[2].as<float>(), pos, Nq, C, q_f32, y_t,
-                                        q_pos_t, st)) return 2;
-            }
-            e->launches++;
-        }
+        if (ffn_stage<T>(e, fuse_ln, has_prev, l, rs, y_t, st)) return 2;
         if (e->taps)
-            OCC_CUDA(cudaMemcpyAsync(e->tap_layer.as<float>() + (size_t)l * Nq * C, q_f32, (size_t)Nq * C * 4,
+            OCC_CUDA(cudaMemcpyAsync(e->tap_layer.as<float>() + (size_t)l * Nq * C, rs.cur, (size_t)Nq * C * 4,
                                      cudaMemcpyDeviceToDevice, st));
     }
-    const int X = c.bev_w, Y = c.bev_h, Z = c.pillar_h, mid = C / Z;
-    // the voxel lift reads the T32 residual stream directly when bev_embed itself is not an output (one kernel instead of two)
-    const bool lift_from_t32 = fuse_ln && sizeof(T) == 2 && out.bev_embed == nullptr && Z == 16 && mid == 16;
-    if (fuse_ln && !lift_from_t32) {                               // back to row-major for the outputs / voxel decoder
-        ProfScope ps(e, st, CAT_PACK);
-        if (launch_t32_convert(q_f32, x_f32, Nq, 1, st)) return 2;
-        advance();
-        e->launches++;
-    }
-    if (out.bev_embed)
-        OCC_CUDA(cudaMemcpyAsync(out.bev_embed, q_f32, (size_t)Nq * C * 4, cudaMemcpyDeviceToDevice, st));
-    if (!out.occ_logits && !out.flow && !out.cls_u8 && !out.cls_i64) return 0;
-    // ---- voxel decoder + heads
-    {
-        ProfScope ps(e, st, CAT_VOX);
-        if (lift_from_t32) {
-            if (launch_t32_to_voxel(q_f32, c.bev_h, c.bev_w, e->vox0.as<bf16>(), st)) return 2;
-        } else if (launch_bev_to_voxel<T>(q_f32, c.bev_h, c.bev_w, Z, mid, e->vox0.as<T>(), st)) return 2;
-    }
-    const bool conv_tc = sizeof(T) == 2 && c.use_tensor_cores && e->conv_wh[0].p && e->conv_wh[1].p && Z == 16;
-    // fp32 storage + tensor cores: both convolutions as three bf16-split passes accumulated in fp32
-    const bool conv_split = sizeof(T) == 4 && c.use_tensor_cores && e->conv_wh_hi[0].p && e->conv_wh_lo[1].p &&
-                            e->vox_split.p && Z == 16 && (mid == 16 || mid == 32) && c.out_dim == 32;
-    if (conv_split) {
-        const int64_t nv = (int64_t)X * Y * Z;
-        ProfScope ps(e, st, CAT_CONV);
-        if (launch_split_bf16(e->vox0.as<float>(), mid, nullptr, 0, nv, e->vox_split.as<bf16>(), st)) return 2;
-        if (launch_conv3d_tc_split(e->vox_split.as<bf16>(), e->conv_wh_hi[0].as<bf16>(), e->conv_wh_lo[0].as<bf16>(), e->conv_b[0].as<float>(),
-                                   X, Y, Z, mid, e->vox1.as<float>(), st)) return 2;
-        if (launch_split_bf16(e->vox1.as<float>(), c.out_dim, nullptr, 0, nv, e->vox_split.as<bf16>(), st)) return 2;
-        if (launch_conv3d_tc_split(e->vox_split.as<bf16>(), e->conv_wh_hi[1].as<bf16>(), e->conv_wh_lo[1].as<bf16>(), e->conv_b[1].as<float>(),
-                                   X, Y, Z, c.out_dim, e->vox2.as<float>(), st)) return 2;
-        e->launches += 6;                                       // (+ the 2 counted below = 2 splits + 6 conv passes)
-    } else {
-    {
-        ProfScope ps(e, st, CAT_CONV);
-        if (conv_tc) {
-            if (launch_conv3d_tc(e->vox0.as<bf16>(), e->conv_wh[0].as<bf16>(), e->conv_b[0].as<float>(), X, Y, Z, mid,
-                                 e->vox1.as<bf16>(), st)) return 2;
-        } else if (launch_conv3d_simt<T>(e->vox0.as<T>(), e->conv_w[0].as<float>(), e->conv_b[0].as<float>(), X, Y, Z,
-                                         mid, e->vox1.as<T>(), st)) return 2;
-    }
-    {
-        ProfScope ps(e, st, CAT_CONV);
-        if (conv_tc) {
-            if (launch_conv3d_tc(e->vox1.as<bf16>(), e->conv_wh[1].as<bf16>(), e->conv_b[1].as<float>(), X, Y, Z,
-                                 c.out_dim, e->vox2.as<bf16>(), st)) return 2;
-        } else if (launch_conv3d_simt<T>(e->vox1.as<T>(), e->conv_w[1].as<float>(), e->conv_b[1].as<float>(), X, Y, Z,
-                                         c.out_dim, e->vox2.as<T>(), st)) return 2;
-    }
-    }   // (!conv_split)
-    HeadWeights hw{e->hw1.as<float>(), e->hb1.as<float>(), e->hw2.as<float>(), e->hb2.as<float>(),
-                   e->fw1.as<float>(), e->fb1.as<float>(), e->fw2.as<float>(), e->fb2.as<float>(), c.num_classes};
-    {
-        ProfScope ps(e, st, CAT_HEAD);
-        if (conv_tc && e->head_w1h.p) {
-            if (launch_occ_head_tc(e->vox2.as<bf16>(), e->head_w1h.as<bf16>(), e->head_w2h.as<bf16>(),
-                                   e->head_b1c.as<float>(), e->head_b2c.as<float>(), c.num_classes, (int64_t)X * Y * Z,
-                                   out.occ_logits, out.flow, out.cls_u8, out.cls_i64, st)) return 2;
-        } else if (launch_occ_head<T>(e->vox2.as<T>(), hw, (int64_t)X * Y * Z, out.occ_logits, out.flow, out.cls_u8,
-                                      out.cls_i64, st))
-            return 2;
-    }
-    e->launches += 4;
-    return 0;
+    return decode_stage<T>(e, fuse_ln, rs, out, st);
 }
 
 // A backbone the engine can drive for input dtype 3: finalized, one image per camera, the engine's level shapes, frames set.
@@ -1007,7 +1061,6 @@ int occb200_engine_load_param(occb200_engine* e, const char* key, const float* d
     if (!ok) { set_last_error("unknown parameter key: " + k); return 3; }
     e->host_params[k].assign(data, data + numel);
     e->finalized = false;
-    e->l0_ready = false;
     return 0;
 }
 
@@ -1016,8 +1069,8 @@ int occb200_engine_finalize(occb200_engine* e)
     OCC_CHECK(e, "null engine");
     const occb200_config& c = e->cfg;
     const int C = 256, Nq = e->Nq, F = c.ffn_dim, od = c.out_dim, mid = C / c.pillar_h;
-    const bool tc = c.precision == 1 && c.use_tensor_cores;
-    const bool tc32 = c.precision == 0 && c.use_tensor_cores;      // fp32 storage, split-bf16 tensor-core GEMMs
+    e->plan = make_frame_plan(c, Nq);
+    const FramePlan& p = e->plan;
     {
         GETP(bq, "bev_embedding.weight", (size_t)Nq * C);
         if (upload(e->bev_queries, bq->data(), bq->size())) return 2;
@@ -1027,13 +1080,11 @@ int occb200_engine_finalize(occb200_engine* e)
         if (upload(dre, re->data(), re->size()) || upload(dce, ce->data(), ce->size())) return 2;
         if (e->pos.alloc((size_t)Nq * C * 4)) return 2;
         if (launch_bev_pos(dre.as<float>(), dce.as<float>(), c.bev_h, c.bev_w, C / 2, e->pos.as<float>(), 0)) return 2;
-        if (tc) {                                                  // T32 copy of pos for the fused LayerNorm epilogue
+        if (p.tc_bf16) {                                           // T32 copy of pos for the fused LayerNorm epilogue
             const size_t rows_pad = ((size_t)Nq + 127) / 128 * 128;
             if (e->pos_t32.alloc(rows_pad * C * 4)) return 2;
             OCC_CUDA(cudaMemset(e->pos_t32.p, 0, rows_pad * C * 4));
             if (launch_t32_convert(e->pos.as<float>(), e->pos_t32.as<float>(), Nq, 0, 0)) return 2;
-            if (e->pos_bf.alloc((size_t)Nq * C * 2)) return 2;
-            if (launch_cast<bf16>(e->pos.as<float>(), e->pos_bf.as<bf16>(), (int64_t)Nq * C, 0)) return 2;
             // bev_queries / pos are parameters: their fp32 (T32) and bf16 operand forms are frame-independent
             if (e->qc_f32.alloc(rows_pad * C * 4) || e->qc_t.alloc((size_t)Nq * C * 2) || e->qc_pos_t.alloc((size_t)Nq * C * 2))
                 return 2;
@@ -1057,8 +1108,8 @@ int occb200_engine_finalize(occb200_engine* e)
             const std::vector<float>* B = find(e, name + ".bias", n);
             if (!W || !B) return 3;
             if (upload(wbuf, W->data(), W->size()) || upload(bbuf, B->data(), B->size())) return 2;
-            if (tc && wh && upload_bf16(*wh, W->data(), W->size())) return 2;
-            if (tc32 && wh && upload_w3(*wh, W->data(), n, k)) return 2;
+            if (p.tc_bf16 && wh && upload_bf16(*wh, W->data(), W->size())) return 2;
+            if (p.tc_split && wh && upload_w3(*wh, W->data(), n, k)) return 2;
             return 0;
         };
         auto up_cat = [&](DevBuf& wbuf, DevBuf& bbuf, DevBuf* wh, const std::string& n1, const std::string& n2,
@@ -1072,9 +1123,9 @@ int occb200_engine_finalize(occb200_engine* e)
             W.insert(W.end(), W2->begin(), W2->end());
             B.insert(B.end(), B2->begin(), B2->end());
             if (upload(wbuf, W.data(), W.size()) || upload(bbuf, B.data(), B.size())) return 2;
-            if (tc && wh && upload_bf16(*wh, W.data(), W.size())) return 2;
-            if (tc32 && wh && upload_w3(*wh, W.data(), r1 + r2, k)) return 2;
-            if (tc && fold) {                                    // k = 2C: (W1 + W2) [r, C] bf16 and the constant W2 pos + b
+            if (p.tc_bf16 && wh && upload_bf16(*wh, W.data(), W.size())) return 2;
+            if (p.tc_split && wh && upload_w3(*wh, W.data(), r1 + r2, k)) return 2;
+            if (p.tc_bf16 && p.qproj_f16 && fold) {              // k = 2C: (W1 + W2) [r, C] bf16 and the constant W2 pos + b
                 const size_t half = k / 2, rows = r1 + r2;
                 std::vector<float> Wf(rows * half), W2h(rows * half);
                 for (size_t r = 0; r < rows; ++r)
@@ -1119,7 +1170,7 @@ int occb200_engine_finalize(occb200_engine* e)
             if (upload(w.ln_g[n], g->data(), C) || upload(w.ln_b[n], b->data(), C)) return 2;
         }
     }
-    if (tc) {
+    if (p.tc_bf16) {
         // SpatialCrossAttention's value_proj input (the camera tokens) does not depend on the layer
         // (spatial_cross_attention.py:334): project once with all layers' weights, [L*256, 256].
         std::vector<float> W, B;
@@ -1153,7 +1204,7 @@ int occb200_engine_finalize(occb200_engine* e)
                     wf[((size_t)t * cin + ci) * od + co] = (*W)[((size_t)co * cin + ci) * 27 + t] * s;
         }
         if (upload(e->conv_w[i], wf.data(), wf.size()) || upload(e->conv_b[i], bf.data(), bf.size())) return 2;
-        if (tc) {                                             // tensor-core layout: [tap][cout][cin], K-major rows
+        if (p.conv == FramePlan::CONV_TC) {                   // tensor-core layout: [tap][cout][cin], K-major rows
             std::vector<float> wt((size_t)27 * od * cin);
             for (int t = 0; t < 27; ++t)
                 for (int co = 0; co < od; ++co)
@@ -1161,7 +1212,7 @@ int occb200_engine_finalize(occb200_engine* e)
                         wt[((size_t)t * od + co) * cin + ci] = wf[((size_t)t * cin + ci) * od + co];
             if (upload_bf16(e->conv_wh[i], wt.data(), wt.size())) return 2;
         }
-        if (tc32 && c.pillar_h == 16) {                       // same layout, split into bf16 hi + lo (3-pass fp32-grade convolution)
+        if (p.conv == FramePlan::CONV_SPLIT) {                // same layout, split into bf16 hi + lo (3-pass fp32-grade convolution)
             std::vector<float> hi((size_t)27 * od * cin), lo(hi.size());
             for (int t = 0; t < 27; ++t)
                 for (int co = 0; co < od; ++co)
@@ -1187,7 +1238,7 @@ int occb200_engine_finalize(occb200_engine* e)
             upload(e->hw2, w2->data(), w2->size()) || upload(e->hb2, b2->data(), b2->size()) ||
             upload(e->fw1, f1->data(), f1->size()) || upload(e->fb1, g1->data(), g1->size()) ||
             upload(e->fw2, f2->data(), f2->size()) || upload(e->fb2, g2->data(), g2->size())) return 2;
-        if (tc && od == 32 && c.num_classes + 2 <= 19) {          // tensor-core head: concatenated / block-diagonal weights
+        if (p.head_tc) {                                          // tensor-core head: concatenated / block-diagonal weights
             const int H = 2 * od, nc = c.num_classes;
             std::vector<float> w1c((size_t)2 * H * od), b1c(2 * H), w2c((size_t)32 * 2 * H, 0.f), b2c(nc + 2);
             for (int i = 0; i < H * od; ++i) { w1c[i] = (*w1)[i]; w1c[(size_t)H * od + i] = (*f1)[i]; }
@@ -1217,27 +1268,23 @@ int occb200_engine_finalize(occb200_engine* e)
         e->vox2.alloc(nvox * od * es) || e->hits.alloc(Nq)) return 2;
     OCC_CUDA(cudaMemset(e->q_f32.p, 0, nq_pad * C * 4));
     OCC_CUDA(cudaMemset(e->x_f32.p, 0, nq_pad * C * 4));
-    if (tc32) {
+    if (p.tc_split) {
         const size_t kmax = (size_t)std::max(2 * C, F);
         if (e->split_ws.alloc((size_t)Nq * 2 * kmax * 2) || e->tokens_split.alloc(ntok * 2 * C * 2)) return 2;
-        if (c.pillar_h == 16 && e->vox_split.alloc(nvox * 2 * od * 2)) return 2;
     }
+    if (p.conv == FramePlan::CONV_SPLIT && e->vox_split.alloc(nvox * 2 * od * 2)) return 2;
     e->host_params.clear();
     if ((c.precision == 0 ? build_tsa_query_values<float>(e) : build_tsa_query_values<bf16>(e))) return 2;
-    e->l0_ready = false;
-    if (tc && e->qc_f32.p != nullptr && getenv("OCC_NO_L0_FOLD") == nullptr) {
+    if (p.fold_layer0) {
         // Layer 0's TemporalSelfAttention (value_proj, query projection over [bev_queries | pos], gather, output_proj) and
-        // its LayerNorm depend on parameters only when prev_bev is None: run the frame path's own kernels once, here.
+        // its LayerNorm depend on parameters only when prev_bev is None: the frame's own fused TSA stage runs once, here.
         const size_t rows_pad = ((size_t)Nq + 127) / 128 * 128;
         if (e->l0_x_f32.alloc(rows_pad * C * 4) || e->l0_q_t.alloc((size_t)Nq * C * 2)) return 2;
         OCC_CUDA(cudaMemset(e->l0_x_f32.p, 0, rows_pad * C * 4));
-        const bool taps = e->taps;
-        e->taps = false;
-        const int rc = forward_impl<bf16>(e, nullptr, 0, PrevBev(), FrameOut(), 0, MODE_L0_TSA_ONLY);
-        e->taps = taps;
-        if (rc) return rc;
+        Residual rs{e->qc_f32.as<float>(), e->l0_x_f32.as<float>(), e->l0_x_f32.as<float>()};
+        if (tsa_stage<bf16>(e, true, false, 0, e->qc_t.as<bf16>(), e->qc_pos_t.as<bf16>(), rs, e->l0_q_t.as<bf16>(), 0))
+            return 2;
         OCC_CUDA(cudaDeviceSynchronize());
-        e->l0_ready = true;
     }
     e->finalized = true;
     return 0;
