@@ -132,7 +132,14 @@ int occb200_engine_rotation_map(occb200_engine* e, double angle_deg, int32_t* ma
  * channels-last bf16 levels into engine-owned buffers (code 2's hand-over), otherwise fp32 NCHW levels.  The backbone's
  * workspace and those level buffers are shared by both _submit_host slots: every frame records an event after its last read
  * of them and the next frame's backbone waits for it, so switching streams between submits stays correct.
- * occb200_engine_launches_per_frame then counts the backbone's kernels too. */
+ * occb200_engine_launches_per_frame then counts the backbone's kernels too.
+ * 4 = JPEG camera files: feats[0] points to an occb200_encoded_frame, declared below, holding the num_cams files in HOST memory,
+ * for every frame call.  The files are checked and parsed on the host (error 1 before any CUDA call, see occb200_jpeg_*; their
+ * size must be the attached backbone's frame format), packed into a pinned staging buffer of the call's buffer set (the
+ * device calls' and _forward_host's, or the slot's) and uploaded in one copy (the slot's copy stream, else `stream`); three
+ * kernels decode them on `stream` into that set's frame buffer, byte-identical to cv2.imdecode(IMREAD_UNCHANGED), and the
+ * frame continues as for 3 with those frames.  The caller may reuse its buffers when the call returns.
+ * occb200_engine_launches_per_frame counts the decode's three kernels too. */
 int occb200_engine_set_input_dtype(occb200_engine* e, int feats_bf16);
 /* Borrowed; NULL detaches.  bb must be finalized, with num_images == num_cams, level shapes equal to the engine's, and a
  * frame format set.  It must outlive the engine's use of it (detach before destroying it). */
@@ -402,6 +409,44 @@ int occb200_backbone_set_frame_format(occb200_backbone* e, int src_h, int src_w,
  * precision 1 only).  Without a frame format set, or with an out-of-range argument, it returns an error and launches nothing. */
 int occb200_backbone_forward_frames(occb200_backbone* e, const uint8_t* frames, void* out0, void* out1, void* out2,
                                     void* out3, int out_layout, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Baseline JPEG decoding on the device, byte-identical to cv2.imdecode(buf, cv2.IMREAD_UNCHANGED) (libjpeg-turbo's default
+ * path: ISLOW IDCT, fancy upsampling, integer YCbCr -> BGR), which is what mmcv.imread(name, 'unchanged') runs in
+ * LoadMultiViewImageFromFiles.  Supported: SOF0 / SOF1 (sequential Huffman), 8-bit samples and quantisation tables, three
+ * YCbCr components in one interleaved scan, 4:2:0 or 4:4:4, any restart interval, any size up to JPEG's 65535 x 65535 with
+ * a scan of at most 256 MiB.  Bytes after the last EOI marker are ignored.  Everything else (progressive, arithmetic, 12-bit,
+ * 16-bit tables, grayscale, CMYK, Adobe transform, 4:2:2 / 4:4:0 / 4:1:1, several scans, a truncated file, a Huffman table
+ * with more codes than its lengths allow) returns 1 on the host, before any CUDA call, with a message naming it.  EXIF orientation is ignored, as IMREAD_UNCHANGED does.
+ *
+ * _info: host only; the size of one file after the same checks.
+ * _decode: n HOST buffers (data[i], sizes[i] bytes); out dev u8 = the n images one after another, image i (h_i, w_i, 3) BGR at
+ *   the sum of the earlier images' h * w * 3 bytes; out_bytes must be that total.  The files are parsed on the host, packed
+ *   into the decoder's pinned staging buffer (after its previous upload has left it) and uploaded and decoded on `stream`
+ *   (three kernels).  The caller's buffers may be reused when the call returns.  Calls on one decoder run in stream order:
+ *   use one stream per decoder.
+ * _status: after the caller has synchronised the decode's stream, bit i % 32 set = image i's scan was corrupt (an invalid code,
+ *   coefficients past the block end, a restart interval that ends early or late, a marker inside the scan).  Such an image
+ *   is decoded from zero coefficients (flat grey); nothing is read or written out of bounds, and the next decode is
+ *   unaffected. */
+typedef struct occb200_jpeg occb200_jpeg;
+int occb200_jpeg_create(occb200_jpeg** out);
+void occb200_jpeg_destroy(occb200_jpeg* d);
+int occb200_jpeg_info(const void* data, int64_t size, int* h, int* w);
+int occb200_jpeg_decode(occb200_jpeg* d, int n, const void* const* data, const int64_t* sizes, uint8_t* out, int64_t out_bytes,
+                        void* stream);
+int occb200_jpeg_status(occb200_jpeg* d, int* status);
+
+/* Input dtype 4 (occb200_engine_set_input_dtype): a frame is the num_cams encoded camera files.  feats[0] points to this HOST
+ * descriptor (feats[1..3] are ignored) in every frame call, device or host; data[c] / size[c] are camera c's HOST buffer. */
+typedef struct occb200_encoded_frame {
+    const void* data[8];
+    int64_t size[8];
+} occb200_encoded_frame;
+/* Status of the last device-call frame (_forward, _forward_video[_angle]) in input dtype 4, once the caller has synchronised
+ * its stream: as occb200_jpeg_status.  The host calls check it themselves and return 5 when a camera's scan was corrupt
+ * (_forward_host when it returns, _wait_host for a slot). */
+int occb200_engine_jpeg_status(occb200_engine* e, int* status);
 
 #ifdef __cplusplus
 }

@@ -81,7 +81,18 @@ SIGNATURES = {
     'occb200_backbone_forward_nhwc_bf16': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'occb200_backbone_set_frame_format': (_i, [_vp, _i, _i, _vp, _vp, _i]),
     'occb200_backbone_forward_frames': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    'occb200_jpeg_create': (_i, [ctypes.POINTER(_vp)]),
+    'occb200_jpeg_destroy': (None, [_vp]),
+    'occb200_jpeg_info': (_i, [_vp, _i64, ctypes.POINTER(_i), ctypes.POINTER(_i)]),
+    'occb200_jpeg_decode': (_i, [_vp, _i, _vp, _vp, _vp, _i64, _vp]),
+    'occb200_jpeg_status': (_i, [_vp, ctypes.POINTER(_i)]),
+    'occb200_engine_jpeg_status': (_i, [_vp, ctypes.POINTER(_i)]),
 }
+
+
+class EncodedFrame(ctypes.Structure):
+    """occb200_encoded_frame: the host buffers of one frame's camera files (input dtype 4)"""
+    _fields_ = [('data', _vp * 8), ('size', _i64 * 8)]
 
 _lib = None
 

@@ -114,6 +114,30 @@ class BackboneEngine:
                                                                 _lib.stream_ptr()))
         return outs
 
+    def forward_jpeg(self, files, channels_last_bf16=False):
+        """files: the num_images encoded camera files (bytes-like, in image order; `occnet_b200.jpeg`) of the frame format's
+        size -> decoded on the GPU into the frames cv2.imdecode(IMREAD_UNCHANGED) gives, then `forward_frames`.  The sizes are
+        checked on the host before anything is launched; `jpeg_status()` after a synchronise reports a corrupt scan."""
+        from .jpeg import JpegDecoder, image_size
+        hw = getattr(self, 'frame_hw', None)
+        if hw is None:
+            raise RuntimeError('BackboneEngine: call set_frame_format() before passing camera files')
+        files = list(files)
+        if len(files) != self.num_images:
+            raise ValueError(f'expected {self.num_images} camera files, got {len(files)}')
+        for i, f in enumerate(files):
+            if image_size(f) != tuple(hw):
+                raise ValueError(f'camera file {i} is {image_size(f)} (h, w), the frame format is {tuple(hw)}')
+        if getattr(self, '_jpeg', None) is None:
+            self._jpeg = JpegDecoder(self.device)
+        with torch.cuda.device(self.device):
+            frames = self._jpeg.decode(files)
+        return self.forward_frames(frames, channels_last_bf16=channels_last_bf16)
+
+    def jpeg_status(self):
+        """after `forward_jpeg` and a synchronise of its stream: bit i set = camera file i had a corrupt scan"""
+        return self._jpeg.status()
+
     def __del__(self):
         h = getattr(self, '_h', None)
         if h:

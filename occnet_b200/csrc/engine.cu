@@ -20,6 +20,7 @@
 #include "common.cuh"
 #include "conv3d_tc.cuh"
 #include "gemm_tc.cuh"
+#include "jpeg.cuh"
 #include "kernels.cuh"
 
 namespace occ {
@@ -65,8 +66,17 @@ struct Requests {
 // feats[0]) and the i64 classes and flow the copies back read; for an armed frame the u8 classes and the flow when the caller
 // asked for neither, and for the host calls the staging of a ray request's records and of a score request's ground truth.
 // One set for the device calls and _forward_host, one per _submit_host slot (a slot's copies overlap the other slot's kernels).
+// Input dtype 4 adds the set's JPEG decoder (its tables, pinned staging and scratch) and the decoded frames it writes.
+struct JpegHandle {
+    occb200_jpeg* p = nullptr;
+    JpegHandle() = default;
+    JpegHandle(const JpegHandle&) = delete;
+    JpegHandle& operator=(const JpegHandle&) = delete;
+    ~JpegHandle() { occb200_jpeg_destroy(p); }
+};
 struct FrameBufs {
-    DevBuf feats[4], occ, flow, sem, rec_cls, rec_dist, rec_flow, gt_sem, gt_flow;
+    DevBuf feats[4], occ, flow, sem, rec_cls, rec_dist, rec_flow, gt_sem, gt_flow, frames;
+    JpegHandle jpeg;
 };
 
 // _submit_host uploads an input buffer above 32 MB in two pieces on two copy streams: when the split was tuned, one
@@ -179,6 +189,7 @@ struct occb200_engine {
         int32_t* rot_pinned = nullptr;
         cudaEvent_t h2d_done[kH2DSplit] = {}, compute_done = nullptr, d2h_done = nullptr;
         bool busy = false;
+        bool jpeg = false;              // the frame in flight decodes JPEG files: _wait_host checks their status
     } slots[2];
     cudaStream_t h2d_stream[kH2DSplit] = {}, d2h_stream = nullptr;
     int launches = 0;
@@ -739,7 +750,7 @@ int check_backbone(const occb200_engine* e, const occb200_backbone* bb)
 // (bf16), or for 3 the uint8 frames [num_cams, src_h, src_w, 3] of the attached backbone (l = 0)
 size_t input_bytes(const occb200_engine* e, int layout, int l)
 {
-    if (layout == 3) {
+    if (layout >= 3) {
         const BackboneInfo bi = backbone_info(e->bb);
         return (size_t)e->cfg.num_cams * bi.src_h * bi.src_w * 3;
     }
@@ -771,15 +782,22 @@ int forward_frames_impl(occb200_engine* e, const uint8_t* frames, const PrevBev&
     return 0;
 }
 
-// Host-side checks of a frame's input pointers (device or host): error 1, nothing enqueued.
-int check_frame(const occb200_engine* e, const float* const* feats)
+// Host-side checks of a frame's input pointers (device or host): error 1, nothing enqueued.  Input dtype 4 also parses the
+// camera files' headers into the decoder of the buffer set `b` the frame will use (host only).
+int check_frame(const occb200_engine* e, const float* const* feats, FrameBufs& b)
 {
     OCC_CHECK(e->finalized, "engine_finalize() has not been called");
     OCC_CHECK(e->cameras_set, "engine_set_cameras() has not been called");
-    if (e->feats_bf16 == 3) {
-        OCC_CHECK(e->bb != nullptr, "input dtype 3 (camera frames) needs an attached backbone (occb200_engine_attach_backbone)");
+    if (e->feats_bf16 >= 3) {
+        OCC_CHECK(e->bb != nullptr, "input dtypes 3 and 4 (camera frames) need an attached backbone (occb200_engine_attach_backbone)");
         OCC_CHECK(feats[0] != nullptr, "null frame buffer");
-        return check_backbone(e, e->bb) ? 1 : 0;
+        if (check_backbone(e, e->bb)) return 1;
+        if (e->feats_bf16 == 3) return 0;
+        const auto* f = reinterpret_cast<const occb200_encoded_frame*>(feats[0]);
+        for (int c = 0; c < e->cfg.num_cams; ++c) OCC_CHECK(f->data[c] != nullptr, "null camera file " + std::to_string(c));
+        if (!b.jpeg.p && occb200_jpeg_create(&b.jpeg.p)) return 1;
+        const BackboneInfo bi = backbone_info(e->bb);
+        return jpeg_prepare(b.jpeg.p, e->cfg.num_cams, f->data, f->size, bi.src_h, bi.src_w);
     }
     for (int l = 0; l < e->cfg.num_levels; ++l) OCC_CHECK(feats[l] != nullptr, "null feature level");
     return 0;
@@ -814,7 +832,7 @@ PrevBev video_prev(const occb200_engine* e, int scene_start, const int32_t* map,
 // stream.  A frame that writes the history waits for the previous one's write (on whatever stream that ran) before it reads
 // it, and records hist_done after its own.
 int run_frame(occb200_engine* e, const float* const* feats, const PrevBev& prev, FrameOut out, const Requests& rq,
-              FrameBufs& b, cudaStream_t st)
+              FrameBufs& b, cudaStream_t st, bool jpeg_uploaded = false)
 {
     if (rq.rays.armed || rq.score.armed) {
         const size_t nvox = (size_t)e->cfg.bev_w * e->cfg.bev_h * e->cfg.pillar_h;
@@ -830,9 +848,17 @@ int run_frame(occb200_engine* e, const float* const* feats, const PrevBev& prev,
     if (prev.writes_history && e->hist_recorded) OCC_CUDA(cudaStreamWaitEvent(st, e->hist_done, 0));
     const bool f32 = e->cfg.precision == 0;
     int rc;
-    if (e->feats_bf16 == 3) {
+    if (e->feats_bf16 >= 3) {
         const uint8_t* frames = reinterpret_cast<const uint8_t*>(feats[0]);
+        if (e->feats_bf16 == 4) {
+            // the camera files (parsed by check_frame) are decoded on the frame's stream into the set's frame buffer
+            if (ensure(b.frames, input_bytes(e, 4, 0))) return 2;
+            if (!jpeg_uploaded && jpeg_upload(b.jpeg.p, st, st)) return 2;
+            if (jpeg_decode(b.jpeg.p, b.frames.as<uint8_t>(), st)) return 2;
+            frames = b.frames.as<uint8_t>();
+        }
         rc = f32 ? forward_frames_impl<float>(e, frames, prev, out, st) : forward_frames_impl<bf16>(e, frames, prev, out, st);
+        if (e->feats_bf16 == 4) e->launches += kJpegLaunches;
     } else {
         rc = f32 ? forward_impl<float>(e, feats, e->feats_bf16, prev, out, st)
                  : forward_impl<bf16>(e, feats, e->feats_bf16, prev, out, st);
@@ -857,6 +883,16 @@ int run_frame(occb200_engine* e, const float* const* feats, const PrevBev& prev,
     return 0;
 }
 
+// error 5 when a camera file of the set's last decode (complete on the host) had a corrupt scan
+int check_jpeg_status(const FrameBufs& b)
+{
+    const int st = jpeg_status_host(b.jpeg.p);
+    if (st == 0) return 0;
+    set_last_error("corrupt JPEG scan in camera file(s) with bit mask " + std::to_string(st) +
+                   " (the frame's outputs are not valid)");
+    return 5;
+}
+
 // Every host-buffer frame (_forward_host, _submit_host, _submit_host_video[_angle]) after its entry point's own checks, in
 // this order: the remaining checks (error 1 before any CUDA call, the requests still armed), the uploads of the inputs and of
 // the host rotation map `map_host` (NULL: none), the request staging, the frame, the copies back.  `slot` -1 (_forward_host):
@@ -867,11 +903,11 @@ int host_frame(occb200_engine* e, int slot, const float* const* feats_host, Prev
 {
     occb200_engine::Slot* s = slot < 0 ? nullptr : &e->slots[slot];
     OCC_CHECK(s == nullptr || !s->busy, "slot still in flight: call occb200_engine_wait_host first");
-    if (check_frame(e, feats_host)) return 1;
+    FrameBufs& b = s ? s->bufs : e->bufs;
+    if (check_frame(e, feats_host, b)) return 1;
     if (map_host)
         for (int q = 0; q < e->Nq; ++q) OCC_CHECK(map_host[q] >= -1 && map_host[q] < e->Nq, "rotation map entry out of range");
 
-    FrameBufs& b = s ? s->bufs : e->bufs;
     if (s && !e->d2h_stream) {
         for (cudaStream_t& hs : e->h2d_stream) OCC_CUDA(cudaStreamCreateWithFlags(&hs, cudaStreamNonBlocking));
         OCC_CUDA(cudaStreamCreateWithFlags(&e->d2h_stream, cudaStreamNonBlocking));
@@ -893,7 +929,11 @@ int host_frame(occb200_engine* e, int slot, const float* const* feats_host, Prev
     }
     const int layout = e->feats_bf16;
     const float* dev_feats[4] = {nullptr, nullptr, nullptr, nullptr};
-    for (int l = 0; l < (layout == 3 ? 1 : 4); ++l) {                     // input dtype 3: one buffer, the uint8 frames
+    if (layout == 4) {                                                     // the packed camera files, decoded by the frame
+        if (jpeg_upload(b.jpeg.p, s ? e->h2d_stream[0] : st, st)) return 2;
+        dev_feats[0] = feats_host[0];
+    }
+    for (int l = 0; l < (layout == 4 ? 0 : layout == 3 ? 1 : 4); ++l) {   // input dtype 3: one buffer, the uint8 frames
         const size_t n = input_bytes(e, layout, l);
         if (ensure(b.feats[l], n)) return 2;
         if (s) {
@@ -938,7 +978,7 @@ int host_frame(occb200_engine* e, int slot, const float* const* feats_host, Prev
     FrameOut out;
     out.flow = b.flow.as<float>();
     out.cls_i64 = occ_host ? b.occ.as<int64_t>() : nullptr;
-    const int rc = run_frame(e, dev_feats, prev, out, rq, b, st);
+    const int rc = run_frame(e, dev_feats, prev, out, rq, b, st, true);
     if (rc) return rc;
 
     cudaStream_t d2h = st;
@@ -958,10 +998,11 @@ int host_frame(occb200_engine* e, int slot, const float* const* feats_host, Prev
     }
     if (!s) {
         OCC_CUDA(cudaStreamSynchronize(st));
-        return 0;
+        return layout == 4 ? check_jpeg_status(b) : 0;
     }
     OCC_CUDA(cudaEventRecord(s->d2h_done, d2h));
     s->busy = true;
+    s->jpeg = layout == 4;
     return 0;
 }
 
@@ -1303,7 +1344,7 @@ int occb200_engine_forward(occb200_engine* e, const float* const* feats, const f
                            float* occ_logits, float* flow, uint8_t* occ_cls_u8, int64_t* occ_cls_i64, void* stream)
 {
     OCC_CHECK(e && feats, "null pointer");
-    if (check_frame(e, feats)) return 1;
+    if (check_frame(e, feats, e->bufs)) return 1;
     PrevBev prev;
     if (prev_bev) {
         prev.src = PrevBev::CALLER;
@@ -1338,7 +1379,7 @@ int occb200_engine_forward_video(occb200_engine* e, const float* const* feats, c
     OCC_CHECK(feats, "null pointer");
     OCC_CHECK(e, "null engine");
     OCC_CHECK(e->hist.p != nullptr, "history not enabled: call occb200_engine_set_history(e, 1) first");
-    if (check_frame(e, feats)) return 1;
+    if (check_frame(e, feats, e->bufs)) return 1;
     return run_frame(e, feats, video_prev(e, scene_start, rot_map_dev, nullptr),
                      {bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64}, take_requests(e), e->bufs, (cudaStream_t)stream);
 }
@@ -1351,7 +1392,7 @@ int occb200_engine_forward_video_angle(occb200_engine* e, const float* const* fe
     OCC_CHECK(feats, "null pointer");
     OCC_CHECK(e, "null engine");
     OCC_CHECK(e->hist.p != nullptr, "history not enabled: call occb200_engine_set_history(e, 1) first");
-    if (check_frame(e, feats)) return 1;
+    if (check_frame(e, feats, e->bufs)) return 1;
     const RotGrid g = rotation_grid(e, angle_deg);
     return run_frame(e, feats, video_prev(e, scene_start, nullptr, &g), {bev_embed, occ_logits, flow, occ_cls_u8, occ_cls_i64},
                      take_requests(e), e->bufs, (cudaStream_t)stream);
@@ -1404,7 +1445,14 @@ int occb200_engine_wait_host(occb200_engine* e, int slot)
     if (!s.busy) return 0;
     OCC_CUDA(cudaEventSynchronize(s.d2h_done));
     s.busy = false;
-    return 0;
+    return s.jpeg ? check_jpeg_status(s.bufs) : 0;
+}
+
+int occb200_engine_jpeg_status(occb200_engine* e, int* status)
+{
+    OCC_CHECK(e && status, "null pointer");
+    OCC_CHECK(e->bufs.jpeg.p != nullptr, "no JPEG frame has run on the device calls");
+    return occb200_jpeg_status(e->bufs.jpeg.p, status);
 }
 
 // origins_host [T,3] (f32, or f64 if is_f64) -> the kernel argument; error 1 for a non-finite coordinate
@@ -1531,8 +1579,8 @@ int occb200_rotation_coeffs(double angle_deg, int bev_h, int bev_w, int cx, int 
 
 int occb200_engine_set_input_dtype(occb200_engine* e, int feats_bf16)
 {
-    OCC_CHECK(e && feats_bf16 >= 0 && feats_bf16 <= 3,
-              "input dtype must be 0 (fp32 NCHW), 1 (bf16 NCHW), 2 (bf16 NHWC) or 3 (uint8 camera frames)");
+    OCC_CHECK(e && feats_bf16 >= 0 && feats_bf16 <= 4,
+              "input dtype must be 0 (fp32 NCHW), 1 (bf16 NCHW), 2 (bf16 NHWC), 3 (uint8 camera frames) or 4 (JPEG camera files)");
     e->feats_bf16 = feats_bf16;
     return 0;
 }

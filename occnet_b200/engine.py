@@ -14,6 +14,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .jpeg import host_buffer
 from .ops import ray_origins_host
 
 PRECISIONS = {'fp32': 0, 'bf16': 1}
@@ -120,9 +121,13 @@ class OccEngine:
         """Feature levels are handed over as `dtype` from now on (torch.float32, the reference's, or torch.bfloat16);
         `channels_last` (bf16 only): tensors of shape (num_cams, C, h, w) whose MEMORY is (num_cams, h, w, C) -- the
         backbone engine's native output.  torch.uint8: each frame is ONE tensor of camera frames (num_cams, src_h, src_w, 3)
-        that the attached backbone (`attach_backbone`) turns into the levels on the device first."""
-        assert dtype in (torch.float32, torch.bfloat16, torch.uint8) and not (channels_last and dtype != torch.bfloat16)
-        code = 3 if dtype == torch.uint8 else (2 if channels_last else int(dtype == torch.bfloat16))
+        that the attached backbone (`attach_backbone`) turns into the levels on the device first.  'jpeg': each frame is the
+        num_cams encoded camera files in camera order (bytes, 1-D uint8 numpy arrays or CPU tensors; `load_jpeg_frame`), in
+        host memory for every call, device or host; the engine decodes them on the GPU into the frames cv2.imdecode gives
+        (occnet_b200/jpeg.py) and runs the attached backbone on them.  A host call whose file has a corrupt scan raises
+        (forward_host, or wait_host for a slot); after a device call, `jpeg_status()` reports it."""
+        assert dtype in (torch.float32, torch.bfloat16, torch.uint8, 'jpeg') and not (channels_last and dtype != torch.bfloat16)
+        code = 4 if dtype == 'jpeg' else 3 if dtype == torch.uint8 else (2 if channels_last else int(dtype == torch.bfloat16))
         _lib.check(self.lib.occb200_engine_set_input_dtype(self._h, code))
         self.feat_dtype, self.feat_channels_last = dtype, bool(channels_last)
 
@@ -226,6 +231,14 @@ class OccEngine:
 
     def _check_feats(self, feats, cuda):
         """A mismatched tensor would be an out-of-bounds device read in the pack kernel: fail on the host instead."""
+        if self.feat_dtype == 'jpeg':
+            if self.backbone is None:
+                raise RuntimeError("JPEG input ('jpeg') needs an attached backbone: call attach_backbone() first")
+            if isinstance(feats, (bytes, bytearray, torch.Tensor, np.ndarray)) or len(feats) != self.cfg['num_cams']:
+                raise ValueError(f'a JPEG frame is a sequence of {self.cfg["num_cams"]} encoded camera files')
+            for f in feats:
+                host_buffer(f)
+            return
         if self.feat_dtype == torch.uint8:
             if self.backbone is None:
                 raise RuntimeError('camera-frame input (torch.uint8) needs an attached backbone: call attach_backbone() first')
@@ -243,6 +256,15 @@ class OccEngine:
                                  f'{self.feat_dtype} {"CUDA" if cuda else "CPU (pinned)"} tensor')
 
     def _feat_ptrs(self, feats):
+        if self.feat_dtype == 'jpeg':
+            # feats[0] -> occb200_encoded_frame; the engine copies the files into its staging buffer before the call returns
+            bufs = [host_buffer(f) for f in feats]
+            desc = _lib.EncodedFrame()
+            for c, (addr, n, _) in enumerate(bufs):
+                desc.data[c], desc.size[c] = addr, n
+            arr = (ctypes.c_void_p * 4)(ctypes.addressof(desc))
+            arr._keep = (desc, bufs)
+            return arr
         arr = (ctypes.c_void_p * 4)()
         for i, f in enumerate([feats] if self.feat_dtype == torch.uint8 else feats):
             arr[i] = f.data_ptr()
@@ -276,7 +298,7 @@ class OccEngine:
         'flow'; the counters are complete when the frame is (stream order)."""
         C = self.cfg['embed_dims']
         dev = self.device
-        if not self.feat_channels_last and self.feat_dtype != torch.uint8:
+        if not self.feat_channels_last and self.feat_dtype in (torch.float32, torch.bfloat16):
             feats = [f.contiguous() for f in feats]
         self._check_feats(feats, cuda=True)
         out = self._outputs(want)
@@ -330,6 +352,13 @@ class OccEngine:
 
     def wait_host(self, slot):
         _lib.check(self.lib.occb200_engine_wait_host(self._h, slot))
+
+    def jpeg_status(self):
+        """After a device call ('jpeg' input) and a synchronise of its stream: bit c set = camera c's file had a corrupt
+        scan (its frame was decoded from zero coefficients, so the outputs are not valid)."""
+        s = ctypes.c_int()
+        _lib.check(self.lib.occb200_engine_jpeg_status(self._h, ctypes.byref(s)))
+        return s.value
 
     def stream_host(self, frames_host, ray_origins=None, volumes=True, score=None, metric=None):
         """Generator over an iterable of host frames with two frames in flight; yields (occ int64 CPU, flow CPU)
@@ -423,7 +452,7 @@ class OccEngine:
         rotation, bit for bit; the frame's BEV stays in the history whether or not 'bev_embed' is in `want`.  An angle
         costs no host work: the engine computes the cells of `rotation_index_map(angle)` on the device.  `ray_origins`,
         `score` and `metric`: as for `forward`."""
-        if not self.feat_channels_last and self.feat_dtype != torch.uint8:
+        if not self.feat_channels_last and self.feat_dtype in (torch.float32, torch.bfloat16):
             feats = [f.contiguous() for f in feats]
         self._check_feats(feats, cuda=True)
         out = self._outputs(want)

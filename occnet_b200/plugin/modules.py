@@ -646,7 +646,12 @@ class BEVFormerOcc(BaseModule):
     `img` may also be the camera frames themselves, uint8 (B, N, h, w, 3) in BGR order as decoded, on CUDA or CPU: the native
     backbone's stem then does the test pipeline's NormalizeMultiviewImage(**frame_norm_cfg) + PadMultiViewImage(**frame_pad)
     + DefaultFormatBundle3D on the device (bit-identical to running them on the host in fp32), and copies of the metas get
-    the keys those transforms set.  The defaults are the shipped config's (bevformer_base_occ.py:14-15, 166-171)."""
+    the keys those transforms set.  The defaults are the shipped config's (bevformer_base_occ.py:14-15, 166-171).
+
+    `img` may also be the cameras' encoded JPEG files (LoadMultiViewImageFromFiles' input): `[frames]` with `frames` a list of
+    B batch items, each a sequence of N bytes-like files (bytes, 1-D uint8 numpy arrays or CPU tensors) in camera order, or
+    one item's N files directly.  They are decoded on the GPU into the uint8 frames cv2.imdecode(IMREAD_UNCHANGED) gives
+    (`occnet_b200.jpeg`), which then take the uint8 path above, metas included; a corrupt scan raises once the frame has run."""
 
     def __init__(self, pts_bbox_head=None, img_backbone=None, img_neck=None, use_grid_mask=False, video_test_mode=False,
                  train_cfg=None, test_cfg=None, pretrained=None, feature_extractor=None, native_backbone=True,
@@ -696,6 +701,38 @@ class BEVFormerOcc(BaseModule):
         # frame into `ray_metric`; 'occ_results' and 'flow_results' are None and nothing is copied to the host
         self.score_only = score_only
         self.prev_frame_info = {'prev_bev': None, 'scene_token': None, 'prev_pos': 0, 'prev_angle': 0}
+
+    @staticmethod
+    def _encoded_batch(img):
+        """`img` as the encoded files of B batch items (a list of B lists of N bytes-like), or None if it holds tensors"""
+        from ..jpeg import is_buffer
+        if not isinstance(img, (list, tuple)) or not img:
+            return None
+        if is_buffer(img[0]):                                            # one item's N files
+            return [list(img)]
+        if isinstance(img[0], (list, tuple)) and img[0] and is_buffer(img[0][0]):
+            return [list(x) for x in img]
+        if isinstance(img[0], (list, tuple)) and img[0] and isinstance(img[0][0], (list, tuple)):
+            return BEVFormerOcc._encoded_batch(img[0])                     # [frames]: the outer test-time list
+        return None
+
+    def _decode_jpeg(self, batch):
+        """B items x N encoded files -> uint8 CUDA frames (B, N, h, w, 3), decoded on the GPU on the current stream"""
+        from ..jpeg import JpegDecoder
+        if not torch.cuda.is_available():
+            raise RuntimeError('BEVFormerOcc: JPEG camera files need a CUDA device (libocc_b200 has no CPU path)')
+        B, N = len(batch), len(batch[0])
+        if any(len(x) != N for x in batch):
+            raise ValueError('every batch item must hold the same number of camera files')
+        p = next(self.pts_bbox_head.parameters())
+        dev = p.device if p.is_cuda else torch.device('cuda', torch.cuda.current_device())
+        if getattr(self, '_jpeg', None) is None or self._jpeg.device != dev:
+            self._jpeg = JpegDecoder(str(dev))
+        with torch.cuda.device(dev):
+            frames = self._jpeg.decode([f for x in batch for f in x])
+        if isinstance(frames, list):
+            raise ValueError('the camera files of one call must all have the same size')
+        return frames.view(B, N, *frames.shape[1:])
 
     def _get_backbone_engine(self, device, shape):
         """the native backbone engine for images of `shape` (B*N, 3, H, W) on `device`, rebuilt when a parameter changes"""
@@ -866,8 +903,21 @@ class BEVFormerOcc(BaseModule):
         truth into `ray_metric.counters` instead, what `evaluate_miou` + `ray_based_miou` do with the volumes on the host;
         the result carries ray records only if the detector is `ray_only`."""
         metas = img_metas[0] if isinstance(img_metas[0], (list, tuple)) else img_metas
+        encoded = self._encoded_batch(img)
+        if encoded is not None:
+            img = self._decode_jpeg(encoded)
+            res = self._forward_test(metas, img, img_feats, lidar_origins, gt_semantics, gt_flow, ray_metric, **kwargs)
+            torch.cuda.current_stream(img.device).synchronize()
+            bad = self._jpeg.status()
+            if bad:
+                raise RuntimeError(f'BEVFormerOcc: corrupt JPEG scan in camera file(s) with bit mask {bad} (item-major '
+                                   'order); the results are not valid')
+            return res
         if isinstance(img, (list, tuple)):
             img = img[0]
+        return self._forward_test(metas, img, img_feats, lidar_origins, gt_semantics, gt_flow, ray_metric, **kwargs)
+
+    def _forward_test(self, metas, img, img_feats, lidar_origins, gt_semantics, gt_flow, ray_metric, **kwargs):
         if self.ray_only and lidar_origins is None:
             raise ValueError('ray_only=True needs lidar_origins for every frame')
         score = None
