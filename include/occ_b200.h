@@ -410,6 +410,30 @@ int occb200_backbone_set_frame_format(occb200_backbone* e, int src_h, int src_w,
 int occb200_backbone_forward_frames(occb200_backbone* e, const uint8_t* frames, void* out0, void* out1, void* out2,
                                     void* out3, int out_layout, void* stream);
 
+/* Single backbone operators, for operator tests: the code the backbone runs, on caller-supplied operands.  Storage is fp32
+ * (precision 0) or bf16 (precision 1); tensors are dense NHWC device arrays.  Every rejection returns 1 before any CUDA call.
+ *   backbone_conv: out [N, Ho, Wo, cout] = act(conv(in [N, H, W, cin], w) + bias), k x k, `stride`, pad (k - 1) / 2, routed as
+ *     the backbone routes the same convolution (use_tensor_cores needs precision 1).  w_host: HOST fp32 [cout][k*k*cin],
+ *     BN already folded, tap-major ((ky*k + kx)*cin + ci); rounded to bf16 for the tensor cores as the backbone rounds it.
+ *     bias_host: HOST fp32 [cout] or NULL.  residual (NULL, or [N, H, W, cout] with stride 1 and act 1): out = relu(conv + bias
+ *     + residual), fused into the convolution where the backbone fuses it, else the convolution rounded to the storage type
+ *     and a separate add + ReLU.  cin % 8 == 0 or cin == 3, cout % 8 == 0, k in {1, 3, 7}, stride in {1, 2}.  Synchronises
+ *     `stream`.  Reports the path (OCCB200_CONV_*), the number of kernels launched and whether the residual was fused. */
+#define OCCB200_CONV_IMPLICIT_TC 1   /* implicit-GEMM tensor-core convolution (conv2d_tc) */
+#define OCCB200_CONV_IM2COL_TC 2     /* im2col + tensor-core GEMM */
+#define OCCB200_CONV_DIRECT_TC 3     /* tensor-core GEMM on the input as is (1x1, stride 1) */
+#define OCCB200_CONV_IM2COL_SIMT 4   /* im2col + CUDA-core GEMM */
+#define OCCB200_CONV_DIRECT_SIMT 5   /* CUDA-core GEMM on the input as is */
+int occb200_backbone_conv(int precision, int use_tensor_cores, const void* in, int N, int H, int W, int cin, const float* w_host,
+                          const float* bias_host, const void* residual, int cout, int k, int stride, int pad, int act, void* out,
+                          int* path, int* launches, int* residual_fused, void* stream);
+/*   backbone_maxpool: out [N, Ho, Wo, C] = MaxPool2d(3, stride 2, padding 1)(in [N, H, W, C]), C % 8 == 0.
+ *   backbone_upsample_add: fine [N, Hf, Wf, C] += F.interpolate(coarse [N, Hc, Wc, C], size (Hf, Wf), mode 'nearest'), the
+ *     add in fp32 and rounded to the storage type; C % 8 == 0. */
+int occb200_backbone_maxpool(int precision, const void* in, int N, int H, int W, int C, void* out, void* stream);
+int occb200_backbone_upsample_add(int precision, void* fine, const void* coarse, int N, int Hf, int Wf, int Hc, int Wc, int C,
+                                  void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Baseline JPEG decoding on the device, byte-identical to cv2.imdecode(buf, cv2.IMREAD_UNCHANGED) (libjpeg-turbo's default
  * path: ISLOW IDCT, fancy upsampling, integer YCbCr -> BGR), which is what mmcv.imread(name, 'unchanged') runs in

@@ -81,6 +81,10 @@ SIGNATURES = {
     'occb200_backbone_forward_nhwc_bf16': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'occb200_backbone_set_frame_format': (_i, [_vp, _i, _i, _vp, _vp, _i]),
     'occb200_backbone_forward_frames': (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    'occb200_backbone_conv': (_i, [_i, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp,
+                                   ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
+    'occb200_backbone_maxpool': (_i, [_i, _vp, _i, _i, _i, _i, _vp, _vp]),
+    'occb200_backbone_upsample_add': (_i, [_i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     'occb200_jpeg_create': (_i, [ctypes.POINTER(_vp)]),
     'occb200_jpeg_destroy': (None, [_vp]),
     'occb200_jpeg_info': (_i, [_vp, _i64, ctypes.POINTER(_i), ctypes.POINTER(_i)]),

@@ -3,7 +3,8 @@
 // bevformer_base_occ.py:48-66 puts in front of the hot path (caller: detectors/bevformer_occ.py:66-99; eval mode:
 // GridMask is the identity, BatchNorm uses running statistics).  SURVEY 8f rank 1 ("next").
 //
-// Checked by tests/test_backbone_gpu.py; default feature extractor of the drop-in detector when it
+// Checked by tests/test_backbone_gpu.py (whole network) and tests/test_backbone_ops_gpu.py (each convolution's route and
+// result through occb200_backbone_conv); default feature extractor of the drop-in detector when it
 // is given images.  See backbone_kernels.cu / conv2d_tc.cu for the design (NHWC activations, BatchNorm folded, stride-1
 // convolutions on the TMA-im2col implicit-GEMM kernel, the others explicit im2col + the wgmma GEMM; fp32 parity
 // configuration: the CUDA-core GEMM).
@@ -48,6 +49,7 @@ struct occb200_backbone {
     bool frames_set = false;
     FrameNorm fn{};
     int launches = 0;                // kernels the last forward launched
+    int conv_path = 0;               // OCCB200_CONV_* path of the last conv()
     // workspace
     DevBuf img_nhwc, col, ping[2], t1, t2, t3, idn, stage_out[3], lat[3], fo[4];
     size_t elt() const { return precision ? 2 : 4; }
@@ -71,7 +73,7 @@ int upload_conv(occb200_backbone* e, ConvW& c, const std::vector<float>& W, cons
 {
     if (c.w.alloc(W.size() * 4) || c.b.alloc(B.size() * 4)) return 2;
     OCC_CUDA(cudaMemcpy(c.w.p, W.data(), W.size() * 4, cudaMemcpyHostToDevice));
-    OCC_CUDA(cudaMemcpy(c.b.p, B.data(), B.size() * 4, cudaMemcpyHostToDevice));
+    if (!B.empty()) OCC_CUDA(cudaMemcpy(c.b.p, B.data(), B.size() * 4, cudaMemcpyHostToDevice));   // none: bias NULL
     if (e->precision && e->use_tc) {
         std::vector<__nv_bfloat16> h(W.size());
         for (size_t i = 0; i < W.size(); ++i) h[i] = __float2bfloat16(W[i]);
@@ -119,13 +121,20 @@ int fold_conv(occb200_backbone* e, ConvW& c, const std::string& conv_key, const 
 
 inline int out_size(int in, int k, int stride, int pad) { return (in + 2 * pad - k) / stride + 1; }
 
+// the tensor-core GEMM takes [M, kpad] x [cout, kpad] (bf16 storage with bf16 weights); otherwise the CUDA-core GEMM runs
+template <typename T>
+bool gemm_on_tc(const occb200_backbone* e, int64_t M, const ConvW& c)
+{
+    return sizeof(T) == 2 && e->use_tc && c.wh.p && gemm_tc_supported((int)M, c.cout, c.kpad, c.kpad);
+}
+
 // out[M, cout] = act(A[M, kpad] . W^T + b)
 template <typename T>
 int conv_gemm(occb200_backbone* e, const T* A, int64_t M, const ConvW& c, T* out, int act, cudaStream_t st)
 {
     OCC_CHECK(M < (1ll << 31), "backbone: too many pixels for one GEMM");
     if constexpr (sizeof(T) == 2) {
-        if (e->use_tc && c.wh.p && gemm_tc_supported((int)M, c.cout, c.kpad, c.kpad))
+        if (gemm_on_tc<T>(e, M, c))
             return gemm_tc<bf16>(reinterpret_cast<const bf16*>(A), nullptr, 0, c.wh.as<bf16>(), c.b.as<float>(), nullptr,
                                  reinterpret_cast<bf16*>(out), (int)M, c.cout, c.kpad, act, st);
     }
@@ -133,37 +142,62 @@ int conv_gemm(occb200_backbone* e, const T* A, int64_t M, const ConvW& c, T* out
                            c.cout, c.kpad, act, st);
 }
 
-// one convolution on NHWC input [N, H, W, cin] -> out [N, Ho, Wo, cout].  On the tensor cores, stride-1 3x3 convolutions
-// (and 1x1 with a residual) go through the TMA-im2col implicit-GEMM kernel conv2d_tc.cu, which skips the im2col round trip
-// through memory; the others take explicit im2col + the GEMM.  `residual` (same shape as out) is only accepted on the
-// implicit-GEMM path, where the add (+ ReLU) is fused into the epilogue; fused_residual reports it.
+// On the tensor cores, stride-1 3x3 convolutions (and 1x1 with a residual) go through the TMA-im2col implicit-GEMM kernel
+// conv2d_tc.cu, which skips the im2col round trip through memory; its epilogue can add the residual (+ ReLU).
+template <typename T>
+bool implicit_gemm(const occb200_backbone* e, const ConvW& c, bool residual)
+{
+    return sizeof(T) == 2 && e->use_tc && c.wh.p && c.stride == 1 && c.kpad == c.kh * c.kw * c.cin &&
+           conv2d_tc_supported(c.cin, c.cout, c.kh, c.kw) && (c.kh == 3 || residual);
+}
+
+// one convolution on NHWC input [N, H, W, cin] -> out [N, Ho, Wo, cout]: the implicit-GEMM kernel where it applies, else
+// explicit im2col (except a 1x1 stride-1 convolution, whose NHWC input IS the operand) + the GEMM.  `residual` (same shape as
+// out; out = relu(conv + residual)) is only accepted where implicit_gemm() fuses it.  e->conv_path reports the path taken.
 template <typename T>
 int conv(occb200_backbone* e, const T* in, int N, int H, int W, const ConvW& c, T* out, int act, int& Ho, int& Wo,
-         cudaStream_t st, const T* residual = nullptr, bool* fused_residual = nullptr)
+         cudaStream_t st, const T* residual = nullptr)
 {
     Ho = out_size(H, c.kh, c.stride, c.pad);
     Wo = out_size(W, c.kw, c.stride, c.pad);
     const int64_t M = (int64_t)N * Ho * Wo;
-    if (fused_residual) *fused_residual = false;
     if constexpr (sizeof(T) == 2) {
-        if (e->use_tc && c.wh.p && c.stride == 1 && c.kpad == c.kh * c.kw * c.cin &&
-            conv2d_tc_supported(c.cin, c.cout, c.kh, c.kw) && (c.kh == 3 || residual != nullptr)) {
-            if (fused_residual) *fused_residual = residual != nullptr;
+        if (implicit_gemm<T>(e, c, residual != nullptr)) {
+            e->conv_path = OCCB200_CONV_IMPLICIT_TC;
             e->launches++;
             return conv2d_tc(reinterpret_cast<const bf16*>(in), c.wh.as<bf16>(), c.b.as<float>(),
                              reinterpret_cast<const bf16*>(residual), reinterpret_cast<bf16*>(out), N, H, W, c.cin, c.cout,
                              c.kh, c.kw, c.pad, residual ? ACT_RELU : act, st);
         }
     }
+    OCC_CHECK(residual == nullptr, "backbone: residual on a convolution that cannot fuse it");
     const T* A = in;
-    if (!(c.kh == 1 && c.kw == 1 && c.stride == 1 && c.kpad == c.cin)) {
+    const bool direct = c.kh == 1 && c.kw == 1 && c.stride == 1 && c.kpad == c.cin;
+    if (!direct) {
         OCC_CHECK((size_t)M * c.kpad * sizeof(T) <= e->col.bytes, "backbone: im2col workspace too small");
         if (launch_im2col_nhwc<T>(in, e->col.as<T>(), N, H, W, c.cin, c.kh, c.kw, c.stride, c.pad, Ho, Wo, c.kpad, st)) return 2;
         e->launches++;
         A = e->col.as<T>();
     }
+    const bool tc = gemm_on_tc<T>(e, M, c);
+    e->conv_path = direct ? (tc ? OCCB200_CONV_DIRECT_TC : OCCB200_CONV_DIRECT_SIMT)
+                          : (tc ? OCCB200_CONV_IM2COL_TC : OCCB200_CONV_IM2COL_SIMT);
     e->launches++;
     return conv_gemm<T>(e, A, M, c, out, act, st);
+}
+
+// The bottleneck's last step, dst = relu(conv(in) + identity): one fused launch where implicit_gemm() applies, else the
+// convolution into e->t3 and add_relu (two roundings to T instead of one).  fused reports which.
+template <typename T>
+int conv_add_relu(occb200_backbone* e, const T* in, int N, int H, int W, const ConvW& c, const T* identity, T* dst, int& Ho,
+                  int& Wo, cudaStream_t st, bool& fused)
+{
+    fused = implicit_gemm<T>(e, c, true);
+    if (fused) return conv<T>(e, in, N, H, W, c, dst, ACT_NONE, Ho, Wo, st, identity);
+    if (conv<T>(e, in, N, H, W, c, e->t3.as<T>(), ACT_NONE, Ho, Wo, st)) return 2;
+    if (launch_add_relu<T>(e->t3.as<T>(), identity, dst, (int64_t)N * Ho * Wo * c.cout, st)) return 2;
+    e->launches++;
+    return 0;
 }
 
 // Input: fp32 images `img` [N, 3, H, W], or uint8 camera frames `frames` [N, src_h, src_w, 3] (img == nullptr) that the stem's
@@ -212,14 +246,8 @@ int forward_impl(occb200_backbone* e, const float* img, const uint8_t* frames, f
             const bool last = b + 1 == e->blocks[s].size();
             T* dst = (cur == e->ping[0].as<T>()) ? e->ping[1].as<T>() : e->ping[0].as<T>();
             if (last && s >= 1) dst = e->stage_out[s - 1].as<T>();           // C3 / C4 / C5 stay alive for the neck
-            // conv3 (1x1): on the implicit-GEMM path the residual add + ReLU ride its epilogue and it writes `dst` directly
-            bool fused = false;
-            if (conv<T>(e, e->t2.as<T>(), N, h2, w2, blk.c3, dst, ACT_NONE, h3, w3, st, identity, &fused)) return 2;
-            if (!fused) {
-                if (conv<T>(e, e->t2.as<T>(), N, h2, w2, blk.c3, e->t3.as<T>(), ACT_NONE, h3, w3, st)) return 2;
-                if (launch_add_relu<T>(e->t3.as<T>(), identity, dst, (int64_t)N * h3 * w3 * blk.c3.cout, st)) return 2;
-                e->launches++;
-            }
+            bool fused;
+            if (conv_add_relu<T>(e, e->t2.as<T>(), N, h2, w2, blk.c3, identity, dst, h3, w3, st, fused)) return 2;
             cur = dst; H = h3; W = w3;
         }
         if (s >= 1) { sh[s - 1] = H; sw[s - 1] = W; }
@@ -410,6 +438,86 @@ int occb200_backbone_forward_frames(occb200_backbone* e, const uint8_t* frames, 
     float* fo[4] = {(float*)out0, (float*)out1, (float*)out2, (float*)out3};
     return e->precision ? forward_impl<bf16>(e, nullptr, frames, fo, (cudaStream_t)stream)
                         : forward_impl<float>(e, nullptr, frames, fo, (cudaStream_t)stream);
+}
+
+// ---- single backbone operators for kernel tests: argument checks only, every rejection before the first CUDA call, then the
+// code forward_impl runs (a ConvW built by upload_conv, conv() / conv_add_relu(), the layer launchers)
+int occb200_backbone_conv(int precision, int use_tensor_cores, const void* in, int N, int H, int W, int cin, const float* w_host,
+                          const float* bias_host, const void* residual, int cout, int k, int stride, int pad, int act, void* out,
+                          int* path, int* launches, int* residual_fused, void* stream)
+{
+    OCC_CHECK(in && w_host && out && path && launches && residual_fused, "null pointer");
+    OCC_CHECK(precision == 0 || precision == 1, "precision must be 0 (fp32) or 1 (bf16)");
+    OCC_CHECK(precision == 1 || !use_tensor_cores, "use_tensor_cores needs bf16 storage (precision 1)");
+    OCC_CHECK(N > 0 && H > 0 && W > 0 && cin > 0 && cout > 0, "shape must be positive");
+    OCC_CHECK(cin % 8 == 0 || cin == 3, "cin must be a multiple of 8 (or 3, the stem's RGB)");
+    OCC_CHECK(cout % 8 == 0, "cout must be a multiple of 8");
+    OCC_CHECK(k == 1 || k == 3 || k == 7, "k must be 1, 3 or 7");
+    OCC_CHECK(stride == 1 || stride == 2, "stride must be 1 or 2");
+    OCC_CHECK(pad == (k - 1) / 2, "pad must be (k - 1) / 2, as in every backbone convolution");
+    OCC_CHECK(act == ACT_NONE || act == ACT_RELU, "act must be 0 (none) or 1 (relu)");
+    OCC_CHECK(residual == nullptr || (stride == 1 && act == ACT_RELU),
+              "a residual [N, H, W, cout] needs a stride-1 convolution (output shape = input shape) and act 1 (relu)");
+    occb200_backbone e;
+    e.precision = precision;
+    e.use_tc = use_tensor_cores ? 1 : 0;
+    ConvW c;
+    c.cout = cout; c.cin = cin; c.kh = c.kw = k; c.stride = stride; c.pad = pad;
+    const int K = k * k * cin;
+    c.kpad = (K + 63) / 64 * 64;
+    const int Ho = out_size(H, k, stride, pad), Wo = out_size(W, k, stride, pad);
+    const int64_t M = (int64_t)N * Ho * Wo;
+    OCC_CHECK(M < (1ll << 31), "too many output pixels for one GEMM");
+    std::vector<float> Wp((size_t)cout * c.kpad, 0.f), B;
+    for (int o = 0; o < cout; ++o) std::copy(w_host + (size_t)o * K, w_host + (size_t)(o + 1) * K, Wp.begin() + (size_t)o * c.kpad);
+    if (bias_host) B.assign(bias_host, bias_host + cout);
+    if (upload_conv(&e, c, Wp, B)) return 2;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const size_t es = e.elt();
+    if (!(k == 1 && stride == 1 && c.kpad == cin) && e.col.alloc((size_t)M * c.kpad * es)) return 2;
+    int ho, wo, rc;
+    bool fused = false;
+    if (precision) {
+        const bf16 *x = reinterpret_cast<const bf16*>(in), *r = reinterpret_cast<const bf16*>(residual);
+        bf16* y = reinterpret_cast<bf16*>(out);
+        if (r && !implicit_gemm<bf16>(&e, c, true) && e.t3.alloc((size_t)M * cout * es)) return 2;
+        rc = r ? conv_add_relu<bf16>(&e, x, N, H, W, c, r, y, ho, wo, st, fused) : conv<bf16>(&e, x, N, H, W, c, y, act, ho, wo, st);
+    } else {
+        const float *x = reinterpret_cast<const float*>(in), *r = reinterpret_cast<const float*>(residual);
+        float* y = reinterpret_cast<float*>(out);
+        if (r && e.t3.alloc((size_t)M * cout * es)) return 2;
+        rc = r ? conv_add_relu<float>(&e, x, N, H, W, c, r, y, ho, wo, st, fused) : conv<float>(&e, x, N, H, W, c, y, act, ho, wo, st);
+    }
+    if (rc) return rc;
+    OCC_CUDA(cudaStreamSynchronize(st));                 // the weights and workspaces are freed on return
+    *path = e.conv_path; *launches = e.launches; *residual_fused = fused ? 1 : 0;
+    return 0;
+}
+
+int occb200_backbone_maxpool(int precision, const void* in, int N, int H, int W, int C, void* out, void* stream)
+{
+    OCC_CHECK(in && out, "null pointer");
+    OCC_CHECK(precision == 0 || precision == 1, "precision must be 0 (fp32) or 1 (bf16)");
+    OCC_CHECK(N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "shape must be positive, C a multiple of 8");
+    const int Ho = out_size(H, 3, 2, 1), Wo = out_size(W, 3, 2, 1);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (precision)
+        return launch_maxpool3x3s2_nhwc<bf16>(reinterpret_cast<const bf16*>(in), reinterpret_cast<bf16*>(out), N, H, W, C, Ho, Wo, st);
+    return launch_maxpool3x3s2_nhwc<float>(reinterpret_cast<const float*>(in), reinterpret_cast<float*>(out), N, H, W, C, Ho, Wo, st);
+}
+
+int occb200_backbone_upsample_add(int precision, void* fine, const void* coarse, int N, int Hf, int Wf, int Hc, int Wc, int C,
+                                  void* stream)
+{
+    OCC_CHECK(fine && coarse, "null pointer");
+    OCC_CHECK(precision == 0 || precision == 1, "precision must be 0 (fp32) or 1 (bf16)");
+    OCC_CHECK(N > 0 && Hf > 0 && Wf > 0 && Hc > 0 && Wc > 0 && C > 0 && C % 8 == 0, "shape must be positive, C a multiple of 8");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (precision)
+        return launch_upsample_add_nhwc<bf16>(reinterpret_cast<bf16*>(fine), reinterpret_cast<const bf16*>(coarse), N, Hf, Wf, Hc,
+                                              Wc, C, st);
+    return launch_upsample_add_nhwc<float>(reinterpret_cast<float*>(fine), reinterpret_cast<const float*>(coarse), N, Hf, Wf, Hc,
+                                           Wc, C, st);
 }
 
 }  // extern "C"

@@ -1,7 +1,8 @@
 // Layout / data-movement kernels of the image backbone + neck (ResNet-50 + FPN feeding the hot path, SURVEY 8f rank 1;
 // reference: detectors/bevformer_occ.py:66-99 with the mmdet modules configured in bevformer_base_occ.py:48-66).
 //
-// Checked by tests/test_backbone_gpu.py (8 tests against the pinned backbone oracle); the bench's
+// Checked by tests/test_backbone_ops_gpu.py (max-pool and the top-down upsample-add bit-exact against torch; im2col through
+// every convolution route, bit-exact on integer operands) and tests/test_backbone_gpu.py (whole network); the bench's
 // `images_to_voxels` leg times it.  The stride-1 3x3 convolutions and the bottleneck's last 1x1 moved to the
 // TMA-im2col kernel conv2d_tc.cu; what is described here is the explicit-im2col path that the remaining convolutions still use.
 //

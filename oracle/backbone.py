@@ -97,4 +97,67 @@ def extract_img_feat(p, img, taps=None):
     return [f.view(B, N, *f.shape[1:]) for f in feats]
 
 
+def fold_conv(p, conv, bn, conv_bias=False):
+    """The engine's BatchNorm fold (backbone.cu fold_conv) in fp32: weight [co, ci, k, k] * scale, bias = shift (+ conv bias *
+    scale), scale = gamma / sqrt(var + eps), shift = beta - mean * scale; without `bn`, scale 1 and shift 0."""
+    w = p[conv + '.weight'].float()
+    co = w.shape[0]
+    scale, shift = torch.ones(co), torch.zeros(co)
+    if bn:
+        # the square root correctly rounded, as std::sqrt gives it (torch's vectorised fp32 sqrt can be 1 ulp off; the
+        # fp64 root of an fp32 value rounds to the correctly rounded fp32 root)
+        var = p[bn + '.running_var'].float() + torch.tensor(BN_EPS, dtype=torch.float32)
+        scale = p[bn + '.weight'].float() / torch.sqrt(var.double()).float()
+        shift = p[bn + '.bias'].float() - p[bn + '.running_mean'].float() * scale
+    if conv_bias:
+        shift = shift + p[conv + '.bias'].float() * scale
+    return w * scale[:, None, None, None], shift
+
+
+def storage_model(p, img, storage=torch.bfloat16, tensor_cores=True, rounding=True):
+    """Storage-rounding model of the engine's ResNet-50 + FPN: exact (fp64) sums over the engine's operands, and a rounding
+    to `storage` at every point where the engine stores one (rounding=False: none, i.e. the fp32 oracle's algorithm in fp64):
+      the image (the stem's NHWC copy); the weights (folded in fp32, then bf16 on the tensor cores, fp32 on the CUDA cores);
+      every convolution's output after bias + ReLU; the bottleneck's residual step, rounded once on the tensor cores (fused
+      into conv3's epilogue) but twice on the CUDA cores (conv3's output, then add + ReLU); each top-down upsample-add.
+    Max-pool and nearest upsampling select stored values and round nothing.  img (N, 3, H, W) -> the four FPN levels, fp64."""
+    def rnd(x):
+        return x.to(storage).double() if rounding else x
+
+    def conv(x, conv_key, bn_key, stride, relu, conv_bias=False, residual=None):
+        w, b = fold_conv(p, conv_key, bn_key, conv_bias)
+        if rounding and tensor_cores:
+            w = w.to(storage)
+        k = w.shape[-1]
+        y = F.conv2d(x, w.double().to(x.device), b.double().to(x.device), stride=stride, padding=(k - 1) // 2)
+        if residual is None:
+            return rnd(F.relu(y) if relu else y)
+        if not tensor_cores:
+            y = rnd(y)
+        return rnd(F.relu(y + residual))
+
+    pre = 'img_backbone.'
+    x = rnd(img.double())
+    x = conv(x, pre + 'conv1', pre + 'bn1', 2, True)
+    x = F.max_pool2d(x, kernel_size=3, stride=2, padding=1)
+    feats = []
+    for s, nblk in enumerate(STAGE_BLOCKS):
+        for b in range(nblk):
+            stride = 2 if (b == 0 and s > 0) else 1
+            q = f'{pre}layer{s + 1}.{b}.'
+            t = conv(x, q + 'conv1', q + 'bn1', 1, True)
+            t = conv(t, q + 'conv2', q + 'bn2', stride, True)
+            idn = conv(x, q + 'downsample.0', q + 'downsample.1', stride, False) if b == 0 else x
+            x = conv(t, q + 'conv3', q + 'bn3', 1, False, residual=idn)
+        if s >= 1:
+            feats.append(x)
+    nk = 'img_neck.'
+    lat = [conv(f, f'{nk}lateral_convs.{i}.conv', None, 1, False, conv_bias=True) for i, f in enumerate(feats)]
+    for i in range(2, 0, -1):
+        lat[i - 1] = rnd(lat[i - 1] + F.interpolate(lat[i], size=lat[i - 1].shape[2:], mode='nearest'))
+    outs = [conv(lat[i], f'{nk}fpn_convs.{i}.conv', None, 1, False, conv_bias=True) for i in range(3)]
+    outs.append(conv(outs[2], f'{nk}fpn_convs.3.conv', None, 2, False, conv_bias=True))
+    return tuple(outs)
+
+
 from occnet_b200.fixtures import init_backbone_params as init_params  # noqa: E402,F401  (synthetic weights live with the fixtures)

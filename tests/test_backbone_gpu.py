@@ -2,7 +2,10 @@
 bit-exactly to torchvision's resnet50 / FeaturePyramidNetwork), and of the channels-last bf16 hand-over to the hot path.
 
 On the tensor cores the stride-1 convolutions run on the TMA-im2col implicit-GEMM kernel (conv2d_tc.cu), the others on
-explicit im2col + gemm_tc.
+explicit im2col + gemm_tc.  The bf16 backbone is held to the storage-rounding model (oracle.backbone.storage_model: exact
+sums, the engine's roundings where it stores a value): per level its distance from the model, relative to the model's
+distance from the fp32 oracle, is held to bars measured on an H100 (see BF16_BARS).  The single convolutions are tested one by
+one in test_backbone_ops_gpu.py.
 """
 import os
 import sys
@@ -33,14 +36,55 @@ def test_backbone_fp32_matches_oracle():
     assert max(err) < 1e-3 * max(1.0, max(mag)), (err, mag)
 
 
+def _run_model(tc, hw=(128, 192), n=2, seed=5):
+    """bf16 engine, fp32 oracle and storage-rounding model on the same input: per FPN level the (mean, max) distances
+    engine-to-model and model-to-oracle, and the engine's largest error against the oracle relative to the level's magnitude"""
+    from occnet_b200.backbone import BackboneEngine
+    from oracle import backbone as OB
+    p = OB.init_params(seed=seed)
+    img = torch.randn(n, 3, *hw, generator=torch.Generator().manual_seed(3))
+    with torch.no_grad():
+        want = OB.fpn(p, OB.resnet50(p, img))
+        model = OB.storage_model(p, img.to(DEV), tensor_cores=tc)
+    got = BackboneEngine(p, n, hw, precision='bf16', use_tensor_cores=tc).forward(img.cuda())
+    em, mo, rel = [], [], []
+    for g, m, w in zip(got, model, want):
+        a, b = (g.double() - m).abs(), (m - w.to(DEV).double()).abs()
+        em.append((a.mean().item(), a.max().item()))
+        mo.append((b.mean().item(), b.max().item()))
+        rel.append((g.cpu() - w).abs().max().item() / max(w.abs().max().item(), 1.0))
+    for l in range(4):
+        print(f'{"tensor cores" if tc else "CUDA cores"} level {l}: engine-model mean {em[l][0]:.3e} max {em[l][1]:.3e}; '
+              f'model-fp32 mean {mo[l][0]:.3e} max {mo[l][1]:.3e}; ratios {em[l][0] / mo[l][0]:.3f} / {em[l][1] / mo[l][1]:.3f}')
+    return em, mo, rel
+
+
+# Engine-to-model distance over model-to-fp32 distance, (mean, max) per FPN level.  Measured on an H100 80GB HBM3 (700 W):
+#   CUDA cores   (1.230, 1.258) (1.253, 1.097) (1.250, 1.196) (1.304, 1.183)
+#   tensor cores (0.918, 0.959) (0.920, 0.981) (0.921, 0.751) (0.942, 1.022)
+# The engine is NOT closer to the model than the model is to fp32: its fp32 accumulation order flips a bf16 rounding of the
+# exact sum for a fraction of the elements of every layer (about K 2^-15 of them), and through 50-odd layers of a randomly
+# initialised network those 1-ulp flips grow into bf16-sized noise that is independent of the model's.  At the whole-network
+# level the model therefore bounds the size of the bf16 noise, not its values; each convolution is held bit-exactly and to a
+# derived fp64 bound in test_backbone_ops_gpu.py.  Bars: 2x the measured ratios, rounded up to 0.1.
+BF16_BARS = {False: ((2.5, 2.6), (2.6, 2.2), (2.5, 2.4), (2.7, 2.4)),
+             True: ((1.9, 2.0), (1.9, 2.0), (1.9, 1.6), (1.9, 2.1))}
+
+
+def _check_bf16_against_model(tc):
+    em, mo, rel = _run_model(tc)
+    assert max(rel) < 8e-2, rel                                      # sanity bound against the fp32 oracle
+    for l, ((mean_bar, max_bar), (a_mean, a_max), (b_mean, b_max)) in enumerate(zip(BF16_BARS[tc], em, mo)):
+        assert a_mean <= mean_bar * b_mean, (l, a_mean, b_mean)
+        assert a_max <= max_bar * b_max, (l, a_max, b_max)
+
+
 def test_backbone_bf16_simt_close_to_oracle():
-    err, mag = _run('bf16', False)
-    assert max(e / max(m, 1.0) for e, m in zip(err, mag)) < 8e-2, (err, mag)
+    _check_bf16_against_model(False)
 
 
 def test_backbone_bf16_tcgen05_close_to_oracle():
-    err, mag = _run('bf16', True)
-    assert max(e / max(m, 1.0) for e, m in zip(err, mag)) < 8e-2, (err, mag)
+    _check_bf16_against_model(True)
 
 
 def test_backbone_odd_sizes_fp32():

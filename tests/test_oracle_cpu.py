@@ -245,6 +245,67 @@ def test_backbone_extract_img_feat_shapes():
     assert shapes == [tuple(s) for s in fixtures.CFG_FULL['level_shapes']]
 
 
+def _fold_np(p, conv, bn, conv_bias=False):
+    """backbone.cu fold_conv in numpy fp32: (weight * scale [co, ci, k, k], shift [co])"""
+    w = p[conv + '.weight']; co = w.shape[0]
+    scale, shift = np.ones(co, np.float32), np.zeros(co, np.float32)
+    if bn:
+        scale = p[bn + '.weight'] / np.sqrt(p[bn + '.running_var'] + np.float32(1e-5))
+        shift = p[bn + '.bias'] - p[bn + '.running_mean'] * scale
+    if conv_bias:
+        shift = shift + p[conv + '.bias'] * scale
+    return w * scale[:, None, None, None], shift.astype(np.float32)
+
+
+def _backbone_convs():
+    """(conv key, BN key or None, conv bias) of every convolution of ResNet-50 + FPN"""
+    b, out = 'img_backbone.', [('img_backbone.conv1', 'img_backbone.bn1', False)]
+    for s, nblk in enumerate((3, 4, 6, 3)):
+        for i in range(nblk):
+            pre = f'{b}layer{s + 1}.{i}.'
+            out += [(pre + f'conv{j}', pre + f'bn{j}', False) for j in (1, 2, 3)]
+            if i == 0:
+                out.append((pre + 'downsample.0', pre + 'downsample.1', False))
+    out += [(f'img_neck.lateral_convs.{i}.conv', None, True) for i in range(3)]
+    return out + [(f'img_neck.fpn_convs.{i}.conv', None, True) for i in range(4)]
+
+
+def test_backbone_storage_model_fold_restates_fold_conv_in_fp32():
+    """oracle.backbone.fold_conv (what the storage-rounding model runs) is backbone.cu's BatchNorm fold, bit for bit"""
+    from oracle import backbone as OB
+    pt = OB.init_params(seed=7)
+    p = {k: v.numpy() for k, v in pt.items()}
+    convs = _backbone_convs()
+    assert len(convs) == 1 + 16 * 3 + 4 + 3 + 4
+    for conv, bn, cb in convs:
+        w, b = OB.fold_conv(pt, conv, bn, cb)
+        wn, bnp = _fold_np(p, conv, bn, cb)
+        assert w.dtype == torch.float32 and np.array_equal(w.numpy(), wn), conv
+        assert b.dtype == torch.float32 and np.array_equal(b.numpy(), bnp), conv
+
+
+@pytest.mark.parametrize('tensor_cores', [True, False])
+def test_backbone_storage_model_without_rounding_equals_fp32_oracle(tensor_cores):
+    """With its roundings off the storage-rounding model is the fp32 oracle's algorithm (BN folded, sums in fp64): equal to
+    it to fp32 round-off.  With them on it sits at bf16 distance, and the two routes (one rounding of the fused residual on the
+    tensor cores, two on the CUDA cores) differ."""
+    from oracle import backbone as OB
+    p = OB.init_params(seed=5)
+    img = torch.randn(2, 3, 72, 104, generator=torch.Generator().manual_seed(2))
+    with torch.no_grad():
+        want = OB.fpn(p, OB.resnet50(p, img))
+        exact = OB.storage_model(p, img, tensor_cores=tensor_cores, rounding=False)
+        rounded = OB.storage_model(p, img, tensor_cores=tensor_cores)
+        other = OB.storage_model(p, img, tensor_cores=not tensor_cores)
+    for lvl, (e, r, o, w) in enumerate(zip(exact, rounded, other, want)):
+        mag = w.abs().max().item()
+        assert e.shape == w.shape and (e - w.double()).abs().max().item() < 2e-5 * mag, lvl
+        d = (r - w.double()).abs()
+        assert 1e-3 * mag < d.max().item() < 8e-2 * mag, lvl
+        assert r.to(torch.bfloat16).double().equal(r), lvl                 # the model's outputs are stored bf16 values
+        assert not torch.equal(r, o), lvl
+
+
 def test_backbone_engine_schedule_emulated_on_cpu():
     """The backbone engine (csrc/backbone.cu) could not be run on a GPU in round 1.  This test re-states its SCHEDULE in
     numpy -- NHWC activations, BN folded into tap-major weights [co][(ky*KW+kx)*Cin + c] zero-padded to 64, explicit
@@ -255,17 +316,12 @@ def test_backbone_engine_schedule_emulated_on_cpu():
     pt = {k: torch.from_numpy(v) for k, v in p.items()}
 
     def fold(conv, bn, k, conv_bias=False):
-        w = p[conv + '.weight']; co, ci = w.shape[:2]
-        scale, shift = np.ones(co, np.float32), np.zeros(co, np.float32)
-        if bn:
-            scale = p[bn + '.weight'] / np.sqrt(p[bn + '.running_var'] + np.float32(1e-5))
-            shift = p[bn + '.bias'] - p[bn + '.running_mean'] * scale
-        if conv_bias:
-            shift = shift + p[conv + '.bias'] * scale
+        w, shift = _fold_np(p, conv, bn, conv_bias)
+        co, ci = w.shape[:2]
         kpad = (k * k * ci + 63) // 64 * 64
         W = np.zeros((co, kpad), np.float32)
-        W[:, :k * k * ci] = (w.transpose(0, 2, 3, 1) * scale[:, None, None, None]).reshape(co, -1)   # (ky, kx, ci) order
-        return W, shift.astype(np.float32), kpad
+        W[:, :k * k * ci] = w.transpose(0, 2, 3, 1).reshape(co, -1)                  # (ky, kx, ci) order
+        return W, shift, kpad
 
     def im2col(x, k, stride, pad, kpad):                       # x [N,H,W,C] -> [N*Ho*Wo, kpad]
         N, H, W, C = x.shape
