@@ -373,6 +373,33 @@ int occb200_sca_gather(const void* value, int value_bf16, const void* qproj, int
                        const float* zs_host, int num_cams, int D, const float pc_range[6], int img_h, int img_w, int bev_h,
                        int bev_w, const int level_hw_host[8], void* out, uint8_t* hits, void* stream);
 
+/* The voxel decoder's steps, for operator tests: the kernels the frame engine launches for a configuration (precision,
+ * use_tensor_cores, num_classes) with pillar_h 16 and out_dim 32, on weights prepared by the engine's own helpers.  Storage is
+ * fp32 (precision 0) or bf16 (precision 1); voxels are dense channels-last device arrays [X][Y][16][C].  Every rejection
+ * returns 1 before any CUDA call.  Each entry synchronises `stream` and reports the number of kernels it launched.
+ *   decoder_lift: vox [W][H][16][16] with vox[x][y][z][cm] = bev[y * W + x][cm * 16 + z] in the storage type, from bev fp32
+ *     [H * W, 256] row-major, or with from_t32 (bf16 storage and tensor cores only) in the T32 layout of the residual stream
+ *     (32 x 32 blocks of [col % 32 / 4][row % 32][4], rows padded to a multiple of 32).  H * W <= 2^24.
+ *   decoder_conv3d: out [X][Y][16][32] = relu(Conv3d 3x3x3, pad 1 (in [X][Y][16][cin]) with BatchNorm3d (eval, eps 1e-5)
+ *     folded in), cin 16 or 32, X, Y in [1, 4096].  w_host: HOST fp32 [32][cin][3][3][3] (torch layout, (z, y, x) taps);
+ *     bn_host: HOST fp32 [4][32] = gamma | beta | running_mean | running_var.  *path: OCCB200_DECODER_*; the split path
+ *     reports 4 launches (the [hi | lo] operand split and three convolution passes).
+ *   decoder_head: over vox [nvox][32], occ_logits [nvox][num_classes] = predicter(vox), flow [nvox][2] = flow_predicter(vox),
+ *     cls_u8 / cls_i64 [nvox] = the first argmax of the logits; any output may be NULL.  w1 b1 w2 b2 / f1 g1 f2 g2: HOST fp32
+ *     predicter.0 / .2 and flow_predicter.0 / .2 weights and biases in torch layout.  num_classes in [1, 32], nvox in
+ *     [1, 2^31).  *path: 1 for the tensor-core head (bf16 storage, tensor cores, at most 17 classes), 0 for the CUDA-core one. */
+#define OCCB200_DECODER_CUDA_CORES 0   /* conv3d_simt: fp32 weights, fp32 accumulation */
+#define OCCB200_DECODER_TC 1           /* conv3d_tc: bf16 weights and operands, fp32 accumulation */
+#define OCCB200_DECODER_SPLIT 2        /* conv3d_tc in three passes on bf16 hi / lo splits of fp32 operands and weights */
+int occb200_decoder_lift(int precision, int use_tensor_cores, int from_t32, const float* bev, int bev_h, int bev_w, void* vox,
+                         int* launches, void* stream);
+int occb200_decoder_conv3d(int precision, int use_tensor_cores, const void* in, int X, int Y, int cin, const float* w_host,
+                           const float* bn_host, void* out, int* path, int* launches, void* stream);
+int occb200_decoder_head(int precision, int use_tensor_cores, int num_classes, const void* vox, int64_t nvox, const float* w1,
+                         const float* b1, const float* w2, const float* b2, const float* f1, const float* g1, const float* f2,
+                         const float* g2, float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, int* path,
+                         int* launches, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Image backbone + neck (SURVEY 8f rank 1, the step immediately BEFORE the hot path); parity vs its oracle:
  * tests/test_backbone_gpu.py (fp32 1e-3 relative to the feature magnitude, bf16 bars stated there).

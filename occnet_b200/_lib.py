@@ -72,6 +72,10 @@ SIGNATURES = {
     'occb200_split_bf16': (_i, [_vp, _i, _vp, _i, _i64, _vp, _vp]),
     'occb200_tsa_gather': (_i, [_vp, _vp, _i, _vp, _i, _i, _i, _vp, _vp]),
     'occb200_sca_gather': (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    'occb200_decoder_lift': (_i, [_i, _i, _i, _vp, _i, _i, _vp, ctypes.POINTER(_i), _vp]),
+    'occb200_decoder_conv3d': (_i, [_i, _i, _vp, _i, _i, _i, _vp, _vp, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
+    'occb200_decoder_head': (_i, [_i, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                  ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
     'occb200_backbone_create': (_vp, [_i, _i, _i, _i, _i]),
     'occb200_backbone_destroy': (None, [_vp]),
     'occb200_backbone_load_param': (_i, [_vp, ctypes.c_char_p, _vp, ctypes.c_int64]),

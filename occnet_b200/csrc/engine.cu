@@ -125,6 +125,20 @@ struct FramePlan {
     bool lift_t32 = false;              // the shapes let the voxel lift read the T32 residual stream directly
 };
 
+// The voxel decoder's weights on the device, built from the torch-layout parameters by upload_decoder_conv /
+// upload_decoder_head for the engine (finalize) and for the occb200_decoder_* test entries alike
+struct DecoderConvW {
+    DevBuf w, b;                        // BatchNorm folded in: fp32 [27][cin][32] (tap = (dz*3+dy)*3+dx) and [32] (every path)
+    DevBuf wh;                          // CONV_TC: bf16 tap-major [27][32][cin] (K-major rows)
+    DevBuf wh_hi, wh_lo;                // CONV_SPLIT: the same layout split into bf16 hi + lo
+};
+struct DecoderHeadW {
+    DevBuf w1, b1, w2, b2, fw1, fb1, fw2, fb2;      // predicter / flow_predicter in torch layout, fp32 (CUDA-core head)
+    // head_tc: [predicter.0 ; flow_predicter.0] bf16 [128][32], block-diagonal [predicter.2 ; flow_predicter.2] bf16 [32][128]
+    // (flow rows at num_classes, num_classes + 1), biases [128] and [num_classes + 2]
+    DevBuf w1h, w2h, b1c, b2c;
+};
+
 }  // namespace
 }  // namespace occ
 
@@ -162,13 +176,13 @@ struct occb200_engine {
     // Self mode (prev_bev = None): layer 0's TemporalSelfAttention + its LayerNorm see only parameters (bev_queries, bev_pos,
     // weights) -- the result is frame-independent and is computed ONCE at finalize by the same kernels (T32 fp32 + bf16 copy)
     DevBuf l0_x_f32, l0_q_t;
-    DevBuf conv_w[2], conv_b[2], conv_wh[2];
-    DevBuf conv_wh_hi[2], conv_wh_lo[2], vox_split;      // fp32 storage + tensor cores: bf16 hi / lo split of the folded conv weights, [hi | lo] voxel operand
+    DecoderConvW dec_conv[2];
+    DevBuf vox_split;                                    // CONV_SPLIT: the [hi | lo] bf16 voxel operand
     DevBuf sca_v_all_wh, sca_v_all_b, sca_value_all;     // value_proj of every layer, concatenated (tensor-core path)
     // TSA queue 1 with a previous BEV (encoder.py:204-209 stacks the layer-0 query once): value_proj_l(bev_queries) of every
     // layer, [L][Nq,256] in the storage type -- parameters only, computed at finalize by the frame path's own GEMM
     DevBuf tsa_v_query;
-    DevBuf hw1, hb1, hw2, hb2, fw1, fb1, fw2, fb2, head_w1h, head_w2h, head_b1c, head_b2c;
+    DecoderHeadW head;
     // workspace
     DevBuf tokens, sca_value, q_f32, q_t, q_pos_t, prev_t, tsa_value, qproj, attn_out, x_f32,
         ffn_h, vox0, vox1, vox2, hits;
@@ -247,6 +261,76 @@ const std::vector<float>* find(const occb200_engine* e, const std::string& k, si
     return &it->second;
 }
 
+// ---- voxel decoder weights (transformer_occ.py:106-141): built here for the engine (finalize) and for the occb200_decoder_*
+// test entries alike, so that the operator tests run the kernels on exactly the weights the engine builds
+// BatchNorm3d (eval) folded into the bias-free Conv3d in fp32: s = gamma / sqrt(var + 1e-5), wf = w s, bf = beta - mean s;
+// torch layout [od][cin][27] -> wf [27][cin][od]
+void fold_conv3d_bn(const float* W, const float* gamma, const float* beta, const float* mean, const float* var, int cin, int od,
+                    std::vector<float>& wf, std::vector<float>& bf)
+{
+    wf.assign((size_t)27 * cin * od, 0.f);
+    bf.assign(od, 0.f);
+    for (int co = 0; co < od; ++co) {
+        const float s = gamma[co] / sqrtf(var[co] + 1e-5f);
+        bf[co] = beta[co] - mean[co] * s;
+        for (int ci = 0; ci < cin; ++ci)
+            for (int t = 0; t < 27; ++t) wf[((size_t)t * cin + ci) * od + co] = W[((size_t)co * cin + ci) * 27 + t] * s;
+    }
+}
+
+// wf [27][cin][od] -> the tensor cores' tap-major [27][od][cin] (K-major rows)
+std::vector<float> conv3d_tap_major(const std::vector<float>& wf, int cin, int od)
+{
+    std::vector<float> wt((size_t)27 * od * cin);
+    for (int t = 0; t < 27; ++t)
+        for (int co = 0; co < od; ++co)
+            for (int ci = 0; ci < cin; ++ci) wt[((size_t)t * od + co) * cin + ci] = wf[((size_t)t * cin + ci) * od + co];
+    return wt;
+}
+
+// One decoder layer's weights for the plan's convolution path: the folded fp32 weights and bias, and on the tensor cores the
+// tap-major bf16 copy (CONV_TC) or its bf16 hi + lo split, lo = bf16(w - hi) (CONV_SPLIT, the 3-pass fp32-grade convolution)
+int upload_decoder_conv(DecoderConvW& d, FramePlan::Conv path, const float* W, const float* gamma, const float* beta,
+                        const float* mean, const float* var, int cin, int od)
+{
+    std::vector<float> wf, bf;
+    fold_conv3d_bn(W, gamma, beta, mean, var, cin, od, wf, bf);
+    if (upload(d.w, wf.data(), wf.size()) || upload(d.b, bf.data(), bf.size())) return 2;
+    if (path == FramePlan::CONV_SIMT) return 0;
+    const std::vector<float> wt = conv3d_tap_major(wf, cin, od);
+    if (path == FramePlan::CONV_TC) return upload_bf16(d.wh, wt.data(), wt.size());
+    std::vector<float> hi(wt.size()), lo(wt.size());
+    for (size_t i = 0; i < wt.size(); ++i) {
+        hi[i] = __bfloat162float(__float2bfloat16(wt[i]));
+        lo[i] = wt[i] - hi[i];
+    }
+    return upload_bf16(d.wh_hi, hi.data(), hi.size()) || upload_bf16(d.wh_lo, lo.data(), lo.size()) ? 2 : 0;
+}
+
+// The occupancy / flow heads' weights, torch layout: w1 / f1 [2 od][od], b1 / g1 [2 od], w2 [nc][2 od], b2 [nc], f2 [2][2 od],
+// g2 [2].  head_tc adds the concatenated first layer and the block-diagonal second layer (flow rows at nc, nc + 1) in bf16.
+int upload_decoder_head(DecoderHeadW& h, bool head_tc, int nc, int od, const float* w1, const float* b1, const float* w2,
+                        const float* b2, const float* f1, const float* g1, const float* f2, const float* g2)
+{
+    const int H = 2 * od;
+    if (upload(h.w1, w1, (size_t)H * od) || upload(h.b1, b1, H) || upload(h.w2, w2, (size_t)nc * H) || upload(h.b2, b2, nc) ||
+        upload(h.fw1, f1, (size_t)H * od) || upload(h.fb1, g1, H) || upload(h.fw2, f2, (size_t)2 * H) || upload(h.fb2, g2, 2))
+        return 2;
+    if (!head_tc) return 0;
+    std::vector<float> w1c((size_t)2 * H * od), b1c(2 * H), w2c((size_t)32 * 2 * H, 0.f), b2c(nc + 2);
+    for (int i = 0; i < H * od; ++i) { w1c[i] = w1[i]; w1c[(size_t)H * od + i] = f1[i]; }
+    for (int i = 0; i < H; ++i) { b1c[i] = b1[i]; b1c[H + i] = g1[i]; }
+    for (int r = 0; r < nc; ++r)
+        for (int k = 0; k < H; ++k) w2c[(size_t)r * 2 * H + k] = w2[(size_t)r * H + k];
+    for (int r = 0; r < 2; ++r)
+        for (int k = 0; k < H; ++k) w2c[(size_t)(nc + r) * 2 * H + H + k] = f2[(size_t)r * H + k];
+    for (int i = 0; i < nc; ++i) b2c[i] = b2[i];
+    b2c[nc] = g2[0]; b2c[nc + 1] = g2[1];
+    if (upload_bf16(h.w1h, w1c.data(), w1c.size()) || upload_bf16(h.w2h, w2c.data(), w2c.size()) ||
+        upload(h.b1c, b1c.data(), b1c.size()) || upload(h.b2c, b2c.data(), b2c.size())) return 2;
+    return 0;
+}
+
 // ---- geometry of the fused spatial cross-attention gather: built here for the engine (creation, set_cameras) and for the
 // occb200_sca_gather test entry alike, so that the operator tests launch the kernels on exactly what the engine builds
 // the four value-map levels of every camera, rows [start, start + h*w) of the [Nv, 256] map; *Nv = the total
@@ -318,6 +402,57 @@ FramePlan make_frame_plan(const occb200_config& c, int Nq)
     p.head_tc = p.conv == FramePlan::CONV_TC && c.out_dim == 32 && c.num_classes + 2 <= 19;
     p.lift_t32 = p.tc_bf16 && c.pillar_h == 16;
     return p;
+}
+
+// ---- voxel decoder steps (transformer_occ.py:305-319), run by decode_stage and by the occb200_decoder_* test entries.  Each
+// enqueues its kernels on `st` and returns how many it launched, or -1 when a launcher failed (its message is set).
+// The lift: bev [H*W, 256] fp32 (from_t32: the T32 layout of the residual stream, bf16 voxels, Z = 16) -> vox [W][H][Z][256/Z]
+template <typename T>
+int decoder_lift(bool from_t32, const float* bev, int bev_h, int bev_w, int Z, T* vox, cudaStream_t st)
+{
+    if (from_t32) return launch_t32_to_voxel(bev, bev_h, bev_w, reinterpret_cast<bf16*>(vox), st) ? -1 : 1;
+    return launch_bev_to_voxel<T>(bev, bev_h, bev_w, Z, 256 / Z, vox, st) ? -1 : 1;
+}
+
+// One Conv3d + folded BatchNorm + ReLU layer on the plan's path: in [X][Y][Z][cin] -> out [X][Y][Z][32] in the storage type T.
+// CONV_SPLIT (T = float) first splits `in` into the [hi | lo] bf16 workspace `split` [X*Y*Z][2 cin].
+template <typename T>
+int decoder_conv(FramePlan::Conv path, const T* in, const DecoderConvW& w, int X, int Y, int Z, int cin, T* out, bf16* split,
+                 cudaStream_t st)
+{
+    if (path == FramePlan::CONV_SPLIT) {
+        if (launch_split_bf16(reinterpret_cast<const float*>(in), cin, nullptr, 0, (int64_t)X * Y * Z, split, st)) return -1;
+        if (launch_conv3d_tc_split(split, w.wh_hi.as<bf16>(), w.wh_lo.as<bf16>(), w.b.as<float>(), X, Y, Z, cin,
+                                   reinterpret_cast<float*>(out), st)) return -1;
+        return 4;                                                   // the split and the launcher's three passes
+    }
+    if (path == FramePlan::CONV_TC)
+        return launch_conv3d_tc(reinterpret_cast<const bf16*>(in), w.wh.as<bf16>(), w.b.as<float>(), X, Y, Z, cin,
+                                reinterpret_cast<bf16*>(out), st) ? -1 : 1;
+    return launch_conv3d_simt<T>(in, w.w.as<float>(), w.b.as<float>(), X, Y, Z, cin, out, st) ? -1 : 1;
+}
+
+// The occupancy / flow heads and the argmax over vox [nvox][32]; any output may be NULL
+template <typename T>
+int decoder_head(bool head_tc, const T* vox, const DecoderHeadW& h, int nc, int64_t nvox, float* occ_logits, float* flow,
+                 uint8_t* cls_u8, int64_t* cls_i64, cudaStream_t st)
+{
+    if (head_tc)
+        return launch_occ_head_tc(reinterpret_cast<const bf16*>(vox), h.w1h.as<bf16>(), h.w2h.as<bf16>(), h.b1c.as<float>(),
+                                  h.b2c.as<float>(), nc, nvox, occ_logits, flow, cls_u8, cls_i64, st) ? -1 : 1;
+    const HeadWeights hw{h.w1.as<float>(), h.b1.as<float>(), h.w2.as<float>(), h.b2.as<float>(),
+                         h.fw1.as<float>(), h.fb1.as<float>(), h.fw2.as<float>(), h.fb2.as<float>(), nc};
+    return launch_occ_head<T>(vox, hw, nvox, occ_logits, flow, cls_u8, cls_i64, st) ? -1 : 1;
+}
+
+// the plan of the occb200_decoder_* test entries: a configuration with the engine's decoder shapes (pillar_h 16, out_dim 32)
+FramePlan decoder_test_plan(int precision, int use_tensor_cores, int num_classes)
+{
+    occb200_config c;
+    memset(&c, 0, sizeof(c));
+    c.precision = precision; c.use_tensor_cores = use_tensor_cores; c.num_classes = num_classes;
+    c.pillar_h = 16; c.out_dim = 32;
+    return make_frame_plan(c, 1);
 }
 
 // ---- GEMM dispatch: the plan's tensor-core path where the shape allows it, the CUDA-core path otherwise
@@ -612,55 +747,36 @@ int decode_stage(occb200_engine* e, bool fuse_ln, Residual& rs, const FrameOut& 
     if (out.bev_embed)
         OCC_CUDA(cudaMemcpyAsync(out.bev_embed, rs.cur, (size_t)Nq * C * 4, cudaMemcpyDeviceToDevice, st));
     if (!out.occ_logits && !out.flow && !out.cls_u8 && !out.cls_i64) return 0;
+    int n;
     {
         ProfScope ps(e, st, CAT_VOX);
-        if (lift_from_t32) {
-            if (launch_t32_to_voxel(rs.cur, c.bev_h, c.bev_w, e->vox0.as<bf16>(), st)) return 2;
-        } else if (launch_bev_to_voxel<T>(rs.cur, c.bev_h, c.bev_w, Z, mid, e->vox0.as<T>(), st)) return 2;
-        e->launches++;
+        if ((n = decoder_lift<T>(lift_from_t32, rs.cur, c.bev_h, c.bev_w, Z, e->vox0.as<T>(), st)) < 0) return 2;
+        e->launches += n;
     }
+    bf16* split = e->vox_split.as<bf16>();
     if (p.conv == FramePlan::CONV_SPLIT) {
         ProfScope ps(e, st, CAT_CONV);
-        if (launch_split_bf16(e->vox0.as<float>(), mid, nullptr, 0, nvox, e->vox_split.as<bf16>(), st)) return 2;
-        e->launches++;
-        if (launch_conv3d_tc_split(e->vox_split.as<bf16>(), e->conv_wh_hi[0].as<bf16>(), e->conv_wh_lo[0].as<bf16>(),
-                                   e->conv_b[0].as<float>(), X, Y, Z, mid, e->vox1.as<float>(), st)) return 2;
-        e->launches += 3;                                           // the launcher's three passes
-        if (launch_split_bf16(e->vox1.as<float>(), c.out_dim, nullptr, 0, nvox, e->vox_split.as<bf16>(), st)) return 2;
-        e->launches++;
-        if (launch_conv3d_tc_split(e->vox_split.as<bf16>(), e->conv_wh_hi[1].as<bf16>(), e->conv_wh_lo[1].as<bf16>(),
-                                   e->conv_b[1].as<float>(), X, Y, Z, c.out_dim, e->vox2.as<float>(), st)) return 2;
-        e->launches += 3;
+        if ((n = decoder_conv<T>(p.conv, e->vox0.as<T>(), e->dec_conv[0], X, Y, Z, mid, e->vox1.as<T>(), split, st)) < 0) return 2;
+        e->launches += n;
+        if ((n = decoder_conv<T>(p.conv, e->vox1.as<T>(), e->dec_conv[1], X, Y, Z, c.out_dim, e->vox2.as<T>(), split, st)) < 0)
+            return 2;
+        e->launches += n;
     } else {
-        const bool tc = p.conv == FramePlan::CONV_TC;
         {
             ProfScope ps(e, st, CAT_CONV);
-            if (tc) {
-                if (launch_conv3d_tc(e->vox0.as<bf16>(), e->conv_wh[0].as<bf16>(), e->conv_b[0].as<float>(), X, Y, Z, mid,
-                                     e->vox1.as<bf16>(), st)) return 2;
-            } else if (launch_conv3d_simt<T>(e->vox0.as<T>(), e->conv_w[0].as<float>(), e->conv_b[0].as<float>(), X, Y, Z,
-                                             mid, e->vox1.as<T>(), st)) return 2;
-            e->launches++;
+            if ((n = decoder_conv<T>(p.conv, e->vox0.as<T>(), e->dec_conv[0], X, Y, Z, mid, e->vox1.as<T>(), split, st)) < 0)
+                return 2;
+            e->launches += n;
         }
         ProfScope ps(e, st, CAT_CONV);
-        if (tc) {
-            if (launch_conv3d_tc(e->vox1.as<bf16>(), e->conv_wh[1].as<bf16>(), e->conv_b[1].as<float>(), X, Y, Z, c.out_dim,
-                                 e->vox2.as<bf16>(), st)) return 2;
-        } else if (launch_conv3d_simt<T>(e->vox1.as<T>(), e->conv_w[1].as<float>(), e->conv_b[1].as<float>(), X, Y, Z,
-                                         c.out_dim, e->vox2.as<T>(), st)) return 2;
-        e->launches++;
+        if ((n = decoder_conv<T>(p.conv, e->vox1.as<T>(), e->dec_conv[1], X, Y, Z, c.out_dim, e->vox2.as<T>(), split, st)) < 0)
+            return 2;
+        e->launches += n;
     }
     ProfScope ps(e, st, CAT_HEAD);
-    if (p.head_tc) {
-        if (launch_occ_head_tc(e->vox2.as<bf16>(), e->head_w1h.as<bf16>(), e->head_w2h.as<bf16>(), e->head_b1c.as<float>(),
-                               e->head_b2c.as<float>(), c.num_classes, nvox, out.occ_logits, out.flow, out.cls_u8,
-                               out.cls_i64, st)) return 2;
-    } else {
-        const HeadWeights hw{e->hw1.as<float>(), e->hb1.as<float>(), e->hw2.as<float>(), e->hb2.as<float>(),
-                             e->fw1.as<float>(), e->fb1.as<float>(), e->fw2.as<float>(), e->fb2.as<float>(), c.num_classes};
-        if (launch_occ_head<T>(e->vox2.as<T>(), hw, nvox, out.occ_logits, out.flow, out.cls_u8, out.cls_i64, st)) return 2;
-    }
-    e->launches++;
+    if ((n = decoder_head<T>(p.head_tc, e->vox2.as<T>(), e->head, c.num_classes, nvox, out.occ_logits, out.flow, out.cls_u8,
+                             out.cls_i64, st)) < 0) return 2;
+    e->launches += n;
     return 0;
 }
 
@@ -1227,7 +1343,7 @@ int occb200_engine_finalize(occb200_engine* e)
         if (e->sca_value_all.alloc((size_t)c.num_layers * c.num_cams * e->Nv * C * 2)) return 2;
         OCC_CUDA(cudaMemset(e->sca_value_all.p, 0, e->sca_value_all.bytes));
     }
-    // decoder: fold BatchNorm3d (eval) into the conv weights; torch layout [Cout][Cin][kz][ky][kx] -> [tap][Cin][Cout]
+    // decoder: BatchNorm3d (eval) folded into the conv weights, laid out for the plan's path; the heads' weights
     for (int i = 0; i < 2; ++i) {
         const int cin = i == 0 ? mid : od;
         const std::string pre = "transformer.decoder." + std::to_string(i);
@@ -1236,35 +1352,7 @@ int occb200_engine_finalize(occb200_engine* e)
         GETP(b, pre + ".bn.bias", (size_t)od);
         GETP(m, pre + ".bn.running_mean", (size_t)od);
         GETP(v, pre + ".bn.running_var", (size_t)od);
-        std::vector<float> wf((size_t)27 * cin * od), bf(od);
-        for (int co = 0; co < od; ++co) {
-            const float s = (*g)[co] / sqrtf((*v)[co] + 1e-5f);
-            bf[co] = (*b)[co] - (*m)[co] * s;
-            for (int ci = 0; ci < cin; ++ci)
-                for (int t = 0; t < 27; ++t)
-                    wf[((size_t)t * cin + ci) * od + co] = (*W)[((size_t)co * cin + ci) * 27 + t] * s;
-        }
-        if (upload(e->conv_w[i], wf.data(), wf.size()) || upload(e->conv_b[i], bf.data(), bf.size())) return 2;
-        if (p.conv == FramePlan::CONV_TC) {                   // tensor-core layout: [tap][cout][cin], K-major rows
-            std::vector<float> wt((size_t)27 * od * cin);
-            for (int t = 0; t < 27; ++t)
-                for (int co = 0; co < od; ++co)
-                    for (int ci = 0; ci < cin; ++ci)
-                        wt[((size_t)t * od + co) * cin + ci] = wf[((size_t)t * cin + ci) * od + co];
-            if (upload_bf16(e->conv_wh[i], wt.data(), wt.size())) return 2;
-        }
-        if (p.conv == FramePlan::CONV_SPLIT) {                // same layout, split into bf16 hi + lo (3-pass fp32-grade convolution)
-            std::vector<float> hi((size_t)27 * od * cin), lo(hi.size());
-            for (int t = 0; t < 27; ++t)
-                for (int co = 0; co < od; ++co)
-                    for (int ci = 0; ci < cin; ++ci) {
-                        const float w = wf[((size_t)t * cin + ci) * od + co];
-                        const float h = __bfloat162float(__float2bfloat16(w));
-                        hi[((size_t)t * od + co) * cin + ci] = h;
-                        lo[((size_t)t * od + co) * cin + ci] = w - h;
-                    }
-            if (upload_bf16(e->conv_wh_hi[i], hi.data(), hi.size()) || upload_bf16(e->conv_wh_lo[i], lo.data(), lo.size())) return 2;
-        }
+        if (upload_decoder_conv(e->dec_conv[i], p.conv, W->data(), g->data(), b->data(), m->data(), v->data(), cin, od)) return 2;
     }
     {
         GETP(w1, "transformer.predicter.0.weight", (size_t)2 * od * od);
@@ -1275,24 +1363,8 @@ int occb200_engine_finalize(occb200_engine* e)
         GETP(g1, "transformer.flow_predicter.0.bias", (size_t)2 * od);
         GETP(f2, "transformer.flow_predicter.2.weight", (size_t)2 * 2 * od);
         GETP(g2, "transformer.flow_predicter.2.bias", (size_t)2);
-        if (upload(e->hw1, w1->data(), w1->size()) || upload(e->hb1, b1->data(), b1->size()) ||
-            upload(e->hw2, w2->data(), w2->size()) || upload(e->hb2, b2->data(), b2->size()) ||
-            upload(e->fw1, f1->data(), f1->size()) || upload(e->fb1, g1->data(), g1->size()) ||
-            upload(e->fw2, f2->data(), f2->size()) || upload(e->fb2, g2->data(), g2->size())) return 2;
-        if (p.head_tc) {                                          // tensor-core head: concatenated / block-diagonal weights
-            const int H = 2 * od, nc = c.num_classes;
-            std::vector<float> w1c((size_t)2 * H * od), b1c(2 * H), w2c((size_t)32 * 2 * H, 0.f), b2c(nc + 2);
-            for (int i = 0; i < H * od; ++i) { w1c[i] = (*w1)[i]; w1c[(size_t)H * od + i] = (*f1)[i]; }
-            for (int i = 0; i < H; ++i) { b1c[i] = (*b1)[i]; b1c[H + i] = (*g1)[i]; }
-            for (int r = 0; r < nc; ++r)
-                for (int k = 0; k < H; ++k) w2c[(size_t)r * 2 * H + k] = (*w2)[(size_t)r * H + k];
-            for (int r = 0; r < 2; ++r)
-                for (int k = 0; k < H; ++k) w2c[(size_t)(nc + r) * 2 * H + H + k] = (*f2)[(size_t)r * H + k];
-            for (int i = 0; i < nc; ++i) b2c[i] = (*b2)[i];
-            b2c[nc] = (*g2)[0]; b2c[nc + 1] = (*g2)[1];
-            if (upload_bf16(e->head_w1h, w1c.data(), w1c.size()) || upload_bf16(e->head_w2h, w2c.data(), w2c.size()) ||
-                upload(e->head_b1c, b1c.data(), b1c.size()) || upload(e->head_b2c, b2c.data(), b2c.size())) return 2;
-        }
+        if (upload_decoder_head(e->head, p.head_tc, c.num_classes, od, w1->data(), b1->data(), w2->data(), b2->data(), f1->data(),
+                                g1->data(), f2->data(), g2->data())) return 2;
     }
     // workspace
     const size_t es = e->elt();
@@ -1825,5 +1897,77 @@ int occb200_sca_gather(const void* value, int value_bf16, const void* qproj, int
                                    hits, st);
 }
 #undef OCC_CHECK_GATHER_TYPES
+
+// ---- the voxel decoder's steps for operator tests: the route make_frame_plan picks for (precision, use_tensor_cores,
+// num_classes) with pillar_h 16 and out_dim 32, weights built by the engine's helpers, then the step the frame runs.  Every
+// rejection returns 1 before the first CUDA call; each entry synchronises `stream` (its weights are freed on return).
+#define OCC_CHECK_DECODER_CONFIG(precision, use_tensor_cores)                          \
+    OCC_CHECK(precision == 0 || precision == 1, "precision must be 0 (fp32) or 1 (bf16)"); \
+    OCC_CHECK(use_tensor_cores == 0 || use_tensor_cores == 1, "use_tensor_cores must be 0 or 1")
+
+int occb200_decoder_lift(int precision, int use_tensor_cores, int from_t32, const float* bev, int bev_h, int bev_w, void* vox,
+                         int* launches, void* stream)
+{
+    OCC_CHECK(bev && vox && launches, "null pointer");
+    OCC_CHECK_DECODER_CONFIG(precision, use_tensor_cores);
+    const FramePlan p = decoder_test_plan(precision, use_tensor_cores, 17);
+    OCC_CHECK(from_t32 == 0 || (from_t32 == 1 && p.lift_t32), "from_t32 must be 0, or 1 with bf16 storage and tensor cores");
+    OCC_CHECK(bev_h > 0 && bev_w > 0 && (int64_t)bev_h * bev_w <= (1 << 24), "the BEV grid must be positive, at most 2^24 cells");
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int n = precision ? decoder_lift<bf16>(from_t32 != 0, bev, bev_h, bev_w, 16, reinterpret_cast<bf16*>(vox), st)
+                            : decoder_lift<float>(false, bev, bev_h, bev_w, 16, reinterpret_cast<float*>(vox), st);
+    if (n < 0) return 2;
+    OCC_CUDA(cudaStreamSynchronize(st));
+    *launches = n;
+    return 0;
+}
+
+int occb200_decoder_conv3d(int precision, int use_tensor_cores, const void* in, int X, int Y, int cin, const float* w_host,
+                           const float* bn_host, void* out, int* path, int* launches, void* stream)
+{
+    OCC_CHECK(in && w_host && bn_host && out && path && launches, "null pointer");
+    OCC_CHECK_DECODER_CONFIG(precision, use_tensor_cores);
+    OCC_CHECK(X >= 1 && X <= 4096 && Y >= 1 && Y <= 4096, "X and Y must be in [1, 4096]");
+    OCC_CHECK(cin == 16 || cin == 32, "cin must be 16 or 32");
+    const FramePlan p = decoder_test_plan(precision, use_tensor_cores, 17);
+    const int od = 32;
+    DecoderConvW w;
+    if (upload_decoder_conv(w, p.conv, w_host, bn_host, bn_host + od, bn_host + 2 * od, bn_host + 3 * od, cin, od)) return 2;
+    DevBuf split;                                                   // CONV_SPLIT: the [hi | lo] operand, as the frame's vox_split
+    if (p.conv == FramePlan::CONV_SPLIT && split.alloc((size_t)X * Y * 16 * 2 * cin * 2)) return 2;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int n = precision ? decoder_conv<bf16>(p.conv, reinterpret_cast<const bf16*>(in), w, X, Y, 16, cin,
+                                                 reinterpret_cast<bf16*>(out), split.as<bf16>(), st)
+                            : decoder_conv<float>(p.conv, reinterpret_cast<const float*>(in), w, X, Y, 16, cin,
+                                                  reinterpret_cast<float*>(out), split.as<bf16>(), st);
+    if (n < 0) return 2;
+    OCC_CUDA(cudaStreamSynchronize(st));
+    *path = p.conv; *launches = n;
+    return 0;
+}
+
+int occb200_decoder_head(int precision, int use_tensor_cores, int num_classes, const void* vox, int64_t nvox, const float* w1,
+                         const float* b1, const float* w2, const float* b2, const float* f1, const float* g1, const float* f2,
+                         const float* g2, float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, int* path,
+                         int* launches, void* stream)
+{
+    OCC_CHECK(vox && w1 && b1 && w2 && b2 && f1 && g1 && f2 && g2 && path && launches, "null pointer");
+    OCC_CHECK_DECODER_CONFIG(precision, use_tensor_cores);
+    OCC_CHECK(num_classes >= 1 && num_classes <= 32, "num_classes must be in [1, 32]");
+    OCC_CHECK(nvox >= 1 && nvox < (1ll << 31), "nvox must be in [1, 2^31)");
+    const FramePlan p = decoder_test_plan(precision, use_tensor_cores, num_classes);
+    DecoderHeadW h;
+    if (upload_decoder_head(h, p.head_tc, num_classes, 32, w1, b1, w2, b2, f1, g1, f2, g2)) return 2;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int n = precision ? decoder_head<bf16>(p.head_tc, reinterpret_cast<const bf16*>(vox), h, num_classes, nvox, occ_logits,
+                                                 flow, cls_u8, cls_i64, st)
+                            : decoder_head<float>(false, reinterpret_cast<const float*>(vox), h, num_classes, nvox, occ_logits,
+                                                  flow, cls_u8, cls_i64, st);
+    if (n < 0) return 2;
+    OCC_CUDA(cudaStreamSynchronize(st));
+    *path = p.head_tc ? 1 : 0; *launches = n;
+    return 0;
+}
+#undef OCC_CHECK_DECODER_CONFIG
 
 }  // extern "C"

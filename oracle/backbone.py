@@ -114,6 +114,14 @@ def fold_conv(p, conv, bn, conv_bias=False):
     return w * scale[:, None, None, None], shift
 
 
+def fold_conv3d_bn(w, gamma, beta, mean, var):
+    """The frame engine's BatchNorm3d fold of the voxel decoder (engine.cu fold_conv3d_bn) in fp32: weight [co, ci, 3, 3, 3] *
+    scale, bias = beta - mean * scale, scale = gamma / sqrt(var + eps), the root correctly rounded as in fold_conv."""
+    var = var.float() + torch.tensor(BN_EPS, dtype=torch.float32)
+    scale = gamma.float() / torch.sqrt(var.double()).float()
+    return w.float() * scale[:, None, None, None, None], beta.float() - mean.float() * scale
+
+
 def storage_model(p, img, storage=torch.bfloat16, tensor_cores=True, rounding=True):
     """Storage-rounding model of the engine's ResNet-50 + FPN: exact (fp64) sums over the engine's operands, and a rounding
     to `storage` at every point where the engine stores one (rounding=False: none, i.e. the fp32 oracle's algorithm in fp64):
