@@ -400,6 +400,42 @@ int occb200_decoder_head(int precision, int use_tensor_cores, int num_classes, c
                          const float* g2, float* occ_logits, float* flow, uint8_t* cls_u8, int64_t* cls_i64, int* path,
                          int* launches, void* stream);
 
+/* The encoder's unfused kernels, for operator tests: what the frame engine launches for a configuration (precision,
+ * use_tensor_cores), on weights prepared by the engine's own helper.  Storage is fp32 (precision 0) or bf16 (precision 1).
+ * Every array is a dense row-major device array, 16-byte aligned, unless marked HOST.  Every rejection returns 1 before any
+ * CUDA call.  Each entry synchronises `stream`.
+ *   encoder_dense: out [M,N] = act([A | A2] . W^T + bias) (+ residual): ReLU (act 1) before the residual add, as every dense
+ *     layer of the engine, on the route make_frame_plan's plan picks for the shape.  A: storage type [M,K], or with A2 != NULL
+ *     the concatenation [A (M x K1) | A2 (M x (K - K1))], 0 < K1 < K, K1 % 8 == 0 (K1 must be 0 without A2).  w_host: HOST
+ *     fp32 [N][K]; bias_host: HOST fp32 [N] or NULL; residual: fp32 [M,N] or NULL.  K % 16 == 0, N % 4 == 0, M >= 0.
+ *     out_dtype 0 fp32, 1 bf16, 2 fp16: the storage type or fp32, or fp16 where the plan writes its sampling projections in
+ *     fp16 (bf16 storage and tensor cores), on shapes the tensor-core route takes.  *path: OCCB200_DENSE_*; *launches: the
+ *     kernels launched (2 on the split route: the entry splits A itself).
+ *   encoder_layernorm: LayerNorm over rows x 256 (eps 1e-5) of x fp32: y_f32 fp32, y_t = T(y), y_pos_t = T(y + pos) (the add
+ *     in fp32).  Any output may be NULL; y_pos_t needs pos.  rows >= 1.
+ *   encoder_pack: tokens [num_cams, Nv, 256] = (level + cams_embeds[cam]) + level_embeds[l] in the storage type, levels in
+ *     order, Nv = sum h_l w_l <= 2^24.  layout 0: fp32 NCHW levels [num_cams, 256, h, w]; 1: bf16 NCHW; 2: bf16 NHWC
+ *     [num_cams, h, w, 256].  feats_dev: HOST array of num_levels (1..8) device pointers; level_hw_host: HOST h0 w0 h1 w1 ..;
+ *     cams_embeds [num_cams,256] or NULL; level_embeds [num_levels,256]; num_cams in 1..8.
+ *   encoder_prepare_query: over n (a multiple of 8) floats of q and pos: q_f32 = q (tiled: in the T32 layout of the residual
+ *     stream, n a multiple of 256), q_t = T(q), q_pos_t = T(q + pos).  Any output may be NULL.
+ *   t32_convert: fp32 [rows, ncols] row-major -> the T32 block layout (32 x 32 blocks of [col % 32 / 4][row % 32][4], rows
+ *     padded to a multiple of 32), or back with untile; ncols a positive multiple of 32.  Pad rows are neither read nor
+ *     written. */
+#define OCCB200_DENSE_CUDA_CORES 0     /* gemm_simt: fp32 weights, fp32 accumulation */
+#define OCCB200_DENSE_TC 1             /* gemm_tc: bf16 weights and operands, fp32 accumulation */
+#define OCCB200_DENSE_SPLIT 2          /* gemm_tc_split3 on bf16 hi / lo splits of fp32 operands and weights */
+int occb200_encoder_dense(int precision, int use_tensor_cores, const void* A, const void* A2, int K1, const float* w_host,
+                          const float* bias_host, const float* residual, void* out, int out_dtype, int M, int N, int K, int act,
+                          int* path, int* launches, void* stream);
+int occb200_encoder_layernorm(int precision, const float* x, const float* gamma, const float* beta, const float* pos, int rows,
+                              float* y_f32, void* y_t, void* y_pos_t, void* stream);
+int occb200_encoder_pack(int precision, int layout, const void* const* feats_dev, int num_levels, const int* level_hw_host,
+                         int num_cams, const float* cams_embeds, const float* level_embeds, void* tokens, void* stream);
+int occb200_encoder_prepare_query(int precision, int tiled, const float* q, const float* pos, int64_t n, float* q_f32, void* q_t,
+                                  void* q_pos_t, void* stream);
+int occb200_t32_convert(const float* src, float* dst, int64_t rows, int untile, int ncols, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Image backbone + neck (SURVEY 8f rank 1, the step immediately BEFORE the hot path); parity vs its oracle:
  * tests/test_backbone_gpu.py (fp32 1e-3 relative to the feature magnitude, bf16 bars stated there).

@@ -76,6 +76,12 @@ SIGNATURES = {
     'occb200_decoder_conv3d': (_i, [_i, _i, _vp, _i, _i, _i, _vp, _vp, _vp, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
     'occb200_decoder_head': (_i, [_i, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                   ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
+    'occb200_encoder_dense': (_i, [_i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, ctypes.POINTER(_i),
+                                   ctypes.POINTER(_i), _vp]),
+    'occb200_encoder_layernorm': (_i, [_i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    'occb200_encoder_pack': (_i, [_i, _i, ctypes.POINTER(_vp), _i, _vp, _i, _vp, _vp, _vp, _vp]),
+    'occb200_encoder_prepare_query': (_i, [_i, _i, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
+    'occb200_t32_convert': (_i, [_vp, _vp, _i64, _i, _i, _vp]),
     'occb200_backbone_create': (_vp, [_i, _i, _i, _i, _i]),
     'occb200_backbone_destroy': (None, [_vp]),
     'occb200_backbone_load_param': (_i, [_vp, ctypes.c_char_p, _vp, ctypes.c_int64]),

@@ -333,13 +333,14 @@ int upload_decoder_head(DecoderHeadW& h, bool head_tc, int nc, int od, const flo
 
 // ---- geometry of the fused spatial cross-attention gather: built here for the engine (creation, set_cameras) and for the
 // occb200_sca_gather test entry alike, so that the operator tests launch the kernels on exactly what the engine builds
-// the four value-map levels of every camera, rows [start, start + h*w) of the [Nv, 256] map; *Nv = the total
-LevelGeom make_level_geom(const int* level_h, const int* level_w, int* Nv)
+// the value-map levels of every camera (four in the engine, up to eight for the occb200_encoder_pack test entry), rows
+// [start, start + h*w) of the [Nv, 256] map; *Nv = the total
+LevelGeom make_level_geom(const int* level_h, const int* level_w, int* Nv, int num_levels = 4)
 {
     LevelGeom lg{};
-    lg.num_levels = 4;
+    lg.num_levels = num_levels;
     int start = 0;
-    for (int l = 0; l < 4; ++l) {
+    for (int l = 0; l < num_levels; ++l) {
         lg.h[l] = level_h[l]; lg.w[l] = level_w[l]; lg.start[l] = start;
         start += level_h[l] * level_w[l];
     }
@@ -455,40 +456,92 @@ FramePlan decoder_test_plan(int precision, int use_tensor_cores, int num_classes
     return make_frame_plan(c, 1);
 }
 
-// ---- GEMM dispatch: the plan's tensor-core path where the shape allows it, the CUDA-core path otherwise
+// the plan of the occb200_encoder_* test entries: a configuration with the engine's attention shapes (4 levels, 8 SCA and 4 TSA
+// points), so that the plan's fp16 sampling projections are what a frame gets
+FramePlan encoder_test_plan(int precision, int use_tensor_cores)
+{
+    occb200_config c;
+    memset(&c, 0, sizeof(c));
+    c.precision = precision; c.use_tensor_cores = use_tensor_cores;
+    c.num_levels = 4; c.sca_points = 8; c.tsa_points = 4;
+    return make_frame_plan(c, 1);
+}
+
+bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+// ---- dense layers (nn.Linear, W [n][k]): built here for the engine (finalize) and for the occb200_encoder_dense test entry
+// alike.  fp32 W and bias on every route (bias may be NULL); for the plan's tensor-core route `wh` (NULL: none) gets the bf16
+// copy (tc_bf16) or [W_hi | W_hi | W_lo] (tc_split).
+int upload_dense(const FramePlan& p, DevBuf& w, DevBuf& b, DevBuf* wh, const float* W, const float* B, size_t n, size_t k)
+{
+    if (upload(w, W, n * k) || (B && upload(b, B, n))) return 2;
+    if (p.tc_bf16 && wh && upload_bf16(*wh, W, n * k)) return 2;
+    if (p.tc_split && wh && upload_w3(*wh, W, n, k)) return 2;
+    return 0;
+}
+
+// The route of one dense layer (OCCB200_DENSE_*): the plan's tensor-core GEMM where the shape allows it, the CUDA-core GEMM
+// otherwise.  Ka: the width of the first operand block (K without a second block).
+template <typename TA, typename TC>
+int dense_route(const FramePlan& p, int M, int N, int K, int Ka)
+{
+    if constexpr (sizeof(TA) == 2)
+        if (p.tc_bf16 && gemm_tc_supported(M, N, K, Ka)) return OCCB200_DENSE_TC;
+    if constexpr (sizeof(TA) == 4 && std::is_same<TC, float>::value)
+        if (p.tc_split && gemm_tc_supported(M, N, 3 * K, 2 * K)) return OCCB200_DENSE_SPLIT;
+    return OCCB200_DENSE_CUDA_CORES;
+}
+
+// C = act([A | A2] . W^T + bias) (+ residual) on the plan's route, run by the engine's gemm() and by occb200_encoder_dense.
+// Enqueues on `st` and returns how many kernels it launched, or -1 when a launcher failed (its message is set).  W: fp32
+// [N][K]; Wh: the route's weight copy (upload_dense).  The split route first splits the operand into `split_ws` ([M, 2K]
+// bf16) unless `A_split` holds it already split (the camera tokens, once per frame).
+template <typename TA, typename TC>
+int dense_gemm(const FramePlan& p, const TA* A, const TA* A2, int K1, const float* W, const void* Wh, const float* bias,
+               const float* residual, TC* C, int M, int N, int K, int act, bf16* split_ws, cudaStream_t st,
+               const bf16* A_split = nullptr)
+{
+    const int Ka = A2 ? K1 : K;
+    const int route = dense_route<TA, TC>(p, M, N, K, Ka);
+    if constexpr (sizeof(TA) == 2) {
+        if (route == OCCB200_DENSE_TC)
+            return gemm_tc<TC>(reinterpret_cast<const bf16*>(A), reinterpret_cast<const bf16*>(A2), K1,
+                               reinterpret_cast<const bf16*>(Wh), bias, residual, C, M, N, K, act, st) ? -1 : 1;
+    }
+    if constexpr (sizeof(TA) == 4 && std::is_same<TC, float>::value) {
+        // fp32 storage + tensor cores: operand split into bf16 hi/lo, weights [W_hi | W_hi | W_lo], three passes in one
+        // wgmma GEMM (relative error ~2^-16: fp32-grade)
+        if (route == OCCB200_DENSE_SPLIT) {
+            const bf16* S = A_split;
+            if (S == nullptr) {
+                if (launch_split_bf16(reinterpret_cast<const float*>(A), Ka, reinterpret_cast<const float*>(A2), K - Ka, M,
+                                      split_ws, st)) return -1;
+                S = split_ws;
+            }
+            if (gemm_tc_split3(S, K, reinterpret_cast<const bf16*>(Wh), bias, residual, C, M, N, act, st)) return -1;
+            return A_split ? 1 : 2;
+        }
+    }
+    if constexpr (std::is_same<TC, __half>::value) {
+        set_last_error("gemm: fp16 outputs exist only on the tensor-core path");
+        return -1;
+    } else {
+        if (gemm_simt<TA, TC>(A, Ka, A2, A2 ? K - K1 : 0, K1, W, bias, residual, N, C, N, M, N, K, act, st)) return -1;
+        return M > 0 ? 1 : 0;
+    }
+}
+
+// ---- the engine's GEMM: dense_gemm on the engine's plan and split workspace, counted and profiled as one GEMM
 template <typename TA, typename TC>
 int gemm(occb200_engine* e, const TA* A, const TA* A2, int K1, const float* W, const void* Wh, const float* bias,
          const float* residual, TC* C, int M, int N, int K, int act, cudaStream_t st, const bf16* A_split = nullptr)
 {
-    e->launches++;
     ProfScope ps(e, st, CAT_GEMM);
-    if constexpr (sizeof(TA) == 2) {
-        if (e->plan.tc_bf16 && gemm_tc_supported(M, N, K, A2 != nullptr ? K1 : K)) {
-            return gemm_tc<TC>(reinterpret_cast<const bf16*>(A), reinterpret_cast<const bf16*>(A2), K1,
-                               reinterpret_cast<const bf16*>(Wh), bias, residual, C, M, N, K, act, st);
-        }
-    }
-    if constexpr (sizeof(TA) == 4 && std::is_same<TC, float>::value) {
-        // fp32 storage + tensor cores: operand split into bf16 hi/lo, weights [W_hi | W_hi | W_lo], three passes in one
-        // wgmma GEMM (relative error ~2^-16: fp32-grade).  `A_split`: A already split (the camera tokens, once per frame).
-        if (e->plan.tc_split && gemm_tc_supported(M, N, 3 * K, 2 * K)) {
-            const bf16* S = A_split;
-            if (S == nullptr) {
-                const int Ka = A2 ? K1 : K;
-                if (launch_split_bf16(reinterpret_cast<const float*>(A), Ka, reinterpret_cast<const float*>(A2), K - Ka, M,
-                                      e->split_ws.as<bf16>(), st)) return 2;
-                e->launches++;
-                S = e->split_ws.as<bf16>();
-            }
-            return gemm_tc_split3(S, K, reinterpret_cast<const bf16*>(Wh), bias, residual, C, M, N, act, st);
-        }
-    }
-    if constexpr (std::is_same<TC, __half>::value) {
-        OCC_CHECK(false, "gemm: fp16 outputs exist only on the tensor-core path");
-    } else {
-        const int lda = A2 ? K1 : K;
-        return gemm_simt<TA, TC>(A, lda, A2, A2 ? K - K1 : 0, K1, W, bias, residual, N, C, N, M, N, K, act, st);
-    }
+    const int n = dense_gemm<TA, TC>(e->plan, A, A2, K1, W, Wh, bias, residual, C, M, N, K, act, e->split_ws.as<bf16>(), st,
+                                     A_split);
+    if (n < 0) return 2;
+    e->launches += n;
+    return 0;
 }
 
 // y = LayerNorm(A.W^T + b + residual): one wgmma kernel (GEMM with LayerNorm epilogue) on the tensor-core path
@@ -1264,10 +1317,7 @@ int occb200_engine_finalize(occb200_engine* e)
             const std::vector<float>* W = find(e, name + ".weight", n * k);
             const std::vector<float>* B = find(e, name + ".bias", n);
             if (!W || !B) return 3;
-            if (upload(wbuf, W->data(), W->size()) || upload(bbuf, B->data(), B->size())) return 2;
-            if (p.tc_bf16 && wh && upload_bf16(*wh, W->data(), W->size())) return 2;
-            if (p.tc_split && wh && upload_w3(*wh, W->data(), n, k)) return 2;
-            return 0;
+            return upload_dense(p, wbuf, bbuf, wh, W->data(), B->data(), n, k);
         };
         auto up_cat = [&](DevBuf& wbuf, DevBuf& bbuf, DevBuf* wh, const std::string& n1, const std::string& n2,
                           size_t r1, size_t r2, size_t k, DevBuf* fold = nullptr, DevBuf* fold_const = nullptr) -> int {
@@ -1279,9 +1329,7 @@ int occb200_engine_finalize(occb200_engine* e)
             std::vector<float> W(*W1), B(*B1);
             W.insert(W.end(), W2->begin(), W2->end());
             B.insert(B.end(), B2->begin(), B2->end());
-            if (upload(wbuf, W.data(), W.size()) || upload(bbuf, B.data(), B.size())) return 2;
-            if (p.tc_bf16 && wh && upload_bf16(*wh, W.data(), W.size())) return 2;
-            if (p.tc_split && wh && upload_w3(*wh, W.data(), r1 + r2, k)) return 2;
+            if (upload_dense(p, wbuf, bbuf, wh, W.data(), B.data(), r1 + r2, k)) return 2;
             if (p.tc_bf16 && p.qproj_f16 && fold) {              // k = 2C: (W1 + W2) [r, C] bf16 and the constant W2 pos + b
                 const size_t half = k / 2, rows = r1 + r2;
                 std::vector<float> Wf(rows * half), W2h(rows * half);
@@ -1901,7 +1949,7 @@ int occb200_sca_gather(const void* value, int value_bf16, const void* qproj, int
 // ---- the voxel decoder's steps for operator tests: the route make_frame_plan picks for (precision, use_tensor_cores,
 // num_classes) with pillar_h 16 and out_dim 32, weights built by the engine's helpers, then the step the frame runs.  Every
 // rejection returns 1 before the first CUDA call; each entry synchronises `stream` (its weights are freed on return).
-#define OCC_CHECK_DECODER_CONFIG(precision, use_tensor_cores)                          \
+#define OCC_CHECK_PLAN_CONFIG(precision, use_tensor_cores)                                 \
     OCC_CHECK(precision == 0 || precision == 1, "precision must be 0 (fp32) or 1 (bf16)"); \
     OCC_CHECK(use_tensor_cores == 0 || use_tensor_cores == 1, "use_tensor_cores must be 0 or 1")
 
@@ -1909,7 +1957,7 @@ int occb200_decoder_lift(int precision, int use_tensor_cores, int from_t32, cons
                          int* launches, void* stream)
 {
     OCC_CHECK(bev && vox && launches, "null pointer");
-    OCC_CHECK_DECODER_CONFIG(precision, use_tensor_cores);
+    OCC_CHECK_PLAN_CONFIG(precision, use_tensor_cores);
     const FramePlan p = decoder_test_plan(precision, use_tensor_cores, 17);
     OCC_CHECK(from_t32 == 0 || (from_t32 == 1 && p.lift_t32), "from_t32 must be 0, or 1 with bf16 storage and tensor cores");
     OCC_CHECK(bev_h > 0 && bev_w > 0 && (int64_t)bev_h * bev_w <= (1 << 24), "the BEV grid must be positive, at most 2^24 cells");
@@ -1926,7 +1974,7 @@ int occb200_decoder_conv3d(int precision, int use_tensor_cores, const void* in, 
                            const float* bn_host, void* out, int* path, int* launches, void* stream)
 {
     OCC_CHECK(in && w_host && bn_host && out && path && launches, "null pointer");
-    OCC_CHECK_DECODER_CONFIG(precision, use_tensor_cores);
+    OCC_CHECK_PLAN_CONFIG(precision, use_tensor_cores);
     OCC_CHECK(X >= 1 && X <= 4096 && Y >= 1 && Y <= 4096, "X and Y must be in [1, 4096]");
     OCC_CHECK(cin == 16 || cin == 32, "cin must be 16 or 32");
     const FramePlan p = decoder_test_plan(precision, use_tensor_cores, 17);
@@ -1952,7 +2000,7 @@ int occb200_decoder_head(int precision, int use_tensor_cores, int num_classes, c
                          int* launches, void* stream)
 {
     OCC_CHECK(vox && w1 && b1 && w2 && b2 && f1 && g1 && f2 && g2 && path && launches, "null pointer");
-    OCC_CHECK_DECODER_CONFIG(precision, use_tensor_cores);
+    OCC_CHECK_PLAN_CONFIG(precision, use_tensor_cores);
     OCC_CHECK(num_classes >= 1 && num_classes <= 32, "num_classes must be in [1, 32]");
     OCC_CHECK(nvox >= 1 && nvox < (1ll << 31), "nvox must be in [1, 2^31)");
     const FramePlan p = decoder_test_plan(precision, use_tensor_cores, num_classes);
@@ -1968,6 +2016,140 @@ int occb200_decoder_head(int precision, int use_tensor_cores, int num_classes, c
     *path = p.head_tc ? 1 : 0; *launches = n;
     return 0;
 }
-#undef OCC_CHECK_DECODER_CONFIG
+
+// ---- the encoder's unfused kernels for operator tests: the plan make_frame_plan makes for (precision, use_tensor_cores) at the
+// engine's attention shapes, dense weights built by the engine's upload_dense, then the GEMM step or launcher the frame runs.
+// Every rejection returns 1 before the first CUDA call; each entry synchronises `stream` (its weights are freed on return).
+int occb200_encoder_dense(int precision, int use_tensor_cores, const void* A, const void* A2, int K1, const float* w_host,
+                          const float* bias_host, const float* residual, void* out, int out_dtype, int M, int N, int K, int act,
+                          int* path, int* launches, void* stream)
+{
+    OCC_CHECK(A && w_host && out && path && launches, "null pointer");
+    OCC_CHECK_PLAN_CONFIG(precision, use_tensor_cores);
+    OCC_CHECK(act == ACT_NONE || act == ACT_RELU, "act must be 0 (none) or 1 (relu)");
+    OCC_CHECK(M >= 0 && N > 0 && N % 4 == 0 && K > 0 && K % 16 == 0, "shape: M >= 0, N a positive multiple of 4, K of 16");
+    OCC_CHECK(A2 ? K1 > 0 && K1 < K && K1 % 8 == 0 : K1 == 0,
+              "split point: 0 < K1 < K and K1 % 8 == 0 with A2, K1 = 0 without");
+    OCC_CHECK(aligned16(A) && aligned16(A2) && aligned16(residual) && aligned16(out), "device arrays must be 16-byte aligned");
+    OCC_CHECK(out_dtype == 0 || (out_dtype == 1 && precision == 1) || out_dtype == 2,
+              "out_dtype must be 0 (fp32), the storage type (1: bf16) or 2 (fp16)");
+    const FramePlan p = encoder_test_plan(precision, use_tensor_cores);
+    const int route = precision ? dense_route<bf16, bf16>(p, M, N, K, A2 ? K1 : K) : dense_route<float, float>(p, M, N, K, A2 ? K1 : K);
+    OCC_CHECK(out_dtype != 2 || (p.qproj_f16 && route == OCCB200_DENSE_TC),
+              "fp16 outputs exist only on the tensor-core route of bf16 storage with tensor cores");
+    DevBuf w, b, wh, split;
+    if (upload_dense(p, w, b, &wh, w_host, bias_host, N, K)) return 2;
+    if (route == OCCB200_DENSE_SPLIT && split.alloc((size_t)M * 2 * K * 2)) return 2;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const float *wf = w.as<float>(), *bf = b.as<float>();
+    bf16* ws = split.as<bf16>();
+    int n;
+    if (precision == 0) {
+        n = dense_gemm<float, float>(p, reinterpret_cast<const float*>(A), reinterpret_cast<const float*>(A2), K1, wf, wh.p, bf,
+                                     residual, reinterpret_cast<float*>(out), M, N, K, act, ws, st);
+    } else {
+        const bf16 *a = reinterpret_cast<const bf16*>(A), *a2 = reinterpret_cast<const bf16*>(A2);
+        n = out_dtype == 0 ? dense_gemm<bf16, float>(p, a, a2, K1, wf, wh.p, bf, residual, reinterpret_cast<float*>(out), M, N, K,
+                                                     act, ws, st)
+          : out_dtype == 1 ? dense_gemm<bf16, bf16>(p, a, a2, K1, wf, wh.p, bf, residual, reinterpret_cast<bf16*>(out), M, N, K,
+                                                    act, ws, st)
+                           : dense_gemm<bf16, __half>(p, a, a2, K1, wf, wh.p, bf, residual, reinterpret_cast<__half*>(out), M, N,
+                                                      K, act, ws, st);
+    }
+    if (n < 0) return 2;
+    OCC_CUDA(cudaStreamSynchronize(st));
+    *path = route; *launches = n;
+    return 0;
+}
+
+int occb200_encoder_layernorm(int precision, const float* x, const float* gamma, const float* beta, const float* pos, int rows,
+                              float* y_f32, void* y_t, void* y_pos_t, void* stream)
+{
+    OCC_CHECK(x && gamma && beta, "null pointer");
+    OCC_CHECK(precision == 0 || precision == 1, "precision must be 0 (fp32) or 1 (bf16)");
+    OCC_CHECK(y_pos_t == nullptr || pos != nullptr, "y_pos_t needs pos");
+    OCC_CHECK(rows >= 1, "rows must be positive");
+    OCC_CHECK(aligned16(x) && aligned16(gamma) && aligned16(beta) && aligned16(pos) && aligned16(y_f32) && aligned16(y_t) &&
+                  aligned16(y_pos_t), "device arrays must be 16-byte aligned");
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int rc = precision ? launch_layernorm<bf16>(x, gamma, beta, pos, rows, 256, y_f32, reinterpret_cast<bf16*>(y_t),
+                                                      reinterpret_cast<bf16*>(y_pos_t), st)
+                             : launch_layernorm<float>(x, gamma, beta, pos, rows, 256, y_f32, reinterpret_cast<float*>(y_t),
+                                                       reinterpret_cast<float*>(y_pos_t), st);
+    if (rc) return rc;
+    OCC_CUDA(cudaStreamSynchronize(st));
+    return 0;
+}
+
+int occb200_encoder_pack(int precision, int layout, const void* const* feats_dev, int num_levels, const int* level_hw_host,
+                         int num_cams, const float* cams_embeds, const float* level_embeds, void* tokens, void* stream)
+{
+    OCC_CHECK(feats_dev && level_hw_host && level_embeds && tokens, "null pointer");
+    OCC_CHECK(precision == 0 || precision == 1, "precision must be 0 (fp32) or 1 (bf16)");
+    OCC_CHECK(layout >= 0 && layout <= 2, "layout must be 0 (fp32 NCHW), 1 (bf16 NCHW) or 2 (bf16 NHWC)");
+    OCC_CHECK(num_levels >= 1 && num_levels <= 8, "num_levels must be in [1, 8]");
+    OCC_CHECK(num_cams >= 1 && num_cams <= 8, "num_cams must be in [1, 8]");
+    int level_h[8], level_w[8];
+    int64_t total = 0;
+    for (int l = 0; l < num_levels; ++l) {
+        level_h[l] = level_hw_host[2 * l]; level_w[l] = level_hw_host[2 * l + 1];
+        OCC_CHECK(level_h[l] >= 1 && level_w[l] >= 1 && (int64_t)level_h[l] * level_w[l] <= (1 << 24),
+                  "every level must be at least 1x1, at most 2^24 pixels");
+        total += (int64_t)level_h[l] * level_w[l];
+        OCC_CHECK(feats_dev[l] != nullptr, "null feature level");
+        OCC_CHECK(aligned16(feats_dev[l]), "device arrays must be 16-byte aligned");
+    }
+    OCC_CHECK(total <= (1 << 24), "the levels must hold at most 2^24 pixels in all");
+    OCC_CHECK(aligned16(cams_embeds) && aligned16(level_embeds) && aligned16(tokens), "device arrays must be 16-byte aligned");
+    int Nv = 0;
+    const LevelGeom lg = make_level_geom(level_h, level_w, &Nv, num_levels);
+    const cudaStream_t st = (cudaStream_t)stream;
+    int rc;
+    if (layout == 2)
+        rc = precision ? launch_pack_levels_nhwc<bf16>(feats_dev, lg, cams_embeds, level_embeds, num_cams, 256, Nv,
+                                                       reinterpret_cast<bf16*>(tokens), st)
+                       : launch_pack_levels_nhwc<float>(feats_dev, lg, cams_embeds, level_embeds, num_cams, 256, Nv,
+                                                        reinterpret_cast<float*>(tokens), st);
+    else
+        rc = precision ? launch_pack_levels<bf16>(feats_dev, layout, lg, cams_embeds, level_embeds, num_cams, 256, Nv,
+                                                  reinterpret_cast<bf16*>(tokens), st)
+                       : launch_pack_levels<float>(feats_dev, layout, lg, cams_embeds, level_embeds, num_cams, 256, Nv,
+                                                   reinterpret_cast<float*>(tokens), st);
+    if (rc) return rc;
+    OCC_CUDA(cudaStreamSynchronize(st));
+    return 0;
+}
+
+int occb200_encoder_prepare_query(int precision, int tiled, const float* q, const float* pos, int64_t n, float* q_f32, void* q_t,
+                                  void* q_pos_t, void* stream)
+{
+    OCC_CHECK(q && pos, "null pointer");
+    OCC_CHECK(precision == 0 || precision == 1, "precision must be 0 (fp32) or 1 (bf16)");
+    OCC_CHECK(tiled == 0 || tiled == 1, "tiled must be 0 or 1");
+    OCC_CHECK(n > 0 && n % 8 == 0 && (!tiled || n % 256 == 0), "n must be a positive multiple of 8 (tiled: of 256)");
+    OCC_CHECK(aligned16(q) && aligned16(pos) && aligned16(q_f32) && aligned16(q_t) && aligned16(q_pos_t),
+              "device arrays must be 16-byte aligned");
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int rc = precision ? launch_prepare_query<bf16>(q, pos, n, q_f32, reinterpret_cast<bf16*>(q_t),
+                                                          reinterpret_cast<bf16*>(q_pos_t), tiled, st)
+                             : launch_prepare_query<float>(q, pos, n, q_f32, reinterpret_cast<float*>(q_t),
+                                                           reinterpret_cast<float*>(q_pos_t), tiled, st);
+    if (rc) return rc;
+    OCC_CUDA(cudaStreamSynchronize(st));
+    return 0;
+}
+
+int occb200_t32_convert(const float* src, float* dst, int64_t rows, int untile, int ncols, void* stream)
+{
+    OCC_CHECK(src && dst, "null pointer");
+    OCC_CHECK(untile == 0 || untile == 1, "untile must be 0 or 1");
+    OCC_CHECK(rows >= 1 && ncols > 0 && ncols % 32 == 0, "rows must be positive, ncols a positive multiple of 32");
+    OCC_CHECK(aligned16(src) && aligned16(dst), "device arrays must be 16-byte aligned");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (launch_t32_convert(src, dst, rows, untile, st, ncols)) return 2;
+    OCC_CUDA(cudaStreamSynchronize(st));
+    return 0;
+}
+#undef OCC_CHECK_PLAN_CONFIG
 
 }  // extern "C"

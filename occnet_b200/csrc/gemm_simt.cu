@@ -2,7 +2,7 @@
 //   C[M,N] = act(A[M,K] . W[N,K]^T + bias[N]) (+ residual[M,N])
 // Every dense layer of the path is an nn.Linear (weight [N,K], K contiguous), reference:
 //   temporal_self_attention.py:99-104, spatial_cross_attention.py:245-249,:67, mmcv FFN.
-// fp32 accumulation; A may be fp32 or bf16, C fp32 or bf16.  The tensor-core (wgmma) path
+// fp32 accumulation; A fp32 with C fp32, or A bf16 with C fp32 or bf16.  The tensor-core (wgmma) path
 // in gemm_tc.cu replaces this for the bf16 configurations.
 #include "common.cuh"
 
@@ -138,7 +138,5 @@ template int gemm_simt<bf16, float>(const bf16*, int, const bf16*, int, int, con
                                     const float*, int, float*, int, int, int, int, int, cudaStream_t);
 template int gemm_simt<bf16, bf16>(const bf16*, int, const bf16*, int, int, const float*, const float*,
                                    const float*, int, bf16*, int, int, int, int, int, cudaStream_t);
-template int gemm_simt<float, bf16>(const float*, int, const float*, int, int, const float*, const float*,
-                                    const float*, int, bf16*, int, int, int, int, int, cudaStream_t);
 
 }  // namespace occ
