@@ -1813,12 +1813,19 @@ int occb200_linear_f32(const float* A, const float* W, const float* bias, const 
                        int K, int act, void* stream)
 {
     OCC_CHECK(A && W && C, "null pointer");
+    OCC_CHECK(M >= 0 && N > 0 && K > 0, "linear: bad sizes");
+    OCC_CHECK(act == ACT_NONE || act == ACT_RELU, "linear: act must be 0 or 1");
+    OCC_CHECK(aligned16(A) && aligned16(W) && aligned16(bias) && aligned16(residual) && aligned16(C),
+              "device arrays must be 16-byte aligned");
     return gemm_simt<float, float>(A, K, nullptr, 0, K, W, bias, residual, N, C, N, M, N, K, act, (cudaStream_t)stream);
 }
 
 int occb200_layernorm_f32(const float* x, const float* gamma, const float* beta, float* y, int rows, int C, void* stream)
 {
     OCC_CHECK(x && gamma && beta && y, "null pointer");
+    OCC_CHECK(rows >= 0, "layernorm: rows must be >= 0");
+    OCC_CHECK(aligned16(x) && aligned16(gamma) && aligned16(beta) && aligned16(y), "device arrays must be 16-byte aligned");
+    if (rows == 0) return 0;
     return launch_layernorm<float>(x, gamma, beta, nullptr, rows, C, y, (float*)nullptr, (float*)nullptr,
                                    (cudaStream_t)stream);
 }

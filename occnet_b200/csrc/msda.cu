@@ -621,7 +621,10 @@ int launch_msda_forward(const float* value, const int64_t* shapes, const int64_t
                         cudaStream_t stream)
 {
     if ((int64_t)B * Nq == 0) return 0;
-    if (C % 8 == 0) {
+    // the 8-channel kernel moves value and out with 16-byte vector loads and stores; mmcv's op takes any contiguous
+    // tensor, so a view whose storage offset is not a multiple of 4 floats runs the per-channel kernel instead
+    const bool vec_ok = (((uintptr_t)value | (uintptr_t)out) & 15) == 0;
+    if (C % 8 == 0 && vec_ok) {
         const int64_t total = (int64_t)B * Nq * M * (C / 8);
         msda_forward_kernel<8><<<ceil_div(total, 256), 256, 0, stream>>>(value, shapes, lstart, loc, wts, B, Nv, M,
                                                                           C, Nq, L, P, out);

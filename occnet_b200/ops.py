@@ -28,15 +28,47 @@ def _require(t, name, dtype=None):
         raise RuntimeError(f'{name} must be {dtype}, got {t.dtype}')
 
 
+def _same_device(ref, *tensors):
+    for t, name in tensors:
+        if t.device != ref.device:
+            raise RuntimeError(f'{name} is on {t.device}, value on {ref.device}: all tensors must be on one device')
+
+
+def _check_shape(t, name, shape):
+    if tuple(t.shape) != tuple(shape):
+        raise RuntimeError(f'{name} has shape {tuple(t.shape)}, expected {tuple(shape)}')
+
+
+def _msda_sizes(value, spatial_shapes, level_start_index, sampling_locations, attention_weights):
+    """(B, Nv, M, C, Nq, L, P) after cross-checking every tensor's shape against value [B, Nv, M, C] and sampling_locations
+    [B, Nq, M, L, P, 2].  The kernels index every buffer with these sizes, so a mismatch would read or write outside it.
+    The CONTENTS of spatial_shapes and level_start_index (each level inside value's Nv rows) stay unchecked, as in mmcv:
+    checking them would need a device-to-host copy and a sync on every call."""
+    if value.dim() != 4:
+        raise RuntimeError(f'value must be [B, Nv, M, C], got shape {tuple(value.shape)}')
+    B, Nv, M, C = value.shape
+    if sampling_locations.dim() != 6:
+        raise RuntimeError(f'sampling_loc must be [B, Nq, M, L, P, 2], got shape {tuple(sampling_locations.shape)}')
+    Nq, L, P = sampling_locations.shape[1], sampling_locations.shape[3], sampling_locations.shape[4]
+    _check_shape(sampling_locations, 'sampling_loc', (B, Nq, M, L, P, 2))
+    _check_shape(attention_weights, 'attn_weight', (B, Nq, M, L, P))
+    _check_shape(spatial_shapes, 'spatial_shapes', (L, 2))
+    _check_shape(level_start_index, 'level_start_index', (L,))
+    _same_device(value, (spatial_shapes, 'spatial_shapes'), (level_start_index, 'level_start_index'),
+                 (sampling_locations, 'sampling_loc'), (attention_weights, 'attn_weight'))
+    return B, Nv, M, C, Nq, L, P
+
+
 def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_locations, attention_weights,
                            im2col_step=64):
+    """mmcv `_ext.ms_deform_attn_forward` drop-in -> out [B, Nq, M*C] fp32.  Any contiguous value is accepted: a view whose
+    storage is not 16-byte aligned runs the per-channel kernel instead of the 8-channel one."""
     _require(value, 'value', torch.float32)
     _require(spatial_shapes, 'spatial_shapes', torch.int64)
     _require(level_start_index, 'level_start_index', torch.int64)
     _require(sampling_locations, 'sampling_loc', torch.float32)
     _require(attention_weights, 'attn_weight', torch.float32)
-    B, Nv, M, C = value.shape
-    _, Nq, _, L, P, _ = sampling_locations.shape
+    B, Nv, M, C, Nq, L, P = _msda_sizes(value, spatial_shapes, level_start_index, sampling_locations, attention_weights)
     out = torch.empty((B, Nq, M * C), dtype=torch.float32, device=value.device)
     lib = _lib.load()
     with torch.cuda.device(value.device):
@@ -48,15 +80,22 @@ def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_lo
 
 def ms_deform_attn_backward(value, spatial_shapes, level_start_index, sampling_locations, attention_weights,
                             grad_output, grad_value, grad_sampling_loc, grad_attn_weight, im2col_step=64):
-    """mmcv `_ext.ms_deform_attn_backward` drop-in: fills the three PRE-ZEROED gradient tensors in place."""
+    """mmcv `_ext.ms_deform_attn_backward` drop-in, in place: grad_value is ACCUMULATED into (pass it zeroed for the
+    gradient alone), grad_sampling_loc and grad_attn_weight are OVERWRITTEN.  Shapes and devices are checked as in
+    `ms_deform_attn_forward`; grad_output must be [B, Nq, M*C] and each gradient the shape of its input."""
     for t, n in ((value, 'value'), (sampling_locations, 'sampling_loc'), (attention_weights, 'attn_weight'),
                  (grad_output, 'grad_output'), (grad_value, 'grad_value'), (grad_sampling_loc, 'grad_sampling_loc'),
                  (grad_attn_weight, 'grad_attn_weight')):
         _require(t, n, torch.float32)
     _require(spatial_shapes, 'spatial_shapes', torch.int64)
     _require(level_start_index, 'level_start_index', torch.int64)
-    B, Nv, M, C = value.shape
-    _, Nq, _, L, P, _ = sampling_locations.shape
+    B, Nv, M, C, Nq, L, P = _msda_sizes(value, spatial_shapes, level_start_index, sampling_locations, attention_weights)
+    _check_shape(grad_output, 'grad_output', (B, Nq, M * C))
+    _check_shape(grad_value, 'grad_value', value.shape)
+    _check_shape(grad_sampling_loc, 'grad_sampling_loc', sampling_locations.shape)
+    _check_shape(grad_attn_weight, 'grad_attn_weight', attention_weights.shape)
+    _same_device(value, (grad_output, 'grad_output'), (grad_value, 'grad_value'),
+                 (grad_sampling_loc, 'grad_sampling_loc'), (grad_attn_weight, 'grad_attn_weight'))
     lib = _lib.load()
     with torch.cuda.device(value.device):
         _lib.check(lib.occb200_ms_deform_attn_backward(
@@ -193,31 +232,67 @@ def _no_autograd(name, *tensors):
                            f'torch.no_grad() or detach the inputs')
 
 
+def _aligned(t):
+    """t itself when its storage is 16-byte aligned (the kernels move it with 16-byte vector accesses), otherwise an
+    aligned copy"""
+    return t if t is None or t.data_ptr() % 16 == 0 else t.clone()
+
+
+def _operand(t, name, shape, x):
+    """fp32, CUDA, contiguous, on x's device, of `shape`"""
+    _require(t, name, torch.float32)
+    if t.device != x.device:
+        raise RuntimeError(f'{name} is on {t.device}, x on {x.device}')
+    _check_shape(t, name, shape)
+
+
 def linear(x, weight, bias=None, residual=None, act=0):
-    """fp32 y = act(x W^T + b) (+ residual) through the CUDA-core GEMM (module-level API mirror)."""
+    """fp32 y = act(x W^T + b) (+ residual) through the CUDA-core GEMM (module-level API mirror).  x [..., K], weight
+    [N, K], bias [N], residual with the M*N elements of the output (it is read as [M, N], it does not broadcast); all fp32,
+    contiguous, on one CUDA device.  K must be a multiple of 16 and N of 4."""
     _no_autograd('linear', x, weight, bias, residual)
     _require(x, 'x', torch.float32)
-    _require(weight, 'weight', torch.float32)
     K = x.shape[-1]
+    if weight is None or getattr(weight, 'dim', lambda: 0)() != 2:
+        raise RuntimeError(f'weight must be [N, K], got {None if weight is None else tuple(weight.shape)}')
     N = weight.shape[0]
+    _operand(weight, 'weight', (N, K), x)
     x2 = x.reshape(-1, K)
-    out = torch.empty((x2.shape[0], N), dtype=torch.float32, device=x.device)
-    res = None if residual is None else residual.reshape(-1, N).contiguous()
+    M = x2.shape[0]
+    if bias is not None:
+        _operand(bias, 'bias', (N,), x)
+    res = None
+    if residual is not None:
+        _require(residual, 'residual', torch.float32)
+        if residual.numel() != M * N:
+            raise RuntimeError(f'residual has shape {tuple(residual.shape)} ({residual.numel()} elements), the output '
+                               f'[{M}, {N}] has {M * N}')
+        res = residual.reshape(M, N)
+        _operand(res, 'residual', (M, N), x)
+    if act not in (0, 1):
+        raise RuntimeError(f'act must be 0 (none) or 1 (ReLU), got {act}')
+    out = torch.empty((M, N), dtype=torch.float32, device=x.device)
+    x2, weight, bias, res = (_aligned(t) for t in (x2, weight, bias, res))     # copies stay alive until the launch
     lib = _lib.load()
     with torch.cuda.device(x.device):
-        _lib.check(lib.occb200_linear_f32(_lib.ptr(x2), _lib.ptr(weight), _lib.ptr(bias), _lib.ptr(res), _lib.ptr(out),
-                                          x2.shape[0], N, K, act, _lib.stream_ptr()))
+        _lib.check(lib.occb200_linear_f32(_lib.ptr(x2), _lib.ptr(weight), _lib.ptr(bias), _lib.ptr(res), _lib.ptr(out), M, N,
+                                          K, act, _lib.stream_ptr()))
     return out.reshape(*x.shape[:-1], N)
 
 
 def layer_norm(x, gamma, beta):
+    """fp32 LayerNorm over the last dimension (eps 1e-5), C = 256: x [..., 256], gamma and beta [256], all fp32,
+    contiguous, on one CUDA device."""
     _no_autograd('layer_norm', x, gamma, beta)
     _require(x, 'x', torch.float32)
     C = x.shape[-1]
+    _operand(gamma, 'gamma', (C,), x)
+    _operand(beta, 'beta', (C,), x)
     x2 = x.reshape(-1, C)
     out = torch.empty_like(x2)
+    x2, gamma, beta = (_aligned(t) for t in (x2, gamma, beta))                  # copies stay alive until the launch
     lib = _lib.load()
     with torch.cuda.device(x.device):
-        _lib.check(lib.occb200_layernorm_f32(_lib.ptr(x2), _lib.ptr(gamma), _lib.ptr(beta), _lib.ptr(out), x2.shape[0],
-                                             C, _lib.stream_ptr()))
+        _lib.check(lib.occb200_layernorm_f32(_lib.ptr(x2), _lib.ptr(gamma), _lib.ptr(beta), _lib.ptr(out), x2.shape[0], C,
+                                             _lib.stream_ptr()))
     return out.reshape(x.shape)

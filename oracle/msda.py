@@ -86,3 +86,122 @@ def msda_loops(value, value_spatial_shapes, level_start_index, sampling_location
                         acc += aw[b, q, m, l, p] * val
                 out[b, q, m] = acc
     return torch.from_numpy(out.reshape(B, Nq, M * C))
+
+
+U24 = 2.0 ** -24          # unit roundoff of fp32
+
+
+def msda_reference(value, shapes, lsi, loc, w, grad_out=None, chunk=2048):
+    """float64 restatement of mmcv's operator, forward and (with grad_out) backward, on the inputs' device.
+
+    value (B, Nv, M, C); shapes (L, 2) [H, W]; lsi (L,) level starts in value's Nv rows (gaps allowed: only the rows a level
+    addresses are read); loc (B, Nq, M, L, P, 2) [x, y]; w (B, Nq, M, L, P); grad_out (B, Nq, M*C).  mmcv's rule:
+      h = y*H - 0.5, x = x*W - 0.5 (in float64 from the stored locations);
+      a sample is skipped unless -1 < h < H and -1 < x < W;
+      corners (floor(h) + {0, 1}, floor(x) + {0, 1}) contribute only inside the level, weights hh*hw, hh*lw, lh*hw, lh*lw;
+      grad_loc = (W, H) * w * sum_c go_c * d bilinear / d(x, h), the one-sided derivative of the floor cell;
+      grad_attn = sum_c go_c * bilinear_c;  grad_value scattered with index_add_.
+    Where the rule differs from F.grid_sample (msda_grid_sample): at h = -1 or x = -1 exactly the sample is skipped, so
+    its value and every gradient are 0, while grid_sample's autograd gives the one-sided derivative into the map.
+
+    Returns a dict of float64 tensors:
+      out (B, Nq, M*C) and out_abs = sum |w * cornerweight * v| over its terms;
+      with grad_out: grad_value (B, Nv, M, C), gv_abs = sum |go * w * cornerweight| and gv_count = the number of
+      (sample, corner) contributions per element (inside corners of valid samples, zero weights included: one atomic add
+      each); grad_attn (B, Nq, M, L, P), ga_abs = sum_c |go_c| * sum_corners cornerweight * |v|; grad_loc
+      (B, Nq, M, L, P, 2), gl_abs = (W, H) * sum_c |go_c w| * (hh(|v1|+|v2|) + lh(|v3|+|v4|), hw(|v1|+|v3|) + lw(|v2|+|v4|))
+      (v1..v4 the top-left, top-right, bottom-left, bottom-right corners, 0 outside).
+      Location sensitivities, for an error d in the pixel coordinates: out_dl = sum |w| (dh A_c + dx B_c), ga_dl =
+      sum_c |go_c| (dh A_c + dx B_c), gv_dl = sum |go w| (dh |d cw / dh| + dx |d cw / dx|) and gl_dl = (W dh, H dx) *
+      |w| sum_c |go_c| (|v1|+|v2|+|v3|+|v4|), with A_c = hw(|v1|+|v3|) + lw(|v2|+|v4|) >= |d bilinear / dh|,
+      B_c = hh(|v1|+|v2|) + lh(|v3|+|v4|) >= |d bilinear / dx| and d the bound 2u(|loc * size| + 1) of fp32's rounding of
+      loc * size - 0.5 (u = 2^-24).  They hold inside one pixel cell: callers keep samples away from pixel lines."""
+    f64 = torch.float64
+    dev = value.device
+    B, Nv, M, C = value.shape
+    _, Nq, _, L, P, _ = loc.shape
+    shapes_h = [(int(h), int(w_)) for h, w_ in shapes.tolist()]
+    starts = [int(s) for s in lsi.tolist()]
+    v64 = value.to(f64)
+    res = {'out': torch.zeros(B, Nq, M, C, dtype=f64, device=dev), 'out_abs': torch.zeros(B, Nq, M, C, dtype=f64, device=dev),
+           'out_dl': torch.zeros(B, Nq, M, C, dtype=f64, device=dev)}
+    bwd = grad_out is not None
+    if bwd:
+        for k in ('grad_value', 'gv_abs', 'gv_count', 'gv_dl'):
+            res[k] = torch.zeros(B * Nv * M, C, dtype=f64, device=dev)
+        for k in ('grad_attn', 'ga_abs', 'ga_dl'):
+            res[k] = torch.zeros(B, Nq, M, L, P, dtype=f64, device=dev)
+        for k in ('grad_loc', 'gl_abs', 'gl_dl'):
+            res[k] = torch.zeros(B, Nq, M, L, P, 2, dtype=f64, device=dev)
+        go_all = grad_out.to(f64).view(B, Nq, M, C)
+    bi = torch.arange(B, device=dev).view(B, 1, 1, 1)
+    mi = torch.arange(M, device=dev).view(1, 1, M, 1)
+    for q0 in range(0, Nq, chunk):
+        q1 = min(Nq, q0 + chunk)
+        nq = q1 - q0
+        if bwd:
+            go = go_all[:, q0:q1, :, None, :]                                     # (B, nq, M, 1, C)
+        for l, (H, W) in enumerate(shapes_h):
+            xy = loc[:, q0:q1, :, l].to(f64)                                      # (B, nq, M, P, 2)
+            wl = w[:, q0:q1, :, l].to(f64)                                        # (B, nq, M, P)
+            x = xy[..., 0] * W - 0.5
+            h = xy[..., 1] * H - 0.5
+            dx = 2 * U24 * (xy[..., 0].abs() * W + 1)
+            dh = 2 * U24 * (xy[..., 1].abs() * H + 1)
+            valid = (h > -1) & (x > -1) & (h < H) & (x < W)
+            h_lo, x_lo = torch.floor(h), torch.floor(x)
+            lh, lw = h - h_lo, x - x_lo
+            hh, hw = 1 - lh, 1 - lw
+            h_lo, x_lo = h_lo.long(), x_lo.long()
+            corners = []
+            for dy, dxc in ((0, 0), (0, 1), (1, 0), (1, 1)):
+                hy, wx = h_lo + dy, x_lo + dxc
+                inside = valid & (hy >= 0) & (hy <= H - 1) & (wx >= 0) & (wx <= W - 1)
+                pix = starts[l] + hy.clamp(0, H - 1) * W + wx.clamp(0, W - 1)       # (B, nq, M, P)
+                row = (bi * Nv + pix) * M + mi                                    # row of value.view(B*Nv*M, C)
+                v = v64.view(B * Nv * M, C)[row] * inside[..., None]              # (B, nq, M, P, C), 0 outside
+                fy = (hh if dy == 0 else lh) * inside
+                fx = (hw if dxc == 0 else lw) * inside
+                corners.append((inside, row, v, fy, fx))
+            (_, _, v1, _, _), (_, _, v2, _, _), (_, _, v3, _, _), (_, _, v4, _, _) = corners
+            bil = sum(c[3][..., None] * c[4][..., None] * c[2] for c in corners)            # (B, nq, M, P, C)
+            babs = sum(c[3][..., None] * c[4][..., None] * c[2].abs() for c in corners)
+            a1, a2, a3, a4 = v1.abs(), v2.abs(), v3.abs(), v4.abs()
+            A = hw[..., None] * (a1 + a3) + lw[..., None] * (a2 + a4)           # >= |d bilinear / dh|
+            Bx = hh[..., None] * (a1 + a2) + lh[..., None] * (a3 + a4)           # >= |d bilinear / dx|
+            sens = dh[..., None] * A + dx[..., None] * Bx
+            res['out'][:, q0:q1] += (wl[..., None] * bil).sum(3)
+            res['out_abs'][:, q0:q1] += (wl.abs()[..., None] * babs).sum(3)
+            res['out_dl'][:, q0:q1] += (wl.abs()[..., None] * sens).sum(3)
+            if not bwd:
+                continue
+            ago = go.abs()
+            res['grad_attn'][:, q0:q1, :, l] = (go * bil).sum(-1)
+            res['ga_abs'][:, q0:q1, :, l] = (ago * babs).sum(-1)
+            res['ga_dl'][:, q0:q1, :, l] = (ago * sens).sum(-1)
+            t = go * wl[..., None]                                                 # (B, nq, M, P, C)
+            at = t.abs()
+            gx = (t * (hh[..., None] * (v2 - v1) + lh[..., None] * (v4 - v3))).sum(-1)
+            gy = (t * (hw[..., None] * (v3 - v1) + lw[..., None] * (v4 - v2))).sum(-1)
+            res['grad_loc'][:, q0:q1, :, l, :, 0] = W * gx
+            res['grad_loc'][:, q0:q1, :, l, :, 1] = H * gy
+            res['gl_abs'][:, q0:q1, :, l, :, 0] = W * (at * Bx).sum(-1)
+            res['gl_abs'][:, q0:q1, :, l, :, 1] = H * (at * A).sum(-1)
+            dsum = (at * (a1 + a2 + a3 + a4)).sum(-1)
+            res['gl_dl'][:, q0:q1, :, l, :, 0] = W * dh * dsum
+            res['gl_dl'][:, q0:q1, :, l, :, 1] = H * dx * dsum
+            for inside, row, _, fy, fx in corners:
+                r = row[inside]
+                cw = (fy * fx)[inside][:, None]
+                tt = t[inside]
+                res['grad_value'].index_add_(0, r, tt * cw)
+                res['gv_abs'].index_add_(0, r, tt.abs() * cw)
+                res['gv_count'].index_add_(0, r, torch.ones_like(tt))
+                res['gv_dl'].index_add_(0, r, tt.abs() * (dh[inside][:, None] * fx[inside][:, None] +
+                                                          dx[inside][:, None] * fy[inside][:, None]))
+    for k in ('out', 'out_abs', 'out_dl'):
+        res[k] = res[k].view(B, Nq, M * C)
+    if bwd:
+        for k in ('grad_value', 'gv_abs', 'gv_count', 'gv_dl'):
+            res[k] = res[k].view(B, Nv, M, C)
+    return res

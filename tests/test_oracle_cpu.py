@@ -537,3 +537,120 @@ def test_rotation_index_map_is_torchvisions_rotation(hw, center):
         assert torch.equal(got, want), ang
         if ang == 0.0:
             assert torch.equal(m, torch.arange(h * w))
+
+
+# ------------------------------------------------------------------------------------------ fp64 operator reference
+def _msda_case(levels, B=2, M=3, C=5, Nq=11, P=3, seed=0, margin=0.02, dtype=torch.float64):
+    """random operands with every sample at least `margin` pixels from a pixel line, from -1 and from H / W"""
+    g = torch.Generator().manual_seed(seed)
+    shapes = torch.tensor(levels)
+    lsi = torch.cat((shapes.new_zeros((1,)), shapes.prod(1).cumsum(0)[:-1]))
+    Nv = int(shapes.prod(1).sum())
+    L = len(levels)
+    value = torch.randn(B, Nv, M, C, generator=g, dtype=dtype)
+    size = shapes.flip(1).to(dtype)[None, None, None, :, None, :]                       # (W, H) per level
+    pix = torch.floor(torch.rand(B, Nq, M, L, P, 2, generator=g, dtype=dtype) * (size + 3)) - 2   # cells -2 .. size
+    frac = margin + (1 - 2 * margin) * torch.rand(B, Nq, M, L, P, 2, generator=g, dtype=dtype)
+    loc = (pix + frac + 0.5) / size
+    w = torch.rand(B, Nq, M, L, P, generator=g, dtype=dtype) * 2 - 1
+    go = torch.randn(B, Nq, M * C, generator=g, dtype=dtype)
+    return value, shapes, lsi, loc, w, go
+
+
+def test_msda_reference_forward_matches_the_kernel_loops():
+    value, shapes, lsi, loc, w, _ = _msda_case([(7, 9), (4, 5), (1, 3), (2, 1)], dtype=torch.float32)
+    ref = OM.msda_reference(value, shapes, lsi, loc, w)
+    loops = OM.msda_loops(value, shapes, lsi, loc, w)
+    np.testing.assert_allclose(ref['out'].numpy(), loops.numpy(), atol=2e-6, rtol=0)
+    assert bool((ref['out'].abs() <= ref['out_abs'] * (1 + 1e-12)).all())
+
+
+def test_msda_reference_matches_autograd_and_finite_differences_away_from_pixel_lines():
+    """float64 autograd through the grid_sample restatement (mmcv's CPU path) gives the same output and gradients; central
+    differences of <out, go> in loc give the same grad_loc"""
+    value, shapes, lsi, loc, w, go = _msda_case([(6, 8), (3, 5), (1, 4)])
+    ref = OM.msda_reference(value, shapes, lsi, loc, w, go)
+    v_, l_, w_ = (t.clone().requires_grad_(True) for t in (value, loc, w))
+    out = OM.msda_grid_sample(v_, shapes, l_, w_)
+    out.backward(go)
+    tol = dict(atol=1e-12, rtol=1e-12)
+    torch.testing.assert_close(ref['out'], out.detach(), **tol)
+    torch.testing.assert_close(ref['grad_value'], v_.grad, **tol)
+    torch.testing.assert_close(ref['grad_attn'], w_.grad, **tol)
+    torch.testing.assert_close(ref['grad_loc'], l_.grad, **tol)
+    eps = 1e-7
+    flat = loc.reshape(-1)
+    idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(1))[:64]
+    for i in idx.tolist():
+        lp, lm = flat.clone(), flat.clone()
+        lp[i] += eps
+        lm[i] -= eps
+        fp = (OM.msda_reference(value, shapes, lsi, lp.view(loc.shape), w)['out'] * go).sum()
+        fm = (OM.msda_reference(value, shapes, lsi, lm.view(loc.shape), w)['out'] * go).sum()
+        fd = ((fp - fm) / (2 * eps)).item()
+        assert abs(fd - ref['grad_loc'].reshape(-1)[i].item()) <= 1e-6 * (1 + abs(fd)), i
+
+
+def _edge_case(hy, wx, H=4, W=8, C=6, seed=0):
+    """one sample per head at pixel coordinates (hy, wx) on one H x W level (power-of-two sizes: exact coordinates)"""
+    g = torch.Generator().manual_seed(seed)
+    value = torch.randn(1, H * W, 1, C, generator=g, dtype=torch.float64)
+    shapes, lsi = torch.tensor([[H, W]]), torch.tensor([0])
+    loc = torch.tensor([(wx + 0.5) / W, (hy + 0.5) / H], dtype=torch.float64).view(1, 1, 1, 1, 1, 2)
+    w = torch.tensor([0.75], dtype=torch.float64).view(1, 1, 1, 1, 1)
+    go = torch.randn(1, 1, C, generator=g, dtype=torch.float64)
+    ref = OM.msda_reference(value, shapes, lsi, loc, w, go)
+    v_, l_, w_ = (t.clone().requires_grad_(True) for t in (value, loc, w))
+    out = OM.msda_grid_sample(v_, shapes, l_, w_)
+    out.backward(go)
+    return ref, out.detach(), v_.grad, l_.grad, w_.grad
+
+
+@pytest.mark.parametrize('hy,wx', [(0, 2.25), (3, 2.25), (4, 2.25), (1.5, 0), (1.5, 7), (1.5, 8), (0, 0), (3, 7)])
+def test_msda_reference_agrees_with_grid_sample_on_the_map_edges(hy, wx):
+    """h (or x) = 0, size - 1 and size: the floor cell of both rules is the same, so output and every gradient agree"""
+    ref, out, gv, gl, gw = _edge_case(hy, wx)
+    tol = dict(atol=1e-12, rtol=1e-12)
+    torch.testing.assert_close(ref['out'], out, **tol)
+    torch.testing.assert_close(ref['grad_value'], gv, **tol)
+    torch.testing.assert_close(ref['grad_loc'], gl, **tol)
+    torch.testing.assert_close(ref['grad_attn'], gw, **tol)
+
+
+@pytest.mark.parametrize('hy,wx,axis', [(-1, 2.25, 1), (1.5, -1, 0)])
+def test_msda_reference_differs_from_grid_sample_at_minus_one(hy, wx, axis):
+    """mmcv's rule: a sample is skipped unless -1 < h and -1 < x, so at exactly -1 its output and all its gradients are 0.
+    grid_sample's output there is 0 as well (the only corner inside has weight 0), but its autograd returns the one-sided
+    derivative into the map, d out / d loc = size * w * <go, v(row or column 0)> != 0.  The reference states mmcv's rule, the
+    kernels' rule."""
+    ref, out, gv, gl, gw = _edge_case(hy, wx)
+    assert float(ref['out'].abs().max()) == 0.0 and float(out.abs().max()) == 0.0
+    for k in ('grad_value', 'grad_loc', 'grad_attn'):
+        assert float(ref[k].abs().max()) == 0.0, k
+    assert float(gv.abs().max()) == 0.0 and float(gw.abs().max()) == 0.0
+    assert abs(float(gl[..., axis])) > 0.1, gl                       # grid_sample: a non-zero one-sided derivative
+    assert float(gl[..., 1 - axis]) == 0.0
+
+
+def test_msda_reference_reads_levels_through_level_start_index():
+    """levels placed with NaN gap rows between and after them give the result of the packed value"""
+    levels = [(3, 4), (1, 5), (2, 2)]
+    value, shapes, lsi, loc, w, go = _msda_case(levels, Nq=9)
+    gaps = [2, 5, 1]
+    starts, rows, pos = [], [], 0
+    for (h, w_), gap, s in zip(levels, gaps, lsi.tolist()):
+        pos += gap
+        starts.append(pos)
+        rows.append((pos, s, h * w_))
+        pos += h * w_
+    big = torch.full((value.shape[0], pos + 3, *value.shape[2:]), float('nan'), dtype=value.dtype)
+    for dst, src, n in rows:
+        big[:, dst:dst + n] = value[:, src:src + n]
+    a = OM.msda_reference(value, shapes, lsi, loc, w, go)
+    b = OM.msda_reference(big, shapes, torch.tensor(starts), loc, w, go)
+    for k in ('out', 'grad_loc', 'grad_attn'):
+        assert torch.equal(a[k], b[k]), k
+    for dst, src, n in rows:
+        assert torch.equal(b['grad_value'][:, dst:dst + n], a['grad_value'][:, src:src + n])
+        assert torch.equal(b['gv_count'][:, dst:dst + n], a['gv_count'][:, src:src + n])
+    assert float(b['gv_count'].sum()) == float(a['gv_count'].sum())
