@@ -281,12 +281,15 @@ int occb200_engine_profile(occb200_engine* e, int enable);
 int occb200_engine_profile_read(occb200_engine* e, float* ms_per_category, int* launches_per_category, int n);
 
 /* ---------------------------------------------------------------------------------------------
- * [R3] dvr.render_forward (phase "test").  sigma dev f32 [N,T,Z,Y,X]; origin dev f32 [N,T,3];
- * points dev f32 [N,M,3]; tindex dev f32 [N,M]; outputs dev f32 pred_dist [N,M], gt_dist [N,M],
- * coord_index [N,M,3] (all written, including the -1 / 0 defaults).
+ * [R3] dvr.render_forward (phase "test").  sigma dev f32 [N,T,Z,Y,X]; origin dev f32 [N,To,3];
+ * points dev f32 [N,M,K], K >= 3 (columns 0..2 are the end point); tindex dev f32 [N,M]; outputs dev f32
+ * pred_dist [N,M], gt_dist [N,M], coord_index [N,M,3] (all written, including the -1 / 0 defaults).
+ * Ray (n, m) with t = (int)tindex[n][m] >= 0 starts at origin[n][t] and walks sigma[n][T == 1 ? 0 : t], as in the
+ * reference; t is checked against neither T nor To (the caller keeps it below both, or below To when T == 1).
+ * A NULL pointer, N outside 0..65535, M < 0, T, To, Z, Y or X < 1, or K < 3 returns 1 before any CUDA call.
  */
 int occb200_render_forward(const float* sigma, const float* origin, const float* points, const float* tindex,
-                           int N, int T, int Z, int Y, int X, int64_t M, float* pred_dist, float* gt_dist,
+                           int N, int T, int To, int Z, int Y, int X, int64_t M, int K, float* pred_dist, float* gt_dist,
                            float* coord_index, void* stream);
 
 /* [R4] One frame of the Ray-mIoU / mAVE metric on a 200x200x16 grid (0.4 m voxels, range [-40,-40,-1]).

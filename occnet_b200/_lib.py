@@ -59,7 +59,7 @@ SIGNATURES = {
     'occb200_engine_launches_per_frame': (_i, [_vp]),
     'occb200_engine_profile': (_i, [_vp, _i]),
     'occb200_engine_profile_read': (_i, [_vp, _vp, _vp, _i]),
-    'occb200_render_forward': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i64, _vp, _vp, _vp, _vp]),
+    'occb200_render_forward': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i64, _i, _vp, _vp, _vp, _vp]),
     'occb200_ray_metric_accumulate': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp]),
     'occb200_linear_f32': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     'occb200_layernorm_f32': (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp]),

@@ -1791,11 +1791,14 @@ int occb200_engine_profile_read(occb200_engine* e, float* ms_per_category, int* 
 }
 
 int occb200_render_forward(const float* sigma, const float* origin, const float* points, const float* tindex, int N,
-                           int T, int Z, int Y, int X, int64_t M, float* pred_dist, float* gt_dist, float* coord_index,
-                           void* stream)
+                           int T, int To, int Z, int Y, int X, int64_t M, int K, float* pred_dist, float* gt_dist,
+                           float* coord_index, void* stream)
 {
     OCC_CHECK(sigma && origin && points && tindex && pred_dist && gt_dist && coord_index, "null pointer");
-    return launch_render_forward(sigma, origin, points, tindex, N, T, Z, Y, X, M, pred_dist, gt_dist, coord_index,
+    OCC_CHECK(N >= 0 && N <= 65535 && M >= 0, "render_forward: N must be in 0..65535 and M >= 0");
+    OCC_CHECK(T >= 1 && To >= 1 && Z >= 1 && Y >= 1 && X >= 1, "render_forward: T, To, Z, Y and X must be positive");
+    OCC_CHECK(K >= 3, "render_forward: points need K >= 3 columns");
+    return launch_render_forward(sigma, origin, points, tindex, N, T, To, Z, Y, X, M, K, pred_dist, gt_dist, coord_index,
                                  (cudaStream_t)stream);
 }
 

@@ -121,7 +121,7 @@ int launch_occ_head(const T* vox, HeadWeights hw, int64_t nvox, float* occ_logit
 // ---- raycast.cu
 // rows a14/a15: DDA first-hit for T origins x M rays through pred and gt volumes + the 187 counters
 int launch_render_forward(const float* sigma, const float* origin, const float* points, const float* tindex,
-                          int N, int T, int Z, int Y, int X, int64_t M, float* pred_dist, float* gt_dist,
+                          int N, int T, int To, int Z, int Y, int X, int64_t M, int K, float* pred_dist, float* gt_dist,
                           float* coord_index, cudaStream_t stream);
 int launch_ray_metric(const uint8_t* sem_pred, const float* flow_pred, const uint8_t* sem_gt, const float* flow_gt,
                       const void* origins, int origin_is_f64, int T, const float* rays, int M, double* counters,

@@ -67,9 +67,11 @@ __device__ __forceinline__ Hit dda_first_hit(double xo, double yo, double zo, do
     return h;
 }
 
+// sigma [N,T,Z,Y,X], origin [N,To,3], points [N,M,K] (K >= 3; columns 0..2 are read), tindex [N,M].  As in the reference,
+// sigma's T only picks the volume (ts), origin is indexed through its own To, and t is checked against neither.
 __global__ void render_forward_kernel(const float* __restrict__ sigma, const float* __restrict__ origin,
-                                      const float* __restrict__ points, const float* __restrict__ tindex, int T,
-                                      int vzsize, int vysize, int vxsize, int64_t M, float* __restrict__ pred_dist,
+                                      const float* __restrict__ points, const float* __restrict__ tindex, int T, int To,
+                                      int vzsize, int vysize, int vxsize, int64_t M, int K, float* __restrict__ pred_dist,
                                       float* __restrict__ gt_dist, float* __restrict__ coord_index)
 {
     const int n = blockIdx.y;
@@ -82,8 +84,8 @@ __global__ void render_forward_kernel(const float* __restrict__ sigma, const flo
     if (tf < 0) return;
     const int t = (int)tf;
     const int ts = (T == 1) ? 0 : t;
-    const float* o = origin + ((int64_t)n * T + t) * 3;
-    const float* p = points + rc * 3;
+    const float* o = origin + ((int64_t)n * To + t) * 3;
+    const float* p = points + rc * K;
     const float* sg = sigma + ((int64_t)n * T + ts) * vzsize * vysize * vxsize;
     double gt_d;
     const Hit h = dda_first_hit(o[0], o[1], o[2], p[0], p[1], p[2], vxsize, vysize, vzsize, gt_d,
@@ -260,12 +262,12 @@ ray_records_kernel(const uint8_t* __restrict__ sem, const float* __restrict__ fl
 }  // namespace
 
 int launch_render_forward(const float* sigma, const float* origin, const float* points, const float* tindex,
-                          int N, int T, int Z, int Y, int X, int64_t M, float* pred_dist, float* gt_dist,
+                          int N, int T, int To, int Z, int Y, int X, int64_t M, int K, float* pred_dist, float* gt_dist,
                           float* coord_index, cudaStream_t stream)
 {
     if (N == 0 || M == 0) return 0;
     dim3 grid(ceil_div(M, 128), N);
-    render_forward_kernel<<<grid, 128, 0, stream>>>(sigma, origin, points, tindex, T, Z, Y, X, M, pred_dist, gt_dist,
+    render_forward_kernel<<<grid, 128, 0, stream>>>(sigma, origin, points, tindex, T, To, Z, Y, X, M, K, pred_dist, gt_dist,
                                                     coord_index);
     OCC_CUDA(cudaGetLastError());
     return 0;

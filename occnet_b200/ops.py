@@ -28,10 +28,10 @@ def _require(t, name, dtype=None):
         raise RuntimeError(f'{name} must be {dtype}, got {t.dtype}')
 
 
-def _same_device(ref, *tensors):
+def _same_device(ref, *tensors, ref_name='value'):
     for t, name in tensors:
         if t.device != ref.device:
-            raise RuntimeError(f'{name} is on {t.device}, value on {ref.device}: all tensors must be on one device')
+            raise RuntimeError(f'{name} is on {t.device}, {ref_name} on {ref.device}: all tensors must be on one device')
 
 
 def _check_shape(t, name, shape):
@@ -138,22 +138,36 @@ MultiScaleDeformableAttnFunction_fp16 = MultiScaleDeformableAttnFunction_fp32   
 
 
 def render_forward(sigma, origin, points, tindex, grid, phase='test'):
-    """dvr.render_forward drop-in: -> [pred_dist (N,M), gt_dist (N,M), coord_index (N,M,3)] fp32 CUDA tensors."""
+    """dvr.render_forward drop-in: sigma [N,T,Z,Y,X] with grid == [T,Z,Y,X], origin [N,To,3], points [N,M,K] (K >= 3,
+    columns 0..2 are the end point), tindex [N,M] -> [pred_dist (N,M), gt_dist (N,M), coord_index (N,M,3)] fp32 CUDA
+    tensors.  Ray (n, m) starts at origin[n][t] and walks sigma[n][T == 1 ? 0 : t], t = int(tindex[n][m]); a negative
+    tindex is a padded point.  Every shape and device is checked before the kernel runs; the contents of tindex are not
+    (as in the reference, whose kernel device-asserts t < T when T > 1): keep t below To, and below T when T > 1."""
     for t, n in ((sigma, 'sigma'), (origin, 'origin'), (points, 'points'), (tindex, 'tindex')):
         _require(t, n, torch.float32)
     if phase != 'test':
         raise RuntimeError(f'UNKNOWN / unsupported PHASE NAME: {phase} (only "test" is on the metric path)')
-    N, M = points.shape[0], points.shape[1]
+    if len(grid) != 4:
+        raise RuntimeError(f'grid must be [T, Z, Y, X], got {list(grid)}')
     T, Z, Y, X = [int(g) for g in grid]
-    assert tuple(sigma.shape) == (N, T, Z, Y, X), (sigma.shape, grid)
+    if points.dim() != 3 or points.shape[2] < 3:
+        raise RuntimeError(f'points must be [N, M, K] with K >= 3, got shape {tuple(points.shape)}')
+    N, M, K = points.shape
+    _check_shape(sigma, 'sigma', (N, T, Z, Y, X))
+    if origin.dim() != 3 or origin.shape[0] != N or origin.shape[1] < 1 or origin.shape[2] != 3:
+        raise RuntimeError(f'origin must be [{N}, To, 3] with To >= 1, got shape {tuple(origin.shape)}')
+    _check_shape(tindex, 'tindex', (N, M))
+    if min(T, Z, Y, X) < 1:
+        raise RuntimeError(f'grid sizes must be positive, got {list(grid)}')
+    _same_device(sigma, (origin, 'origin'), (points, 'points'), (tindex, 'tindex'), ref_name='sigma')
     pred = torch.empty((N, M), dtype=torch.float32, device=sigma.device)
     gt = torch.empty_like(pred)
     coord = torch.empty((N, M, 3), dtype=torch.float32, device=sigma.device)
     lib = _lib.load()
     with torch.cuda.device(sigma.device):
         _lib.check(lib.occb200_render_forward(_lib.ptr(sigma), _lib.ptr(origin), _lib.ptr(points), _lib.ptr(tindex),
-                                              N, T, Z, Y, X, M, _lib.ptr(pred), _lib.ptr(gt), _lib.ptr(coord),
-                                              _lib.stream_ptr()))
+                                              N, T, origin.shape[1], Z, Y, X, M, K, _lib.ptr(pred), _lib.ptr(gt),
+                                              _lib.ptr(coord), _lib.stream_ptr()))
     torch.cuda.current_stream().synchronize()      # the reference op returns after cudaDeviceSynchronize (dvr.cu:384)
     return [pred, gt, coord]
 

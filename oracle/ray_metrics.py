@@ -43,24 +43,36 @@ def _lib():
     if _LIB is None:
         _LIB = ctypes.CDLL(build_dda())
         f32p = ctypes.POINTER(ctypes.c_float)
-        _LIB.oracle_render_forward.argtypes = [f32p, f32p, f32p, f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                               ctypes.c_int, ctypes.c_int64, f32p, f32p, f32p]
+        i = ctypes.c_int
+        _LIB.oracle_render_forward.argtypes = [f32p, f32p, f32p, f32p, i, i, i, i, i, i, ctypes.c_int64, i, f32p, f32p, f32p]
         _LIB.oracle_render_forward.restype = None
     return _LIB
 
 
 def render_forward(sigma, origin, points, tindex):
-    """sigma (T,Z,Y,X) f32; origin (T,3); points (M,3); tindex (M,) -> pred_dist (M,), gt_dist (M,), coord (M,3)."""
+    """dvr.render_forward(sigma, origin, points, tindex, grid, 'test') in double (oracle/ray_dda.c).
+
+    Batched, the reference's full argument meaning: sigma (N,T,Z,Y,X), origin (N,To,3), points (N,M,K) with K >= 3,
+    tindex (N,M) -> pred_dist (N,M), gt_dist (N,M), coord (N,M,3).  Unbatched (N = 1 dropped): sigma (T,Z,Y,X),
+    origin (To,3), points (M,K), tindex (M,) -> (M,), (M,), (M,3).  tindex must stay below To (and below T when T > 1):
+    like the reference, nothing here checks it."""
     sigma = np.ascontiguousarray(sigma, np.float32)
+    batched = sigma.ndim == 5
+    if not batched:
+        sigma, origin, points, tindex = sigma[None], np.asarray(origin)[None], np.asarray(points)[None], np.asarray(tindex)[None]
     origin = np.ascontiguousarray(origin, np.float32)
     points = np.ascontiguousarray(points, np.float32)
     tindex = np.ascontiguousarray(tindex, np.float32)
-    T, Z, Y, X = sigma.shape
-    M = points.shape[0]
-    pd = np.empty(M, np.float32); gd = np.empty(M, np.float32); ci = np.empty((M, 3), np.float32)
+    N, T, Z, Y, X = sigma.shape
+    _, M, K = points.shape
+    To = origin.shape[1]
+    assert origin.shape == (N, To, 3) and To >= 1 and K >= 3 and points.shape[0] == N and tindex.shape == (N, M)
+    ok = tindex[tindex >= 0].astype(np.int64)
+    assert (ok < To).all() and (T == 1 or (ok < T).all()), 'tindex points past origin or sigma'
+    pd = np.empty((N, M), np.float32); gd = np.empty((N, M), np.float32); ci = np.empty((N, M, 3), np.float32)
     p = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
-    _lib().oracle_render_forward(p(sigma), p(origin), p(points), p(tindex), T, Z, Y, X, M, p(pd), p(gd), p(ci))
-    return pd, gd, ci
+    _lib().oracle_render_forward(p(sigma), p(origin), p(points), p(tindex), N, T, To, Z, Y, X, M, K, p(pd), p(gd), p(ci))
+    return (pd, gd, ci) if batched else (pd[0], gd[0], ci[0])
 
 
 def generate_lidar_rays():
