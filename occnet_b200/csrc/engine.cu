@@ -1222,8 +1222,33 @@ int occb200_engine_create(const occb200_config* cfg, occb200_engine** out)
     OCC_CHECK(cfg->num_points_in_pillar >= 1 && cfg->num_points_in_pillar <= 8 && 8 % cfg->num_points_in_pillar == 0,
               "num_points_in_pillar must be 1, 2, 4 or 8");
     OCC_CHECK(cfg->pillar_h == 16 && cfg->out_dim == 32, "only pillar_h=16, out_dim=32 are supported");
-    OCC_CHECK(cfg->ffn_dim % 64 == 0 && cfg->num_classes <= 32 && cfg->num_layers >= 1, "bad ffn_dim/num_classes");
+    OCC_CHECK(cfg->ffn_dim > 0 && cfg->ffn_dim % 64 == 0,
+              "ffn_dim must be a positive multiple of 64, got " + std::to_string(cfg->ffn_dim));
+    OCC_CHECK(cfg->num_classes >= 1 && cfg->num_classes <= 32,
+              "num_classes must be in [1,32], got " + std::to_string(cfg->num_classes));
+    OCC_CHECK(cfg->num_layers >= 1, "num_layers must be >= 1, got " + std::to_string(cfg->num_layers));
     OCC_CHECK(cfg->precision == 0 || cfg->precision == 1, "precision must be 0 (fp32) or 1 (bf16)");
+    // the TSA gather samples a 2x2 neighbourhood of the BEV grid, the SCA gather one of every level
+    OCC_CHECK(cfg->bev_h >= 2 && cfg->bev_w >= 2, "bev_h and bev_w must be >= 2, got " + std::to_string(cfg->bev_h) + "x" +
+                                                      std::to_string(cfg->bev_w));
+    int64_t nv = 0;
+    for (int l = 0; l < 4; ++l) {
+        OCC_CHECK(cfg->level_h[l] >= 2 && cfg->level_w[l] >= 2,
+                  "level_h / level_w of level " + std::to_string(l) + " must be >= 2, got " + std::to_string(cfg->level_h[l]) +
+                      "x" + std::to_string(cfg->level_w[l]));
+        nv += (int64_t)cfg->level_h[l] * cfg->level_w[l];
+    }
+    for (int i = 0; i < 3; ++i)
+        OCC_CHECK(std::isfinite(cfg->pc_range[i]) && std::isfinite(cfg->pc_range[3 + i]) && cfg->pc_range[3 + i] > cfg->pc_range[i],
+                  "pc_range must be finite with max > min on every axis (axis " + std::to_string(i) + ")");
+    // Every frame buffer's element count must fit an int: the launchers take row counts as int (gemm M = num_cams * Nv for
+    // the SCA value map, layernorm rows = Nq), and bev_to_voxel / layernorm256 / the pack kernel form their row and pixel
+    // indices in int before widening them; bounding the elements also bounds those rows and pixels.
+    const int64_t kIntMax = 2147483647;
+    OCC_CHECK((int64_t)cfg->bev_h * cfg->bev_w * 256 <= kIntMax, "bev_h * bev_w * 256 must be <= 2^31 - 1");
+    OCC_CHECK(cfg->num_cams * nv * 256 <= kIntMax, "num_cams * (sum of level h * w) * 256 must be <= 2^31 - 1");
+    OCC_CHECK((int64_t)cfg->bev_h * cfg->bev_w * cfg->pillar_h * cfg->out_dim <= kIntMax,
+              "bev_h * bev_w * pillar_h * out_dim must be <= 2^31 - 1");
     int dev_count = 0;
     if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count == 0) {
         set_last_error("no CUDA device: libocc_b200 has no CPU fallback");

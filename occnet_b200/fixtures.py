@@ -66,6 +66,45 @@ def camera_rig(num_cams=6, img_hw=(928, 1600)):
     return np.stack(out), ego2lidar
 
 
+IMG_RIG = (928, 1600)
+
+
+def _camera(yaw, f, t, img_hw):
+    """lidar2img of one camera built like fixtures.camera_rig"""
+    R0 = np.array([[0.0, 0.0, 1.0], [-1.0, 0.0, 0.0], [0.0, -1.0, 0.0]])
+    ego2lidar = np.linalg.inv(PSEUDO_LIDAR2EGO)
+    a = math.radians(yaw)
+    Rz = np.array([[math.cos(a), -math.sin(a), 0.0], [math.sin(a), math.cos(a), 0.0], [0.0, 0.0, 1.0]])
+    cam2ego = np.eye(4)
+    cam2ego[:3, :3] = Rz @ R0
+    cam2ego[:3, 3] = t
+    s2l = ego2lidar @ cam2ego
+    r = np.linalg.inv(s2l[:3, :3])
+    rt = np.eye(4)
+    rt[:3, :3] = r.T
+    rt[3, :3] = -(s2l[:3, 3] @ r.T)
+    sx, sy = img_hw[1] / 1600.0, img_hw[0] / 928.0
+    K = np.array([[f * sx, 0.0, 816.0 * sx], [0.0, f * sy, 491.0 * sy], [0.0, 0.0, 1.0]], dtype=np.float32)
+    vp = np.eye(4)
+    vp[:3, :3] = K
+    return vp @ rt.T
+
+
+# two extra cameras of the eight-camera rig: they overlap the front-left / rear-right cameras of the fixture rig
+EXTRA_CAMS = [(28.0, 1000.0, (1.6, 0.3, 1.6)), (-150.0, 900.0, (-0.4, -0.4, 1.4))]
+
+
+def rig_metas(num_cams, img_hw=IMG_RIG, can_bus_angle=None):
+    """img_metas of the first num_cams cameras of the fixture rig, extended by EXTRA_CAMS beyond six"""
+    l2i, e2l = camera_rig(min(num_cams, 6), img_hw)
+    mats = [l2i[i] for i in range(min(num_cams, 6))] + [_camera(*c, img_hw) for c in EXTRA_CAMS[:max(0, num_cams - 6)]]
+    m = dict(lidar2img=mats, ego2lidar=e2l, img_shape=[tuple(img_hw) + (3,)] * num_cams)
+    if can_bus_angle is not None:
+        m['can_bus'] = np.zeros(18)
+        m['can_bus'][-1] = can_bus_angle
+    return [m]
+
+
 def make_img_metas(cfg, bs=1, can_bus_angle=None):
     l2i, e2l = camera_rig(cfg['num_cams'], cfg['img_shape'][:2])
     metas = []
