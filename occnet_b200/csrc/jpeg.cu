@@ -7,16 +7,16 @@
 // buffer, guarded by an event.  The end of the segment is the EOI marker at the end of the file, so the host never scans it.
 //
 // Device, all images of a call in the same three launches:
-//   jpeg_entropy_kernel  one 1024-thread block per image: removes the FF00 stuffing and the RSTn markers (recording every
-//                        restart interval's start), cuts each interval into kSubBits-bit subsequences and decodes them with
-//                        self-synchronising Huffman decoding (Weissenberger & Schmidt, ICPP 2018): every subsequence decodes
-//                        from a guessed start state (bit position, block of the MCU, zig-zag index) to the first codeword
-//                        boundary at or past its end; then, until no start changes, each takes its predecessor's exit state as
-//                        its start and decodes again.  An interval's first subsequence starts from the true state, so at
-//                        convergence every start is a true codeword boundary (the worst case is serial decoding, never a
-//                        wrong one).  A scan of the per-subsequence block counts places every block; the coefficients go to
-//                        an int16 block array in decode order and the DC differences are summed by a segmented scan that
-//                        restarts at every interval.
+//   jpeg_entropy_kernel  one 1024-thread block per image: removes the FF00 stuffing, the RSTn markers (recording every restart
+//                        interval's start) and the FF fill bytes before RSTn and EOI, cuts each interval into kSubBits-bit
+//                        subsequences and decodes them with self-synchronising Huffman decoding (Weissenberger & Schmidt, ICPP
+//                        2018): every subsequence decodes from a guessed start state (bit position, block of the MCU, zig-zag
+//                        index) to the first codeword boundary at or past its end; then, until no start changes, each takes its
+//                        predecessor's exit state as its start and decodes again.  An interval's first subsequence starts from
+//                        the true state, so at convergence every start is a true codeword boundary (the worst case is serial
+//                        decoding, never a wrong one).  A scan of the per-subsequence block counts places every block; the
+//                        coefficients go to an int16 block array in decode order and the DC differences are summed by a
+//                        segmented scan that restarts at every interval.
 //   jpeg_idct_kernel     dequantisation + ISLOW IDCT (jidctint.c), 8 threads per block, into per-component sample planes.
 //   jpeg_color_kernel    h2v2 fancy upsampling (4:2:0) + YCbCr -> BGR, interleaved uint8 straight into the frame buffer.
 // Corrupt data (an invalid code, a run past coefficient 63, an interval that ends early or late, a marker inside the scan) never
@@ -382,6 +382,34 @@ __device__ int block_seg_scan(int f, int v, int* shf, int* shv, int& carry_f)
 
 __device__ __forceinline__ bool is_rst(uint8_t b) { return b >= 0xD0 && b <= 0xD7; }
 
+enum { kKeep, kRst, kDrop };
+
+// Calls f(kind, i) for every byte i in [b0, b1) of the entropy-coded segment in[0, n): kKeep for a data byte (the FF of FF00
+// included), kRst for the FF of an RSTn marker, kDrop for the 00 of FF00, an RSTn byte and a fill byte.  A marker may be
+// preceded by any number of FF fill bytes (T.81 B.1.1.2): a run of FF bytes that ends in an RSTn byte, or at the end of the
+// segment (the EOI marker follows), is fill plus that marker.  Any other FF not followed by 00, FF FF 00 included, sets `bad`.
+// A run that crosses the chunk is classified from its own bytes, so every thread gives the bytes of its chunk the same kind.
+template <class F>
+__device__ __forceinline__ void for_each_byte(const uint8_t* in, int n, int b0, int b1, int& bad, F f)
+{
+    for (int i = b0; i < b1;) {
+        if (in[i] != 0xFF) {
+            f(i > 0 && in[i - 1] == 0xFF ? kDrop : kKeep, i);
+            ++i;
+            continue;
+        }
+        int k = i + 1;                                               // the run of FF bytes containing i ends at k - 1
+        while (k < n && in[k] == 0xFF) ++k;
+        const bool single = k - 1 == 0 || in[k - 2] != 0xFF;
+        int last;                                                    // what the run's last FF is
+        if (k == n) last = kDrop;
+        else if (is_rst(in[k])) last = kRst;
+        else if (in[k] == 0 && single) last = kKeep;
+        else { bad = 1; last = kDrop; }
+        for (; i < min(k, b1); ++i) f(i == k - 1 ? last : kDrop, i);
+    }
+}
+
 __global__ void __launch_bounds__(kThreads, 1) jpeg_entropy_kernel(Bufs B)
 {
     const JpegImage& im = B.img[blockIdx.x];
@@ -405,40 +433,25 @@ __global__ void __launch_bounds__(kThreads, 1) jpeg_entropy_kernel(Bufs B)
     // zero the coefficients (the decoder writes the non-zero ones only)
     for (int64_t i = tid; i < nblocks * 8; i += kThreads) reinterpret_cast<int4*>(coef)[i] = make_int4(0, 0, 0, 0);
 
-    // ---- 1. unstuffing: each thread a contiguous chunk of bytes; byte i is kept unless it is the 00 of FF00 or part of a
-    // marker.  RSTn markers record the start of the next interval and must count 0..7 in order.
+    // ---- 1. unstuffing: each thread a contiguous chunk of bytes; byte i is kept unless it is the 00 of FF00, part of a
+    // marker or a fill byte.  RSTn markers record the start of the next interval and must count 0..7 in order.
     {
         const int chunk = (n + kThreads - 1) / kThreads;
         const int b0 = min(n, tid * chunk), b1 = min(n, b0 + chunk);
         int keep = 0, rst = 0, bad = 0;
-        for (int i = b0; i < b1; ++i) {
-            const uint8_t b = in[i];
-            const uint8_t prev = i > 0 ? in[i - 1] : 0;
-            if (b == 0xFF) {
-                if (i + 1 < n && in[i + 1] == 0) ++keep;
-                else if (i + 1 < n && is_rst(in[i + 1])) ++rst;
-                else bad = 1;
-            } else if (prev != 0xFF || i == 0) {
-                ++keep;
-            }
-        }
+        for_each_byte(in, n, b0, b1, bad, [&](int kind, int) { keep += kind == kKeep; rst += kind == kRst; });
         int tk, tr;
         int ok = block_scan(keep, sh, &tk);
         int orr = block_scan(rst, sh, &tr);
-        for (int i = b0; i < b1; ++i) {
-            const uint8_t b = in[i];
-            const uint8_t prev = i > 0 ? in[i - 1] : 0;
-            if (b == 0xFF) {
-                if (i + 1 < n && in[i + 1] == 0) us[ok++] = 0xFF;
-                else if (i + 1 < n && is_rst(in[i + 1])) {
-                    if (orr + 1 < n_iv) iv[orr + 1] = ok;
-                    if ((in[i + 1] & 7) != (orr & 7)) bad = 1;
-                    ++orr;
-                }
-            } else if (prev != 0xFF || i == 0) {
-                us[ok++] = b;
+        for_each_byte(in, n, b0, b1, bad, [&](int kind, int i) {
+            if (kind == kKeep) {
+                us[ok++] = in[i];
+            } else if (kind == kRst) {
+                if (orr + 1 < n_iv) iv[orr + 1] = ok;
+                if ((in[i + 1] & 7) != (orr & 7)) bad = 1;
+                ++orr;
             }
-        }
+        });
         if (bad) s_bad = 1;
         if (tid < kPad) us[tk + tid] = 0xFF;
         if (tid == 0) {

@@ -134,19 +134,26 @@ def parse(data):
 
 
 def unstuff(scan):
-    """entropy-coded segment -> (bytes without FF00 stuffing / RSTn markers, byte offset of every interval start)"""
-    out, starts, i = bytearray(), [0], 0
-    while i < len(scan):
+    """entropy-coded segment -> (bytes without FF00 stuffing / RSTn markers, byte offset of every interval start).
+    A marker may be preceded by any number of FF fill bytes (T.81 B.1.1.2): a run of FF bytes that ends in an RSTn byte, or
+    at the end of the segment (the EOI marker follows), is fill plus that marker.  Every other FF not followed by 00, and
+    FF FF 00 in particular, is corrupt (libjpeg-turbo's two bit readers disagree on what FF FF 00 means)."""
+    out, starts, i, n = bytearray(), [0], 0, len(scan)
+    while i < n:
         b = scan[i]
         if b == 0xFF:
-            nxt = scan[i + 1]
-            if nxt == 0:
-                out.append(0xFF)
-            elif 0xD0 <= nxt <= 0xD7:
+            k = i + 1
+            while k < n and scan[k] == 0xFF:
+                k += 1
+            if k == n:                                       # fill bytes before the EOI marker
+                break
+            if 0xD0 <= scan[k] <= 0xD7:
                 starts.append(len(out))
+            elif scan[k] == 0 and k == i + 1:
+                out.append(0xFF)
             else:
                 raise ValueError('marker inside the scan')
-            i += 2
+            i = k + 1
         else:
             out.append(b)
             i += 1
@@ -155,11 +162,14 @@ def unstuff(scan):
 
 class _Bits:
     def __init__(self, data):
-        self.v = int.from_bytes(data + b'\xff' * 8, 'big')
-        self.n = (len(data) + 8) * 8
+        self.d = bytes(data) + b'\xff' * 12
 
     def get(self, pos, k):
-        return (self.v >> (self.n - pos - k)) & ((1 << k) - 1) if k else 0
+        """k <= 16 bits from bit `pos` (the stream continues with 1-bits past its end)"""
+        if not k:
+            return 0
+        v = int.from_bytes(self.d[pos >> 3:(pos >> 3) + 4], 'big')
+        return (v >> (32 - (pos & 7) - k)) & ((1 << k) - 1)
 
 
 def _extend(v, s):
